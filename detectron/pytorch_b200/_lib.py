@@ -89,6 +89,17 @@ _SIGNATURES = {
     "b200_fast_rcnn_targets": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                               ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
                                               ctypes.c_void_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _stream_t]),
+    "b200_segm_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int]),
+    # (masks, mask_class, boxes, D, Kc, M, im_h, im_w, thresh, sizes_out, workspace, workspace_bytes, stream)
+    "b200_segm_rle_sizes": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, _c_float_p] + [ctypes.c_int] * 5 + [ctypes.c_float, ctypes.c_void_p,
+                                                                                                             ctypes.c_void_p, ctypes.c_size_t, _stream_t]),
+    # (masks, mask_class, boxes, D, Kc, M, im_h, im_w, thresh, sizes, workspace, workspace_bytes, counts, count_offs, strings, string_offs, stream)
+    "b200_segm_rle_emit": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, _c_float_p] + [ctypes.c_int] * 5 + [ctypes.c_float, ctypes.c_void_p,
+                                                                                                            ctypes.c_void_p, ctypes.c_size_t] +
+                           [ctypes.c_void_p] * 4 + [_stream_t]),
+    # (masks, mask_class, boxes, D, Kc, M, im_h, im_w, thresh, out, stream)
+    "b200_paste_masks": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, _c_float_p] + [ctypes.c_int] * 5 + [ctypes.c_float, ctypes.c_void_p,
+                                                                                                          _stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

@@ -14,6 +14,10 @@ Inputs and outputs are numpy arrays like the reference's; CUDA tensors are accep
 Flavour note (as for the proposal NMS): the device NMS keeps the reference CUDA kernel's `IoU > thresh` test, the Cython
 routine the reference calls here uses `>=`; they differ only on pairs whose IoU equals the threshold to the last bit.
 Soft-NMS follows lib/utils/cython_nms.pyx:98-203 step for step (same greedy order, same drop rule).
+
+`segm_results(cls_boxes, masks, ref_boxes, im_h, im_w)` is the Mask R-CNN step after it (lib/core/test.py:793-847): every
+detection's mask is pasted into the image and run-length encoded on the device in two launches per image, with one host
+read of the per-detection sizes; the result is the reference's list of COCO RLE dicts.
 """
 import numpy as np
 import torch
@@ -98,3 +102,59 @@ def box_results_with_nms_and_limit(scores, boxes, cfg=None, **kw):
                 cls_boxes[j] = cls_boxes[j][keep, :]
     im_results = np.vstack([cls_boxes[j] for j in range(1, K)]) if K > 1 else np.zeros((0, 5), np.float32)
     return im_results[:, -1], im_results[:, :-1], cls_boxes
+
+
+def _segm_params(cfg, kw):
+    if cfg is not None:
+        p = dict(num_classes=cfg.MODEL.NUM_CLASSES, resolution=cfg.MRCNN.RESOLUTION, cls_specific_mask=cfg.MRCNN.CLS_SPECIFIC_MASK,
+                 thresh_binarize=cfg.MRCNN.THRESH_BINARIZE)
+    else:
+        p = dict(num_classes=None, resolution=14, cls_specific_mask=True, thresh_binarize=0.5)       # lib/core/config.py:741-776
+    p.update(kw)
+    return p
+
+
+def segm_results(cls_boxes, masks, ref_boxes, im_h, im_w, cfg=None, **kw):
+    """cls_segms of lib/core/test.py:793-847: a list over classes of lists of COCO RLEs {'size': [im_h, im_w], 'counts': str},
+    one per row of cls_boxes[j] (j >= 1), in the reference's order.  The masks are pasted and run-length encoded on the device
+    (ops.segm_rle_raw: cv2's IPP-off resize arithmetic; pycocotools is not needed); the host only slices one string buffer.
+
+    masks: the mask head's output, a numpy array (R, Kc, M, M) like the reference's or a float32 CUDA tensor (R, Kc * M * M) /
+    (R, Kc, M, M), which skips the device-to-host copy; Kc is the number of classes for class-specific masks, else 1.
+    ref_boxes: (R, 4) detections, numpy or CUDA, in the class-major order of cls_boxes.  Configuration: the reference's
+    `cfg` (MODEL.NUM_CLASSES, MRCNN.RESOLUTION / CLS_SPECIFIC_MASK / THRESH_BINARIZE) or keyword arguments num_classes,
+    resolution, cls_specific_mask, thresh_binarize."""
+    p = _segm_params(cfg, kw)
+    K = int(p["num_classes"] or len(cls_boxes))
+    M = int(p["resolution"])
+    im_h, im_w = int(im_h), int(im_w)
+    n_per_class = [len(cls_boxes[j]) for j in range(1, K)]
+    D = sum(n_per_class)
+    if int(masks.shape[0]) != D:
+        raise ValueError("segm_results: %d masks for %d detections" % (int(masks.shape[0]), D))
+    cls_segms = [[] for _ in range(K)]
+    if D == 0:
+        return cls_segms
+    dev = masks.device if torch.is_tensor(masks) and masks.is_cuda else torch.device("cuda", torch.cuda.current_device())
+    mk = masks if torch.is_tensor(masks) else torch.from_numpy(np.ascontiguousarray(masks, dtype=np.float32))
+    mk = mk.to(dev, dtype=torch.float32).reshape(D, -1, M, M)
+    bx = ref_boxes if torch.is_tensor(ref_boxes) else torch.from_numpy(np.ascontiguousarray(ref_boxes, dtype=np.float32))
+    bx = bx.to(dev, dtype=torch.float32)[:, :4]
+    cls_of = np.repeat(np.arange(1, K, dtype=np.int32), n_per_class)
+    if p["cls_specific_mask"]:
+        if mk.size(1) < K:
+            raise ValueError("segm_results: class-specific masks need %d channels, got %d" % (K, mk.size(1)))
+        mask_class = torch.from_numpy(cls_of).to(dev)
+    else:
+        mask_class = torch.zeros((D,), dtype=torch.int32, device=dev)
+    _, _, strings, string_offs = ops.segm_rle_raw(mk, mask_class, bx, im_h, im_w, float(p["thresh_binarize"]))
+    buf = strings.cpu().numpy().tobytes()
+    offs = string_offs.cpu().numpy()
+    d = 0
+    for j in range(1, K):
+        segms = []
+        for _ in range(n_per_class[j - 1]):
+            segms.append({"size": [im_h, im_w], "counts": buf[offs[d]:offs[d + 1]].decode("ascii")})
+            d += 1
+        cls_segms[j] = segms
+    return cls_segms

@@ -72,6 +72,12 @@ int roi_assign(const float*, int, const float*, const int*, int, float*, int*, i
 int roi_select(const float*, int, float, float, float, int*, int*, int*, cudaStream_t);
 int fast_rcnn_targets(const float*, const float*, const int*, const int*, const int*, int, int, const float*, int, int, float, float, int*,
                       float*, float*, float*, float*, cudaStream_t);
+size_t segm_workspace_bytes(int);
+bool segm_args_ok(int, int, int, int, int);
+int segm_rle_sizes(const float*, const int*, const float*, int, int, int, int, int, float, int*, void*, cudaStream_t);
+int segm_rle_emit(const float*, const int*, const float*, int, int, int, int, int, float, const int*, const void*, int*, long long*,
+                  unsigned char*, long long*, cudaStream_t);
+int paste_masks(const float*, const int*, const float*, int, int, int, int, int, float, unsigned char*, cudaStream_t);
 
 // B200_ROI_ALIGN_PATH=generic|tiled|stream|auto (default auto) -- test/benchmark override of the forward dispatch
 //   0 auto: streaming-strip path -> quad-strip path -> tiled path -> generic, each when it applies.  On H100 the streaming
@@ -556,6 +562,42 @@ int b200_fast_rcnn_targets(const float* boxes_dev, const float* gt_boxes_dev, co
     return fast_rcnn_targets(boxes_dev, gt_boxes_dev, argmax_dev, max_classes_dev, keep_inds_dev, num_keep, num_fg, bbox_reg_weights_host,
                              num_reg_classes, cls_agnostic, im_scale, batch_idx, labels_out_dev, rois_out_dev, bbox_targets_out_dev,
                              inside_weights_out_dev, outside_weights_out_dev, (cudaStream_t)stream);
+}
+
+size_t b200_segm_workspace_bytes(int num_dets) { return segm_workspace_bytes(num_dets); }
+
+int b200_segm_rle_sizes(const float* masks_dev, const int* mask_class_dev, const float* boxes_dev, int num_dets, int num_channels,
+                        int resolution, int im_h, int im_w, float thresh, int* sizes_out_dev, void* workspace, size_t workspace_bytes,
+                        b200_stream_t stream) {
+    if (!segm_args_ok(num_dets, num_channels, resolution, im_h, im_w)) return B200_ROI_EINVAL;
+    if (num_dets == 0) return B200_ROI_OK;
+    if (!masks_dev || !mask_class_dev || !boxes_dev || !sizes_out_dev) return B200_ROI_EINVAL;
+    if (!workspace || workspace_bytes < segm_workspace_bytes(num_dets)) return B200_ROI_EWORKSPACE;
+    return segm_rle_sizes(masks_dev, mask_class_dev, boxes_dev, num_dets, num_channels, resolution, im_h, im_w, thresh, sizes_out_dev,
+                          workspace, (cudaStream_t)stream);
+}
+
+int b200_segm_rle_emit(const float* masks_dev, const int* mask_class_dev, const float* boxes_dev, int num_dets, int num_channels,
+                       int resolution, int im_h, int im_w, float thresh, const int* sizes_dev, const void* workspace,
+                       size_t workspace_bytes, int* counts_out_dev, long long* count_offsets_out_dev, unsigned char* strings_out_dev,
+                       long long* string_offsets_out_dev, b200_stream_t stream) {
+    if (!segm_args_ok(num_dets, num_channels, resolution, im_h, im_w)) return B200_ROI_EINVAL;
+    if (num_dets == 0) return B200_ROI_OK;
+    if (!masks_dev || !mask_class_dev || !boxes_dev || !sizes_dev || !counts_out_dev || !count_offsets_out_dev || !strings_out_dev ||
+        !string_offsets_out_dev)
+        return B200_ROI_EINVAL;
+    if (!workspace || workspace_bytes < segm_workspace_bytes(num_dets)) return B200_ROI_EWORKSPACE;
+    return segm_rle_emit(masks_dev, mask_class_dev, boxes_dev, num_dets, num_channels, resolution, im_h, im_w, thresh, sizes_dev,
+                         workspace, counts_out_dev, count_offsets_out_dev, strings_out_dev, string_offsets_out_dev, (cudaStream_t)stream);
+}
+
+int b200_paste_masks(const float* masks_dev, const int* mask_class_dev, const float* boxes_dev, int num_dets, int num_channels,
+                     int resolution, int im_h, int im_w, float thresh, unsigned char* out_dev, b200_stream_t stream) {
+    if (!segm_args_ok(num_dets, num_channels, resolution, im_h, im_w) || num_dets > 65535) return B200_ROI_EINVAL;
+    if (num_dets == 0) return B200_ROI_OK;
+    if (!masks_dev || !mask_class_dev || !boxes_dev || !out_dev) return B200_ROI_EINVAL;
+    return paste_masks(masks_dev, mask_class_dev, boxes_dev, num_dets, num_channels, resolution, im_h, im_w, thresh, out_dev,
+                       (cudaStream_t)stream);
 }
 
 }  // extern "C"

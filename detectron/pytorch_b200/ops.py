@@ -505,3 +505,61 @@ def nms_raw(dets, thresh):
                                 ws.data_ptr(), ws_bytes, _stream()),
                    "b200_nms")
     return keep, num_out
+
+
+# ------------------------------------------------------------------------------------------------
+# Test-time mask paste + COCO RLE (SURVEY.md 8f N3, lib/core/test.py:793-847)
+# ------------------------------------------------------------------------------------------------
+def _segm_inputs(masks, mask_class, boxes, im_h, im_w):
+    _need_cuda_f32(masks, "masks"); _need_cuda_f32(boxes, "boxes")
+    if masks.dim() != 4 or masks.size(2) != masks.size(3):
+        raise ValueError("masks must be (D, Kc, M, M), got %s" % (tuple(masks.shape),))
+    D = masks.size(0)
+    if boxes.dim() != 2 or boxes.size(0) != D or boxes.size(1) != 4:
+        raise ValueError("boxes must be (D, 4) = [x1, y1, x2, y2] with D = %d, got %s" % (D, tuple(boxes.shape)))
+    if not torch.is_tensor(mask_class) or mask_class.dim() != 1 or mask_class.numel() != D:
+        raise ValueError("mask_class must be a (D,) tensor with D = %d" % D)
+    if int(im_h) <= 0 or int(im_w) <= 0:
+        raise ValueError("image size must be positive, got %s x %s" % (im_h, im_w))
+    mask_class = mask_class.to(device=masks.device, dtype=torch.int32).contiguous()
+    return masks.contiguous(), mask_class, boxes.to(masks.device).contiguous(), D, masks.size(1), masks.size(2)
+
+
+def segm_rle_raw(masks, mask_class, boxes, im_h, im_w, thresh):
+    """COCO RLEs of the pasted masks of one image (lib/core/test.py:793-847 per detection, cv2 IPP-off arithmetic).
+    masks: float32 CUDA (D, Kc, M, M); mask_class: (D,) channel per detection; boxes: float32 CUDA (D, 4), not expanded.
+    Returns device tensors (counts int32, count_offsets int64 (D + 1,), strings uint8, string_offsets int64 (D + 1,)):
+    detection d's column-major run lengths are counts[count_offsets[d]:count_offsets[d + 1]], its compressed COCO string
+    strings[string_offsets[d]:string_offsets[d + 1]].  Two launches and one host read of the per-detection sizes."""
+    masks, mask_class, boxes, D, Kc, M = _segm_inputs(masks, mask_class, boxes, im_h, im_w)
+    dev = masks.device
+    if D == 0:
+        z = torch.zeros((1,), dtype=torch.int64, device=dev)
+        return torch.empty((0,), dtype=torch.int32, device=dev), z, torch.empty((0,), dtype=torch.uint8, device=dev), z.clone()
+    lib = _lib.load()
+    ws_bytes = int(lib.b200_segm_workspace_bytes(D))
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    sizes = torch.empty((D, 2), dtype=torch.int32, device=dev)
+    args = (masks.data_ptr(), mask_class.data_ptr(), boxes.data_ptr(), D, Kc, M, int(im_h), int(im_w), float(thresh))
+    with torch.cuda.device(dev):
+        _lib.check(lib.b200_segm_rle_sizes(*args, sizes.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "b200_segm_rle_sizes")
+        total = sizes.cpu().to(torch.int64).sum(dim=0)
+        counts = torch.empty((int(total[0]),), dtype=torch.int32, device=dev)
+        strings = torch.empty((int(total[1]),), dtype=torch.uint8, device=dev)
+        count_offs = torch.empty((D + 1,), dtype=torch.int64, device=dev)
+        string_offs = torch.empty((D + 1,), dtype=torch.int64, device=dev)
+        _lib.check(lib.b200_segm_rle_emit(*args, sizes.data_ptr(), ws.data_ptr(), ws_bytes, counts.data_ptr(), count_offs.data_ptr(),
+                                          strings.data_ptr(), string_offs.data_ptr(), _stream()), "b200_segm_rle_emit")
+    return counts, count_offs, strings, string_offs
+
+
+def paste_masks(masks, mask_class, boxes, im_h, im_w, thresh):
+    """The full-image binary masks segm_results encodes: uint8 CUDA (D, im_h, im_w), the reference's `im_mask` per detection."""
+    masks, mask_class, boxes, D, Kc, M = _segm_inputs(masks, mask_class, boxes, im_h, im_w)
+    out = torch.empty((D, int(im_h), int(im_w)), dtype=torch.uint8, device=masks.device)
+    if D == 0:
+        return out
+    with torch.cuda.device(masks.device):
+        _lib.check(_lib.load().b200_paste_masks(masks.data_ptr(), mask_class.data_ptr(), boxes.data_ptr(), D, Kc, M, int(im_h), int(im_w),
+                                                float(thresh), out.data_ptr(), _stream()), "b200_paste_masks")
+    return out

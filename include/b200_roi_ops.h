@@ -217,6 +217,35 @@ B200_API int b200_box_voting_batched(const float* top_dets_dev, const int* top_c
                                      const int* all_counts_host, int num_problems, float thresh, int scoring_method, float beta,
                                      float* out_dev, b200_stream_t stream);
 
+/* ---- test-time mask paste + COCO RLE (SURVEY.md 8f N3, lib/core/test.py:793-847) ---------------------------------
+ * The loop body of segm_results for the D detections of one image: box expanded by (M + 2) / M in float32 and truncated
+ * to int32, M x M soft mask zero-padded and resized to the box with cv2.resize's float32 INTER_LINEAR arithmetic (IPP
+ * off; 2x shrinks on both axes are cv2's INTER_AREA), thresholded with `> thresh`, pasted into an im_h x im_w image.
+ *   masks_dev       float32 (D, num_channels, M, M), dense;
+ *   mask_class_dev  int32 (D,): the channel detection d reads (a value outside [0, num_channels) reads as all zeros);
+ *   boxes_dev       float32 (D, 4) = [x1, y1, x2, y2], not yet expanded.
+ * A box whose expanded box lies wholly outside the image gives an empty mask (one count, im_h * im_w); non-finite boxes
+ * do not fault, their result is unspecified.  1 <= M <= 64, im_h * im_w < 2^28, else B200_ROI_EINVAL.
+ * COCO RLE of each detection's full-image mask (pycocotools mask.encode + rleToString), in two launches whatever D is:
+ *   b200_segm_rle_sizes  writes sizes_out_dev int32 (D, 2) = [number of counts, string bytes] and leaves its scan state
+ *                        in `workspace` (b200_segm_workspace_bytes(D) bytes, host arithmetic; else B200_ROI_EWORKSPACE);
+ *   b200_segm_rle_emit   same inputs, the sizes and the workspace of that call: counts_out_dev int32 (sum of counts):
+ *                        column-major run lengths starting with a run of zeros, summing to im_h * im_w per detection;
+ *                        strings_out_dev (sum of bytes): the compressed COCO strings, no terminators; count_offsets /
+ *                        string_offsets int64 (D + 1): where detection d's counts and string start.
+ * The caller reads the sizes once to allocate the outputs.
+ * b200_paste_masks: the full-image masks themselves, uint8 (D, im_h, im_w) (D <= 65535), the reference's im_mask. */
+B200_API size_t b200_segm_workspace_bytes(int num_dets);
+B200_API int b200_segm_rle_sizes(const float* masks_dev, const int* mask_class_dev, const float* boxes_dev, int num_dets, int num_channels,
+                                 int resolution, int im_h, int im_w, float thresh, int* sizes_out_dev, void* workspace,
+                                 size_t workspace_bytes, b200_stream_t stream);
+B200_API int b200_segm_rle_emit(const float* masks_dev, const int* mask_class_dev, const float* boxes_dev, int num_dets, int num_channels,
+                                int resolution, int im_h, int im_w, float thresh, const int* sizes_dev, const void* workspace,
+                                size_t workspace_bytes, int* counts_out_dev, long long* count_offsets_out_dev,
+                                unsigned char* strings_out_dev, long long* string_offsets_out_dev, b200_stream_t stream);
+B200_API int b200_paste_masks(const float* masks_dev, const int* mask_class_dev, const float* boxes_dev, int num_dets, int num_channels,
+                              int resolution, int im_h, int im_w, float thresh, unsigned char* out_dev, b200_stream_t stream);
+
 /* ---- introspection used by the benchmark / tests (no compute) ----------------------------------
  * Number of kernel launches the library has enqueued since load (all entry points). */
 B200_API unsigned long long b200_roi_ops_launch_count(void);
