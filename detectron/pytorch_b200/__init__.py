@@ -13,7 +13,7 @@ or, to make an unmodified checkout of the reference pick these up under ITS impo
 __version__ = "0.1.0"
 
 
-def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False):
+def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False):
     """Register this package's op modules in sys.modules under the reference's import paths.
 
     After this, `from modeling.roi_xfrom.roi_align.functions.roi_align import RoIAlignFunction`
@@ -30,6 +30,9 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
     `segms=True` re-points the reference's `core.test.segm_results` (lib/core/test.py:793-847, called from im_detect_all)
     at the device mask paste + RLE (`core/test.py` here), which needs no pycocotools; the reference's `core.test` must be
     importable for that.
+    `keypoints=True` re-points the reference's `core.test.keypoint_results` (lib/core/test.py:850-866, called from
+    im_detect_all) at the device keypoint extraction and OKS NMS (`core/test.py` here), reading the reference's `cfg`
+    at call time; the reference's `core.test` must be importable for that.
     """
     import importlib
     import sys
@@ -75,4 +78,10 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
         ref_test.segm_results = lambda cls_boxes, masks, ref_boxes, im_h, im_w: ours(cls_boxes, masks, ref_boxes, im_h, im_w,
                                                                                      cfg=ref_test.cfg)
         installed.append("core.test.segm_results")
+    if keypoints:
+        ref_test = importlib.import_module("core.test")              # the reference's module
+        ours_kp = importlib.import_module(__name__ + ".core.test").keypoint_results
+        ref_test.keypoint_results = lambda cls_boxes, pred_heatmaps, ref_boxes: ours_kp(cls_boxes, pred_heatmaps, ref_boxes,
+                                                                                         cfg=ref_test.cfg)
+        installed.append("core.test.keypoint_results")
     return installed

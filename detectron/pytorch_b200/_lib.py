@@ -100,6 +100,11 @@ _SIGNATURES = {
     # (masks, mask_class, boxes, D, Kc, M, im_h, im_w, thresh, out, stream)
     "b200_paste_masks": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, _c_float_p] + [ctypes.c_int] * 5 + [ctypes.c_float, ctypes.c_void_p,
                                                                                                           _stream_t]),
+    # (maps, rois, D, K, M, min_size, xy_preds, stream)
+    "b200_heatmaps_to_keypoints": (ctypes.c_int, [_c_float_p, _c_float_p] + [ctypes.c_int] * 4 + [_c_float_p, _stream_t]),
+    # (xy_preds, rois, D, K, thresh, keep, num_keep, stream)
+    "b200_nms_oks": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p,
+                                    _stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

@@ -18,6 +18,10 @@ Soft-NMS follows lib/utils/cython_nms.pyx:98-203 step for step (same greedy orde
 `segm_results(cls_boxes, masks, ref_boxes, im_h, im_w)` is the Mask R-CNN step after it (lib/core/test.py:793-847): every
 detection's mask is pasted into the image and run-length encoded on the device in two launches per image, with one host
 read of the per-detection sizes; the result is the reference's list of COCO RLE dicts.
+
+`keypoint_results(cls_boxes, pred_heatmaps, ref_boxes)` is the Keypoint R-CNN step (lib/core/test.py:850-866): every
+detection's 17 heatmaps are resized, searched for their maximum and soft-maxed on the device in one launch (plus one for
+the optional OKS NMS), with one host read of the (R, 4, 17) result; the result is the reference's cls_keyps.
 """
 import numpy as np
 import torch
@@ -158,3 +162,55 @@ def segm_results(cls_boxes, masks, ref_boxes, im_h, im_w, cfg=None, **kw):
             d += 1
         cls_segms[j] = segms
     return cls_segms
+
+
+PERSON_CLASS_INDEX = 1          # lib/utils/keypoints.py:66-68
+
+
+def _keypoint_params(cfg, kw):
+    if cfg is not None:
+        p = dict(num_classes=cfg.MODEL.NUM_CLASSES, num_keypoints=cfg.KRCNN.NUM_KEYPOINTS, inference_min_size=cfg.KRCNN.INFERENCE_MIN_SIZE,
+                 nms_oks=cfg.KRCNN.NMS_OKS)
+    else:
+        p = dict(num_classes=None, num_keypoints=17, inference_min_size=0, nms_oks=False)        # lib/core/config.py:782-870
+    p.update(kw)
+    return p
+
+
+def keypoint_results(cls_boxes, pred_heatmaps, ref_boxes, cfg=None, **kw):
+    """cls_keyps of lib/core/test.py:850-866: a list over classes, empty except at the person class (index 1), which holds
+    one float32 (4, K) array of (x, y, logit, prob) rows per detection, in the order of ref_boxes.  With NMS_OKS the OKS
+    NMS (threshold 0.3) drops detections and cls_boxes[1] is filtered in place, like the reference.
+
+    pred_heatmaps: the keypoint head's logits, a numpy array (R, K, M, M) like the reference's or a float32 CUDA tensor,
+    which skips the device-to-host copy.  ref_boxes: (R, >=4) detections, numpy or CUDA.  The keypoints are extracted on
+    the device in one launch (ops.heatmaps_to_keypoints_raw: cv2's float32 INTER_CUBIC arithmetic), plus one for the OKS
+    NMS; the host reads the (R, 4, K) result once (and, with NMS_OKS, the kept indices).  Configuration: the reference's
+    `cfg` (MODEL.NUM_CLASSES, KRCNN.NUM_KEYPOINTS / INFERENCE_MIN_SIZE / NMS_OKS) or keyword arguments num_classes,
+    num_keypoints, inference_min_size, nms_oks."""
+    p = _keypoint_params(cfg, kw)
+    num_classes = int(p["num_classes"] or len(cls_boxes))
+    cls_keyps = [[] for _ in range(num_classes)]
+    D = int(pred_heatmaps.shape[0])
+    if len(pred_heatmaps.shape) != 4 or int(pred_heatmaps.shape[1]) != int(p["num_keypoints"]):
+        raise ValueError("keypoint_results: heatmaps must be (R, %d, M, M), got %s" % (int(p["num_keypoints"]), tuple(pred_heatmaps.shape)))
+    if int(ref_boxes.shape[0]) != D:
+        raise ValueError("keypoint_results: %d heatmaps for %d boxes" % (D, int(ref_boxes.shape[0])))
+    if D == 0:
+        return cls_keyps
+    dev = next((x.device for x in (pred_heatmaps, ref_boxes) if torch.is_tensor(x) and x.is_cuda),
+               torch.device("cuda", torch.cuda.current_device()))
+    maps = pred_heatmaps if torch.is_tensor(pred_heatmaps) else torch.from_numpy(np.ascontiguousarray(pred_heatmaps, dtype=np.float32))
+    rois = ref_boxes if torch.is_tensor(ref_boxes) else torch.from_numpy(np.ascontiguousarray(ref_boxes, dtype=np.float32))
+    maps = maps.to(dev, dtype=torch.float32)
+    rois = rois.to(dev, dtype=torch.float32)
+    xy = ops.heatmaps_to_keypoints_raw(maps, rois, int(p["inference_min_size"]))
+    if p["nms_oks"]:
+        keep_dev, num_keep = ops.nms_oks_raw(xy, rois, 0.3)
+    xy_preds = xy.cpu().numpy()
+    if p["nms_oks"]:
+        keep = keep_dev[:int(num_keep.item())].cpu().tolist()
+        xy_preds = xy_preds[keep]
+        cls_boxes[PERSON_CLASS_INDEX] = cls_boxes[PERSON_CLASS_INDEX][keep, :]
+    cls_keyps[PERSON_CLASS_INDEX] = [xy_preds[i] for i in range(xy_preds.shape[0])]
+    return cls_keyps

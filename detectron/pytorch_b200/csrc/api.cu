@@ -78,6 +78,10 @@ int segm_rle_sizes(const float*, const int*, const float*, int, int, int, int, i
 int segm_rle_emit(const float*, const int*, const float*, int, int, int, int, int, float, const int*, const void*, int*, long long*,
                   unsigned char*, long long*, cudaStream_t);
 int paste_masks(const float*, const int*, const float*, int, int, int, int, int, float, unsigned char*, cudaStream_t);
+bool keypoints_args_ok(int, int, int, int);
+bool nms_oks_args_ok(int, int);
+int heatmaps_to_keypoints(const float*, const float*, int, int, int, int, float*, cudaStream_t);
+int nms_oks(const float*, const float*, int, double, int*, int*, cudaStream_t);
 
 // B200_ROI_ALIGN_PATH=generic|tiled|stream|auto (default auto) -- test/benchmark override of the forward dispatch
 //   0 auto: streaming-strip path -> quad-strip path -> tiled path -> generic, each when it applies.  On H100 the streaming
@@ -598,6 +602,22 @@ int b200_paste_masks(const float* masks_dev, const int* mask_class_dev, const fl
     if (!masks_dev || !mask_class_dev || !boxes_dev || !out_dev) return B200_ROI_EINVAL;
     return paste_masks(masks_dev, mask_class_dev, boxes_dev, num_dets, num_channels, resolution, im_h, im_w, thresh, out_dev,
                        (cudaStream_t)stream);
+}
+
+int b200_heatmaps_to_keypoints(const float* maps_dev, const float* rois_dev, int num_rois, int num_keypoints, int heatmap_size,
+                               int min_size, float* xy_preds_dev, b200_stream_t stream) {
+    if (!keypoints_args_ok(num_rois, num_keypoints, heatmap_size, min_size)) return B200_ROI_EINVAL;
+    if (num_rois == 0) return B200_ROI_OK;
+    if (!maps_dev || !rois_dev || !xy_preds_dev) return B200_ROI_EINVAL;
+    return heatmaps_to_keypoints(maps_dev, rois_dev, num_rois, num_keypoints, heatmap_size, min_size, xy_preds_dev, (cudaStream_t)stream);
+}
+
+int b200_nms_oks(const float* xy_preds_dev, const float* rois_dev, int num_rois, int num_keypoints, double thresh, int* keep_dev,
+                 int* num_keep_dev, b200_stream_t stream) {
+    if (!nms_oks_args_ok(num_rois, num_keypoints)) return B200_ROI_EINVAL;
+    if (num_rois == 0) return B200_ROI_OK;
+    if (!xy_preds_dev || !rois_dev || !keep_dev || !num_keep_dev) return B200_ROI_EINVAL;
+    return nms_oks(xy_preds_dev, rois_dev, num_rois, thresh, keep_dev, num_keep_dev, (cudaStream_t)stream);
 }
 
 }  // extern "C"

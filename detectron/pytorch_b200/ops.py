@@ -563,3 +563,55 @@ def paste_masks(masks, mask_class, boxes, im_h, im_w, thresh):
         _lib.check(_lib.load().b200_paste_masks(masks.data_ptr(), mask_class.data_ptr(), boxes.data_ptr(), D, Kc, M, int(im_h), int(im_w),
                                                 float(thresh), out.data_ptr(), _stream()), "b200_paste_masks")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# Test-time keypoint extraction + OKS NMS (SURVEY.md 8f N3, lib/utils/keypoints.py:103-157, 225-266)
+# ------------------------------------------------------------------------------------------------
+def _keypoint_rois(rois, D, device):
+    _need_cuda_f32(rois, "rois")
+    if rois.dim() != 2 or rois.size(0) != D or rois.size(1) < 4:
+        raise ValueError("rois must be (D, >=4) = [x1, y1, x2, y2, ...] with D = %d, got %s" % (D, tuple(rois.shape)))
+    return rois[:, :4].to(device).contiguous()
+
+
+def heatmaps_to_keypoints_raw(maps, rois, min_size=0):
+    """Keypoints of one image's detections from the keypoint head's logits (lib/utils/keypoints.py:103-157, cv2's float32
+    INTER_CUBIC arithmetic).  maps: float32 CUDA (D, K, M, M); rois: float32 CUDA (D, >=4) = [x1, y1, x2, y2];
+    min_size: KRCNN.INFERENCE_MIN_SIZE (<= 0: none).  Returns a float32 CUDA (D, 4, K) tensor of rows (x, y, logit, prob).
+    One launch, no host sync."""
+    _need_cuda_f32(maps, "maps")
+    if maps.dim() != 4 or maps.size(2) != maps.size(3):
+        raise ValueError("maps must be (D, K, M, M), got %s" % (tuple(maps.shape),))
+    D, K, M = maps.size(0), maps.size(1), maps.size(2)
+    rois = _keypoint_rois(rois, D, maps.device)
+    maps = maps.contiguous()
+    out = torch.empty((D, 4, K), dtype=torch.float32, device=maps.device)
+    if D == 0:
+        return out
+    with torch.cuda.device(maps.device):
+        _lib.check(_lib.load().b200_heatmaps_to_keypoints(maps.data_ptr(), rois.data_ptr(), D, K, M, int(min_size), out.data_ptr(),
+                                                          _stream()),
+                   "b200_heatmaps_to_keypoints")
+    return out
+
+
+def nms_oks_raw(xy_preds, rois, thresh):
+    """Greedy OKS NMS of lib/utils/keypoints.py:225-266 on (D, 4, 17) predictions and their (D, >=4) boxes, float32 CUDA.
+    Returns (keep int32 (D,), num_keep int32 (1,)) on the device, no host sync: keep[:num_keep] are the kept indices in
+    greedy order (descending mean logit; equal scores the higher index first)."""
+    _need_cuda_f32(xy_preds, "xy_preds")
+    if xy_preds.dim() != 3 or xy_preds.size(1) != 4:
+        raise ValueError("xy_preds must be (D, 4, K), got %s" % (tuple(xy_preds.shape),))
+    D, K = xy_preds.size(0), xy_preds.size(2)
+    rois = _keypoint_rois(rois, D, xy_preds.device)
+    xy_preds = xy_preds.contiguous()
+    keep = torch.empty((max(D, 1),), dtype=torch.int32, device=xy_preds.device)
+    if D == 0:
+        return keep[:0], torch.zeros((1,), dtype=torch.int32, device=xy_preds.device)
+    num_keep = torch.empty((1,), dtype=torch.int32, device=xy_preds.device)
+    with torch.cuda.device(xy_preds.device):
+        _lib.check(_lib.load().b200_nms_oks(xy_preds.data_ptr(), rois.data_ptr(), D, K, float(thresh), keep.data_ptr(), num_keep.data_ptr(),
+                                            _stream()),
+                   "b200_nms_oks")
+    return keep, num_keep

@@ -1,0 +1,41 @@
+"""Host-array front door of the device keypoint extraction, named like the reference's `utils.keypoints`
+(lib/utils/keypoints.py): `heatmaps_to_keypoints(maps, rois)` (:103-157) and `nms_oks(kp_predictions, rois, thresh)`
+(:225-266).  Both take numpy arrays like the reference's or CUDA tensors, and return numpy results.
+
+The resize, argmax and coordinates reproduce the reference's numpy 2 / cv2 float32 INTER_CUBIC arithmetic bit for bit;
+prob (the spatial softmax at the maximum) is summed in double on the device where numpy sums float32 pairwise, so it
+agrees to ~1e-7 relative.  nms_oks takes equal scores the higher index first (the reference's order for ties comes from
+numpy's unstable argsort), and its float64 exp may differ from numpy's by an ulp.
+"""
+import numpy as np
+import torch
+
+from .. import ops
+
+
+def _device_of(*xs):
+    for x in xs:
+        if torch.is_tensor(x) and x.is_cuda:
+            return x.device
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _f32(x, dev):
+    t = x if torch.is_tensor(x) else torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32))
+    return t.to(dev, dtype=torch.float32)
+
+
+def heatmaps_to_keypoints(maps, rois, min_size=0):
+    """(D, 4, K) float32 numpy array of (x, y, logit, prob) rows from the (D, K, M, M) logits and (D, >=4) boxes;
+    min_size is KRCNN.INFERENCE_MIN_SIZE (<= 0: none)."""
+    dev = _device_of(maps, rois)
+    return ops.heatmaps_to_keypoints_raw(_f32(maps, dev), _f32(rois, dev), min_size).cpu().numpy()
+
+
+def nms_oks(kp_predictions, rois, thresh):
+    """Kept indices (list of int, greedy order) of the OKS NMS over (D, 4, 17) predictions and (D, >=4) boxes."""
+    if kp_predictions.shape[0] == 0:
+        return []
+    dev = _device_of(kp_predictions, rois)
+    keep, num_keep = ops.nms_oks_raw(_f32(kp_predictions, dev), _f32(rois, dev), thresh)
+    return keep[:int(num_keep.item())].cpu().tolist()

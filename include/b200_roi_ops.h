@@ -246,6 +246,27 @@ B200_API int b200_segm_rle_emit(const float* masks_dev, const int* mask_class_de
 B200_API int b200_paste_masks(const float* masks_dev, const int* mask_class_dev, const float* boxes_dev, int num_dets, int num_channels,
                               int resolution, int im_h, int im_w, float thresh, unsigned char* out_dev, b200_stream_t stream);
 
+/* ---- test-time keypoint extraction + OKS NMS (SURVEY.md 8f N3, lib/utils/keypoints.py:103-157, 225-266) -----------
+ * b200_heatmaps_to_keypoints: heatmaps_to_keypoints for the D detections of one image, one launch.
+ *   maps_dev      float32 (D, K, M, M), dense: the keypoint head's logits;
+ *   rois_dev      float32 (D, 4) = [x1, y1, x2, y2];
+ *   xy_preds_dev  float32 (D, 4, K): rows x, y, logit, prob.
+ * Each heatmap is resized to max(ceil(max(x2 - x1, 1)), min_size) x ... pixels (min_size <= 0: no minimum) with
+ * cv2.resize's float32 INTER_CUBIC arithmetic on the K-channel image; x, y are the box coordinates of the first maximum
+ * (row-major), logit its value, prob the spatial softmax there (the sum of exponentials is accumulated in double).
+ * The resized maps are never stored.  A side above 16384 pixels, or a non-finite box, is resized to 16384 pixels (the
+ * reference would build that map); non-finite logits give an unspecified result.  1 <= M <= 64, K >= 1,
+ * min_size <= 16384, D * K < 2^31, else B200_ROI_EINVAL.
+ * b200_nms_oks: the greedy OKS NMS of nms_oks on those predictions (K must be 17, the COCO keypoints; D <= 4096), one
+ * single-CTA launch.  Score = float32 mean of the 17 logits; descending score, equal scores the higher index first; OKS
+ * in float64 with the COCO sigmas and the area (x2 - x1 + 1)(y2 - y1 + 1); a candidate is dropped when OKS > thresh.
+ * Writes the kept indices in greedy order to keep_dev int32 (D,) and their number to num_keep_dev int32 (1,).
+ * D == 0: both return B200_ROI_OK without writing anything. */
+B200_API int b200_heatmaps_to_keypoints(const float* maps_dev, const float* rois_dev, int num_rois, int num_keypoints, int heatmap_size,
+                                        int min_size, float* xy_preds_dev, b200_stream_t stream);
+B200_API int b200_nms_oks(const float* xy_preds_dev, const float* rois_dev, int num_rois, int num_keypoints, double thresh, int* keep_dev,
+                          int* num_keep_dev, b200_stream_t stream);
+
 /* ---- introspection used by the benchmark / tests (no compute) ----------------------------------
  * Number of kernel launches the library has enqueued since load (all entry points). */
 B200_API unsigned long long b200_roi_ops_launch_count(void);
