@@ -67,6 +67,8 @@ _SIGNATURES = {
     # (boxes, counts_host, P, dim, thresh, keep_out, num_out, workspace, workspace_bytes, stream)
     "b200_nms_batched": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_void_p,
                                         ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, _stream_t]),
+    "b200_nms_batched_cython": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_void_p,
+                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, _stream_t]),
     # (dets, counts_host, P, sigma, Nt, score_thresh, method, inds_out, num_out, stream)
     "b200_soft_nms_batched": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
                                              ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, _stream_t]),

@@ -11,9 +11,16 @@ Configuration: pass the reference's `cfg` object (read at call time like the ref
 cfg.TEST.SCORE_THRESH / NMS / SOFT_NMS.* / BBOX_VOTE.* / DETECTIONS_PER_IM) or the same values as keyword arguments.
 Inputs and outputs are numpy arrays like the reference's; CUDA tensors are accepted and skip the upload.
 
-Flavour note (as for the proposal NMS): the device NMS keeps the reference CUDA kernel's `IoU > thresh` test, the Cython
-routine the reference calls here uses `>=`; they differ only on pairs whose IoU equals the threshold to the last bit.
-Soft-NMS follows lib/utils/cython_nms.pyx:98-203 step for step (same greedy order, same drop rule).
+Flavour note: classic NMS is the Cython routine the reference calls here, cython_nms.nms (lib/utils/cython_nms.pyx:37-87):
+`b200_nms_batched_cython` rounds both box areas on their own, forms IoU = inter / ((area_i + area_j) - inter) in float32
+and suppresses when IoU >= float32(NMS).  (The proposal layer keeps the reference CUDA kernel's fused area and `>`; the
+two differ on pairs whose IoU lies within about one ulp of the threshold.)  Tie rule: each class's candidates are sorted
+by descending score, stably, so among equal scores the lower detection index comes first and suppresses the other.  The
+reference sorts with `scores.argsort()[::-1]`, which is not stable, so where two overlapping boxes of one class tie its
+result is arbitrary; elsewhere the order of tied boxes does not change the result.
+Soft-NMS follows lib/utils/cython_nms.pyx:98-203 step for step (same greedy order, same drop rule, and the arithmetic of
+the C that Cython generates from it: the literal 1.0 makes box areas and the union double expressions, rounded to float
+once).
 
 `segm_results(cls_boxes, masks, ref_boxes, im_h, im_w)` is the Mask R-CNN step after it (lib/core/test.py:793-847): every
 detection's mask is pasted into the image and run-length encoded on the device in two launches per image, with one host
@@ -79,7 +86,7 @@ def box_results_with_nms_and_limit(scores, boxes, cfg=None, **kw):
                 seg = slice(int(offs[j]), int(offs[j + 1]))
                 order[seg] = torch.sort(sc[seg], descending=True, stable=True)[1] + int(offs[j])
             sorted_dets = dets[order]
-            keep, num = ops.nms_batched_chunked(sorted_dets, [int(c) for c in counts], float(p["nms"]))
+            keep, num = ops.nms_batched_chunked(sorted_dets, [int(c) for c in counts], float(p["nms"]), cython=True)
             num = num.cpu().numpy()
             for j in live:
                 k = keep[offs[j]:offs[j] + int(num[j])].long() + int(offs[j])      # positions in the sorted copy

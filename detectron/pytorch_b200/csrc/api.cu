@@ -117,7 +117,7 @@ int nms(const float*, int, int, float, int*, int*, void*, size_t, cudaStream_t);
 size_t nms_batched_workspace_bytes(const int*, int);
 int soft_nms_batched(float*, const int*, int, float, float, float, int, int*, int*, cudaStream_t);
 int box_voting_batched(const float*, const int*, const float*, const int*, int, float, int, float, float*, cudaStream_t);
-int nms_batched(const float*, const int*, int, int, float, int*, int*, void*, size_t, cudaStream_t);
+int nms_batched(const float*, const int*, int, int, float, bool, int*, int*, void*, size_t, cudaStream_t);
 size_t roi_align_bwd_nhwc_workspace_bytes(int, int, int, int);
 int roi_align_backward_nhwc(const float*, float, int, int, int, int, int, int, int, int, const float*, float*, const int*, void*, size_t, cudaStream_t);
 
@@ -481,15 +481,27 @@ size_t b200_nms_batched_workspace_bytes(const int* counts_host, int num_problems
     return nms_batched_workspace_bytes(counts_host, num_problems);
 }
 
-int b200_nms_batched(const float* boxes_dev, const int* counts_host, int num_problems, int boxes_dim, float nms_overlap_thresh,
-                     int* keep_out_dev, int* num_out_dev, void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+static int nms_batched_entry(const float* boxes_dev, const int* counts_host, int num_problems, int boxes_dim, float nms_overlap_thresh,
+                             bool cython, int* keep_out_dev, int* num_out_dev, void* workspace, size_t workspace_bytes, b200_stream_t stream) {
     if (!counts_host || num_problems < 1 || !num_out_dev) return B200_ROI_EINVAL;
     long long total = 0;
     for (int p = 0; p < num_problems && p < 64; ++p) total += counts_host[p] > 0 ? counts_host[p] : 0;
     if (total > 0 && (!boxes_dev || !keep_out_dev)) return B200_ROI_EINVAL;
-    const int rc = nms_batched(boxes_dev, counts_host, num_problems, boxes_dim, nms_overlap_thresh, keep_out_dev, num_out_dev, workspace,
-                               workspace_bytes, (cudaStream_t)stream);
+    const int rc = nms_batched(boxes_dev, counts_host, num_problems, boxes_dim, nms_overlap_thresh, cython, keep_out_dev, num_out_dev,
+                               workspace, workspace_bytes, (cudaStream_t)stream);
     return rc == 1000 ? B200_ROI_EINVAL : rc;
+}
+
+int b200_nms_batched(const float* boxes_dev, const int* counts_host, int num_problems, int boxes_dim, float nms_overlap_thresh,
+                     int* keep_out_dev, int* num_out_dev, void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+    return nms_batched_entry(boxes_dev, counts_host, num_problems, boxes_dim, nms_overlap_thresh, false, keep_out_dev, num_out_dev, workspace,
+                             workspace_bytes, stream);
+}
+
+int b200_nms_batched_cython(const float* boxes_dev, const int* counts_host, int num_problems, int boxes_dim, float nms_overlap_thresh,
+                            int* keep_out_dev, int* num_out_dev, void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+    return nms_batched_entry(boxes_dev, counts_host, num_problems, boxes_dim, nms_overlap_thresh, true, keep_out_dev, num_out_dev, workspace,
+                             workspace_bytes, stream);
 }
 
 int b200_soft_nms_batched(float* dets_dev, const int* counts_host, int num_problems, float sigma, float overlap_thresh,

@@ -53,15 +53,19 @@ soft_nms_kernel(float* __restrict__ boxes_all, int* __restrict__ inds_all, int* 
         }
         __syncwarp();
         const float tx1 = boxes[i * 5], ty1 = boxes[i * 5 + 1], tx2 = boxes[i * 5 + 2], ty2 = boxes[i * 5 + 3];
+        // The C that Cython generates from the .pyx adds the literal 1.0 in double: a box's area is a double product rounded
+        // to float once (cython_area), iw / ih are double sums rounded to float, and the union is the double expression
+        // (t_area + area) - iw * ih rounded to float once.  The intersection, the IoU and the score product are float.
+        const double t_area = __dmul_rn(__dadd_rn((double)__fsub_rn(tx2, tx1), 1.0), __dadd_rn((double)__fsub_rn(ty2, ty1), 1.0));
         for (int k = i + 1 + lane; k < N; k += 32) {
             const float x1 = boxes[k * 5], y1 = boxes[k * 5 + 1], x2 = boxes[k * 5 + 2], y2 = boxes[k * 5 + 3];
-            const float area = __fmul_rn(__fadd_rn(__fsub_rn(x2, x1), 1.f), __fadd_rn(__fsub_rn(y2, y1), 1.f));
-            const float iw = __fadd_rn(__fsub_rn(fminf(tx2, x2), fmaxf(tx1, x1)), 1.f);
+            const float area = cython_area(x1, y1, x2, y2);
+            const float iw = (float)__dadd_rn((double)__fsub_rn(fminf(tx2, x2), fmaxf(tx1, x1)), 1.0);
             if (iw > 0.f) {
-                const float ih = __fadd_rn(__fsub_rn(fminf(ty2, y2), fmaxf(ty1, y1)), 1.f);
+                const float ih = (float)__dadd_rn((double)__fsub_rn(fminf(ty2, y2), fmaxf(ty1, y1)), 1.0);
                 if (ih > 0.f) {
                     const float inter = __fmul_rn(iw, ih);
-                    const float ua = __fsub_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fsub_rn(tx2, tx1), 1.f), __fadd_rn(__fsub_rn(ty2, ty1), 1.f)), area), inter);
+                    const float ua = (float)__dsub_rn(__dadd_rn(t_area, (double)area), (double)inter);
                     const float ov = __fdiv_rn(inter, ua);
                     float weight;
                     if (method == 1) weight = (ov > Nt) ? __fsub_rn(1.f, ov) : 1.f;

@@ -53,6 +53,11 @@ struct __align__(16) ColBox {
     float x0, y0, x1, y1;
 };
 
+// The exact IoU test of one pair (a = the higher-scoring "row" box, Sa its rounded area).  Two flavours:
+//   CUDA   (kCython = false): the reference CUDA kernel's recipe, den = FFMA(bw, bh, Sa) - inter, suppress on IoU > thresh;
+//   Cython (kCython = true):  lib/utils/cython_nms.pyx:37-87, both areas rounded on their own, den = (Sa + Sb) - inter,
+//                             suppress on IoU >= thresh.
+template <bool kCython>
 __device__ __forceinline__ bool nms_bit(float a0, float a1, float a2, float a3, float Sa,
                                         float b0, float b1, float b2, float b3, float thresh) {
     const float left = fmaxf(a0, b0), right = fminf(a2, b2);
@@ -60,9 +65,9 @@ __device__ __forceinline__ bool nms_bit(float a0, float a1, float a2, float a3, 
     const float w = fmaxf(__fadd_rn(__fsub_rn(right, left), 1.f), 0.f);
     const float h = fmaxf(__fadd_rn(__fsub_rn(bottom, top), 1.f), 0.f);
     const float inter = __fmul_rn(w, h);
-    const float t = __fmaf_rn(__fadd_rn(__fsub_rn(b2, b0), 1.f), __fadd_rn(__fsub_rn(b3, b1), 1.f), Sa);
-    const float den = __fsub_rn(t, inter);
-    return __fdiv_rn(inter, den) > thresh;
+    const float bw = __fadd_rn(__fsub_rn(b2, b0), 1.f), bh = __fadd_rn(__fsub_rn(b3, b1), 1.f);
+    if (kCython) return __fdiv_rn(inter, __fsub_rn(__fadd_rn(Sa, __fmul_rn(bw, bh)), inter)) >= thresh;
+    return __fdiv_rn(inter, __fsub_rn(__fmaf_rn(bw, bh, Sa), inter)) > thresh;
 }
 
 struct __align__(16) ColBoxEx {
@@ -78,6 +83,9 @@ struct __align__(16) ColBoxEx {
 // [2^-20, 2^20]: lo = -inf, hi = +inf) is marked undecided and re-evaluated with the exact recipe (nms_bit) after
 // the main loop.  Results are therefore bit-identical to the all-division version; the main loop is branch-free,
 // fully unrolled (bit positions are immediates) and ~26 instructions per pair instead of ~42.
+// The screen serves both flavours of nms_bit: their denominators differ by about one rounding, far inside the band, and
+// `>` and `>=` differ only at the threshold itself, so only the exact re-evaluation and the transposed words depend on it.
+template <bool kCython>
 __device__ __forceinline__ void nms_mask_tile(const float* __restrict__ boxes, int n, int dim, float thresh, float lo, float hi,
                                               u64* __restrict__ mask, u64* __restrict__ diag_t, int idx) {
     const int col_blocks = (n + kNmsTile - 1) / kNmsTile;
@@ -141,7 +149,7 @@ __device__ __forceinline__ void nms_mask_tile(const float* __restrict__ boxes, i
         const int i = __ffsll((long long)und) - 1;
         und &= und - 1ULL;
         const ColBoxEx b = cols[i];
-        if (nms_bit(a0, a1, a2, a3, Sa, b.x0, b.y0, b.x1, b.y1, thresh)) t |= 1ULL << i;
+        if (nms_bit<kCython>(a0, a1, a2, a3, Sa, b.x0, b.y0, b.x1, b.y1, thresh)) t |= 1ULL << i;
     }
     mask[(size_t)cur * col_blocks + col_start] = t;
     if (row_start == col_start) {
@@ -151,7 +159,7 @@ __device__ __forceinline__ void nms_mask_tile(const float* __restrict__ boxes, i
         u64 tt = 0;
         for (int j = 0; j < (int)threadIdx.x; ++j) {
             const ColBoxEx r = cols[j];
-            if (nms_bit(r.x0, r.y0, r.x1, r.y1, __fmul_rn(r.bw, r.bh), a0, a1, a2, a3, thresh)) tt |= 1ULL << j;
+            if (nms_bit<kCython>(r.x0, r.y0, r.x1, r.y1, __fmul_rn(r.bw, r.bh), a0, a1, a2, a3, thresh)) tt |= 1ULL << j;
         }
         diag_t[cur] = tt;
     }
@@ -160,7 +168,7 @@ __device__ __forceinline__ void nms_mask_tile(const float* __restrict__ boxes, i
 __global__ void __launch_bounds__(kNmsTile)
 nms_mask_kernel(const float* __restrict__ boxes, int n, int dim, float thresh, float lo, float hi,
                 u64* __restrict__ mask, u64* __restrict__ diag_t) {
-    nms_mask_tile(boxes, n, dim, thresh, lo, hi, mask, diag_t, (int)blockIdx.x);
+    nms_mask_tile<false>(boxes, n, dim, thresh, lo, hi, mask, diag_t, (int)blockIdx.x);
 }
 
 // ---- several independent problems in one launch (SURVEY 8f N1: the (image, level) proposal sets of one step) ----
@@ -174,6 +182,7 @@ struct NmsBatch {
     unsigned long long diag_off[kNmsMaxProblems];
 };
 
+template <bool kCython>
 __global__ void __launch_bounds__(kNmsTile)
 nms_mask_batched_kernel(const float* __restrict__ boxes, const __grid_constant__ NmsBatch nb, int dim, float thresh, float lo, float hi,
                         u64* __restrict__ ws) {
@@ -186,7 +195,7 @@ nms_mask_batched_kernel(const float* __restrict__ boxes, const __grid_constant__
         }
         p = lo_p;
     }
-    nms_mask_tile(boxes + (size_t)nb.box_off[p] * dim, nb.n[p], dim, thresh, lo, hi, ws + nb.mask_off[p], ws + nb.diag_off[p],
+    nms_mask_tile<kCython>(boxes + (size_t)nb.box_off[p] * dim, nb.n[p], dim, thresh, lo, hi, ws + nb.mask_off[p], ws + nb.diag_off[p],
                   (int)blockIdx.x - nb.tile_off[p]);
 }
 
@@ -484,7 +493,8 @@ size_t nms_batched_workspace_bytes(const int* counts, int num_problems) {
     return (words * sizeof(u64) + 255) / 256 * 256 + 256;
 }
 
-int nms_batched(const float* boxes, const int* counts, int num_problems, int dim, float thresh, int* keep_out, int* num_out,
+// cython: the IoU test of lib/utils/cython_nms.pyx (see nms_bit) instead of the reference CUDA kernel's
+int nms_batched(const float* boxes, const int* counts, int num_problems, int dim, float thresh, bool cython, int* keep_out, int* num_out,
                 void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     NmsBatch nb; size_t words = 0; int mx = 0;
     if (dim < 4 || !nms_batch_plan(counts, num_problems, &nb, &words, &mx)) return B200_ROI_EINVAL;
@@ -504,7 +514,8 @@ int nms_batched(const float* boxes, const int* counts, int num_problems, int dim
     if (reach == 0) return 1000;                        // a problem too large for the pipelined scan: the caller loops over b200_nms
     u64* ws = (u64*)workspace;
     if (nb.tile_off[num_problems] > 0)
-        nms_mask_batched_kernel<<<(unsigned)nb.tile_off[num_problems], kNmsTile, 0, stream>>>(boxes, nb, dim, thresh, lo, hi, ws);
+        (cython ? nms_mask_batched_kernel<true> : nms_mask_batched_kernel<false>)<<<(unsigned)nb.tile_off[num_problems], kNmsTile, 0, stream>>>(
+            boxes, nb, dim, thresh, lo, hi, ws);
     void (*kern)(const u64*, const NmsBatch, int*, int*) =
         (reach == 4) ? nms_scan_resolver_batched_kernel<4> : (reach == 3) ? nms_scan_resolver_batched_kernel<3> : nms_scan_resolver_batched_kernel<2>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_res);

@@ -393,10 +393,12 @@ def topk_batched_raw(score_maps, ks):
     return order[:total], scores[:total]
 
 
-def nms_batched_raw(dets, counts, thresh):
+def nms_batched_raw(dets, counts, thresh, cython=False):
     """`len(counts)` independent NMS problems in one pair of launches.  dets: (sum(counts), >=4) rows of the problems back to
     back, each problem score-sorted; counts: host ints.  Returns (keep int32 (sum(counts),), num_out int32 (P,)) on the
-    device: problem p's kept indices (relative to its first row) sit at keep[offset_p : offset_p + num_out[p]]."""
+    device: problem p's kept indices (relative to its first row) sit at keep[offset_p : offset_p + num_out[p]].
+    cython=False: the reference CUDA kernel's IoU test (fused area, IoU > thresh, b200_nms_batched); True: the Cython
+    NMS's (separately rounded areas, IoU >= thresh, b200_nms_batched_cython)."""
     import ctypes
     _need_cuda_f32(dets, "dets")
     if dets.dim() != 2 or dets.size(1) < 4:
@@ -415,16 +417,17 @@ def nms_batched_raw(dets, counts, thresh):
         raise ValueError("b200_nms_batched: 1..64 problems expected, got %d" % P)
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dets.device)
     with torch.cuda.device(dets.device):
-        _lib.check(lib.b200_nms_batched(dets.data_ptr(), ctypes.cast(c_arr, ctypes.c_void_p), P, dets.size(1), float(thresh), keep.data_ptr(),
-                                        num_out.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "b200_nms_batched")
+        fn, name = (lib.b200_nms_batched_cython, "b200_nms_batched_cython") if cython else (lib.b200_nms_batched, "b200_nms_batched")
+        _lib.check(fn(dets.data_ptr(), ctypes.cast(c_arr, ctypes.c_void_p), P, dets.size(1), float(thresh), keep.data_ptr(), num_out.data_ptr(),
+                      ws.data_ptr(), ws_bytes, _stream()), name)
     return keep, num_out
 
 
-def nms_batched_chunked(dets, counts, thresh):
+def nms_batched_chunked(dets, counts, thresh, cython=False):
     """nms_batched_raw for any number of problems (b200_nms_batched takes up to 64 per call): same return layout."""
     counts = [int(c) for c in counts]
     if len(counts) <= 64:
-        return nms_batched_raw(dets, counts, thresh)
+        return nms_batched_raw(dets, counts, thresh, cython)
     keeps, nums, off = [], [], 0
     for c0 in range(0, len(counts), 64):
         chunk = counts[c0:c0 + 64]
@@ -433,7 +436,7 @@ def nms_batched_chunked(dets, counts, thresh):
             keeps.append(torch.empty((0,), dtype=torch.int32, device=dets.device))
             nums.append(torch.zeros((len(chunk),), dtype=torch.int32, device=dets.device))
         else:
-            k, m = nms_batched_raw(dets[off:off + n], chunk, thresh)
+            k, m = nms_batched_raw(dets[off:off + n], chunk, thresh, cython)
             keeps.append(k[:n]); nums.append(m)
         off += n
     return torch.cat(keeps), torch.cat(nums)

@@ -3,22 +3,28 @@
 
 `generate_proposals.py:161` and `core/test.py:764` call `box_utils.nms(dets, thresh)` with numpy arrays; re-pointing
 that name at this function (`install_reference_aliases(nms=True)` or `utils.boxes.nms = nms`) moves the O(N^2) work to
-`b200_nms` while the callers stay unchanged.  Flavour note: the device kernel keeps the reference CUDA kernel's
-`IoU > thresh` test and fused IoU arithmetic (lib/model/nms/src/nms_cuda_kernel.cu:31-39), the Cython routine uses
-`>=` (lib/utils/cython_nms.pyx:83-84); they differ only on pairs whose IoU is within one ulp of the threshold.
+the device while the callers stay unchanged.  Flavour note: this is the routine the reference calls there,
+cython_nms.nms (lib/utils/cython_nms.pyx:37-87): both box areas rounded on their own, IoU = inter / ((area_i + area_j) -
+inter) in float32, suppress when IoU >= float32(thresh).  It runs as one problem of `b200_nms_batched_cython`.  The
+proposal layer of this package (modeling/generate_proposals.py) and `nms_gpu` keep the reference CUDA kernel's fused
+area and `IoU > thresh` instead (lib/model/nms/src/nms_cuda_kernel.cu:31-39); the two differ on pairs whose IoU lies
+within about one ulp of the threshold, for example integer boxes whose IoU is exactly 0.5 or 7/10.
+
+Tied scores: the reference orders by `scores.argsort()[::-1]`, which is not stable, so among boxes with equal scores its
+order is arbitrary; here they go lower index first.  The results differ only where tied boxes overlap each other.
 """
 import numpy as np
 import torch
 
-from ..model.nms.nms_gpu import nms_gpu
+from .. import ops
 
 
 def nms(dets, thresh):
     """Classic greedy NMS.  Returns the kept row indices in ascending order, like cython_nms.nms
-    (`np.where(suppressed == 0)[0]`, lib/utils/cython_nms.pyx:87)."""
+    (`np.where(suppressed == 0)[0]`, lib/utils/cython_nms.pyx:87).  Up to ~13 800 rows (b200_nms_batched_cython)."""
     if dets.shape[0] == 0:
         return []
     dets = np.ascontiguousarray(dets, dtype=np.float32)
-    order = np.argsort(-dets[:, 4], kind="stable")                  # nms_gpu expects score-sorted rows
-    keep = nms_gpu(torch.from_numpy(dets[order]).cuda(), float(thresh)).view(-1).cpu().numpy()
-    return np.sort(order[keep]).astype(np.int64)
+    order = np.argsort(-dets[:, 4], kind="stable")                  # the batched NMS expects score-sorted rows
+    keep, num = ops.nms_batched_raw(torch.from_numpy(dets[order]).cuda(), [dets.shape[0]], float(thresh), cython=True)
+    return np.sort(order[keep[:int(num[0])].cpu().numpy()]).astype(np.int64)

@@ -200,11 +200,18 @@ B200_API size_t b200_nms_batched_workspace_bytes(const int* counts_host, int num
 B200_API int b200_nms_batched(const float* boxes_dev, const int* counts_host, int num_problems, int boxes_dim,
                               float nms_overlap_thresh, int* keep_out_dev, int* num_out_dev, void* workspace,
                               size_t workspace_bytes, b200_stream_t stream);
+/* The same with the IoU test of the reference's Cython NMS (lib/utils/cython_nms.pyx:37-87), which its test-time
+ * post-processing calls per class: both box areas rounded on their own, IoU = inter / ((Sa + Sb) - inter), suppress on
+ * IoU >= thresh (b200_nms / b200_nms_batched: the reference CUDA kernel's fused area and IoU > thresh).  The kept indices
+ * are those of cython_nms.nms on the same score-sorted rows.  Workspace: b200_nms_batched_workspace_bytes. */
+B200_API int b200_nms_batched_cython(const float* boxes_dev, const int* counts_host, int num_problems, int boxes_dim,
+                                     float nms_overlap_thresh, int* keep_out_dev, int* num_out_dev, void* workspace,
+                                     size_t workspace_bytes, b200_stream_t stream);
 
 /* ---- test-time detection post-processing (SURVEY.md 8f N3) ------------------------------------------------------
  * The per-class problems of lib/core/test.py:732-790 (box_results_with_nms_and_limit), batched like b200_nms_batched:
  * problem p = the detections of one class, counts_host[p] rows of [x1, y1, x2, y2, score] stored back to back
- * (1 <= num_problems <= 128).  Classic NMS goes through b200_nms_batched.
+ * (1 <= num_problems <= 128).  Classic NMS goes through b200_nms_batched_cython.
  * b200_soft_nms_batched: lib/utils/cython_nms.pyx:98-203 step for step (method 1 linear, 2 gaussian, else hard), IN PLACE:
  *   afterwards problem p's first num_out_dev[p] rows are its surviving detections with decayed scores, in the
  *   reference's output order, and inds_out_dev holds their original row indices (relative to the problem).
