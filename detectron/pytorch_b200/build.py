@@ -69,8 +69,7 @@ def build(force=False, verbose=False):
     nvcc = find_nvcc()
     if nvcc is None:
         raise RuntimeError("nvcc not found: cannot build libb200_roi_ops.so (set $NVCC)")
-    extra = os.environ.get("B200_NVCC_EXTRA", "").split()       # e.g. -DB200_FWD_TIMING for tools/fwd_phase_probe.py
-    cmd = [nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-I", INCLUDE, "-o", LIB_PATH + ".tmp"] + sources()
+    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-I", INCLUDE, "-o", LIB_PATH + ".tmp"] + sources()
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if verbose or res.returncode != 0:
         sys.stderr.write(res.stdout)

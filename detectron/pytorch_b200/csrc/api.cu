@@ -9,8 +9,7 @@ namespace b200 {
 unsigned long long g_launch_count = 0;
 
 static const char* const kOptionNames[kNumOptions] = {"B200_ROI_ALIGN_PATH", "B200_ROI_ALIGN_BWD_PATH", "B200_ROI_ALIGN_BWD_CPL",
-                                                      "B200_FWD_ZERO", "B200_NMS_SCAN", "B200_STREAM_STAGE", "B200_STREAM_PHASES",
-                                                      "B200_FPN_PATH", "B200_STRIP_ROWCOST", "B200_STRIP_PDL", "B200_BWD_TRCH"};
+                                                      "B200_NMS_SCAN"};
 static int g_options[kNumOptions];
 static std::once_flag g_options_once;
 
@@ -49,14 +48,10 @@ size_t roi_crop_backward_workspace_bytes(int, int, int, int, int, int, int);
 size_t nms_workspace_bytes(int);
 int proposal_decode(const float*, const float*, const long long*, const float*, int, int, int, int, float, float, float, float, float*, int*, cudaStream_t);
 size_t roi_align_tiled_workspace_bytes(int, int, int, int, int, int, int);
-void roi_align_tiled_set_timing_buffer(unsigned long long*);
 void nms_set_timing_buffer(unsigned long long*);
 void roi_align_stream_set_debug_buffer(unsigned long long*);
 int roi_align_forward_tiled(const float*, float, int, int, int, int, int, int, int, int, const float*, float*, const int*, void*, size_t, cudaStream_t);
 size_t roi_align_stream_workspace_bytes(int, int, int, int, int, int, int);
-size_t roi_align_stream_fpn_workspace_bytes(int, const int*, const int*, int, int, int, int, int);
-int roi_align_forward_stream_fpn(int, const float* const*, const int*, const int*, const float*, const int*, int, int, int, int, int, int,
-                                 const float*, float*, const int*, void*, size_t, cudaStream_t);
 int roi_align_forward_stream(const float*, float, int, int, int, int, int, int, int, int, const float*, float*, const int*, void*, size_t, cudaStream_t);
 size_t roi_align_strip_workspace_bytes(int, int, int, int, int, int, int);
 size_t roi_align_strip_fpn_workspace_bytes(int, const int*, const int*, int, int, int, int, int);
@@ -96,6 +91,9 @@ static int forward_path_mode() {
     if (e == 'q') return 4;
     return 0;
 }
+
+// The pyramid call (b200_roi_align_forward_fpn) runs the quad strips: in auto mode and under B200_ROI_ALIGN_PATH=quad.
+static bool fpn_fused(int mode) { return mode == 0 || mode == 4; }
 
 static size_t forward_workspace_bytes(int mode, int N, int R, int H, int W, int PH, int PW, int sr) {
     if (mode == 1) return 0;
@@ -186,9 +184,8 @@ unsigned long long b200_roi_ops_launch_count(void) { return g_launch_count; }
 int b200_roi_ops_set_option(const char* name, const char* value) { return option_set(name, value); }
 
 void b200_roi_ops_debug_timing_buffer(void* device_u64x16) {
-    roi_align_tiled_set_timing_buffer((unsigned long long*)device_u64x16);
     nms_set_timing_buffer((unsigned long long*)device_u64x16);
-    roi_align_stream_set_debug_buffer((unsigned long long*)device_u64x16);      // -DB200_STREAM_DEBUG builds only
+    roi_align_stream_set_debug_buffer((unsigned long long*)device_u64x16);      // watchdog records of the streaming-strip path
     roi_align_strip_set_debug_buffer((unsigned long long*)device_u64x16);       // watchdog records of the quad-strip path
 }
 
@@ -219,19 +216,19 @@ int b200_roi_align_forward_indexed(const float* bottom_data, float spatial_scale
         const int rc = roi_align_forward_stream(bottom_data, spatial_scale, batch_size, num_rois, height, width, channels,
                                                 aligned_height, aligned_width, sampling_ratio, bottom_rois, top_data, top_rows,
                                                 workspace, workspace_bytes, (cudaStream_t)stream);
-        if (rc != 1000) return rc;
+        if (rc != kPathDeclined) return rc;
     }
     if (workspace != nullptr && (mode == 4 || (mode == 0 && pays))) {
         const int rc = roi_align_forward_strip(bottom_data, spatial_scale, batch_size, num_rois, height, width, channels,
                                                aligned_height, aligned_width, sampling_ratio, bottom_rois, top_data, top_rows,
                                                workspace, workspace_bytes, (cudaStream_t)stream);
-        if (rc != 1000) return rc;
+        if (rc != kPathDeclined) return rc;
     }
     if (workspace != nullptr && (mode == 2 || (mode == 0 && pays))) {
         const int rc = roi_align_forward_tiled(bottom_data, spatial_scale, batch_size, num_rois, height, width, channels,
                                                aligned_height, aligned_width, sampling_ratio, bottom_rois, top_data, top_rows,
                                                workspace, workspace_bytes, (cudaStream_t)stream);
-        if (rc != 1000) return rc;
+        if (rc != kPathDeclined) return rc;
     }
     return roi_align_forward_generic(bottom_data, spatial_scale, batch_size, num_rois, height, width, channels,
                                      aligned_height, aligned_width, sampling_ratio, bottom_rois, top_data, top_rows,
@@ -292,14 +289,14 @@ int b200_roi_align_backward_indexed(const float* top_diff, const int* top_rows, 
         const int rc = roi_align_backward_rows(top_diff, spatial_scale, batch_size, num_rois, height, width, channels,
                                                aligned_height, aligned_width, sampling_ratio, bottom_rois, bottom_diff,
                                                top_rows, workspace, workspace_bytes, (cudaStream_t)stream);
-        if (rc != 1000) return rc;
+        if (rc != kPathDeclined) return rc;
         path = 2;                                   // workspace too small for the gather path: try the NHWC one
     }
     if (path == 2) {
         const int rc = roi_align_backward_nhwc(top_diff, spatial_scale, batch_size, num_rois, height, width, channels,
                                                aligned_height, aligned_width, sampling_ratio, bottom_rois, bottom_diff,
                                                top_rows, workspace, workspace_bytes, (cudaStream_t)stream);
-        if (rc != 1000) return rc;
+        if (rc != kPathDeclined) return rc;
     }
     return roi_align_backward_generic(top_diff, spatial_scale, batch_size, num_rois, height, width, channels,
                                       aligned_height, aligned_width, sampling_ratio, bottom_rois, bottom_diff, top_rows,
@@ -427,14 +424,9 @@ int b200_nms(const float* boxes_dev, int boxes_num, int boxes_dim, float nms_ove
 
 size_t b200_roi_align_fpn_workspace_bytes(int num_levels, const int* heights_host, const int* widths_host, int batch_size, int num_rois,
                                           int aligned_height, int aligned_width, int sampling_ratio) {
-    if (num_levels < 1 || !heights_host || !widths_host || batch_size <= 0 || num_rois <= 0 || forward_path_mode() == 1 || forward_path_mode() == 2 ||
-        option_get(kOptFpnPath) == 'l')
-        return 0;
-    const size_t a = roi_align_stream_fpn_workspace_bytes(num_levels, heights_host, widths_host, batch_size, num_rois, aligned_height,
-                                                          aligned_width, sampling_ratio);
-    const size_t b = forward_path_mode() == 3 ? 0 : roi_align_strip_fpn_workspace_bytes(num_levels, heights_host, widths_host, batch_size, num_rois,
-                                                                                        aligned_height, aligned_width, sampling_ratio);
-    return a > b ? a : b;
+    if (num_levels < 1 || !heights_host || !widths_host || batch_size <= 0 || num_rois <= 0 || !fpn_fused(forward_path_mode())) return 0;
+    return roi_align_strip_fpn_workspace_bytes(num_levels, heights_host, widths_host, batch_size, num_rois, aligned_height, aligned_width,
+                                               sampling_ratio);
 }
 
 int b200_roi_align_forward_fpn(int num_levels, const float* const* bottom_data_host, const int* heights_host, const int* widths_host,
@@ -448,8 +440,8 @@ int b200_roi_align_forward_fpn(int num_levels, const float* const* bottom_data_h
     if (level_roi_begin_host[0] != 0 || level_roi_begin_host[num_levels] != num_rois) return B200_ROI_EINVAL;
     for (int l = 0; l < num_levels; ++l)
         if (!bottom_data_host[l] || level_roi_begin_host[l + 1] < level_roi_begin_host[l]) return B200_ROI_EINVAL;
-    int rc = 1000;
-    if (forward_path_mode() != 3) {
+    int rc = kPathDeclined;
+    if (fpn_fused(forward_path_mode())) {
         // Levels that TMA can stage (W % 4 == 0, 16-byte aligned base) and levels that need the cp.async producers (FPN P5 of an
         // 800 x 1333 image: W = 42) go to separate launch sequences: runs of consecutive levels of the same kind, each over its
         // own contiguous range of the level-major RoIs.  The workspace is reused (stream order).
@@ -471,9 +463,9 @@ int b200_roi_align_forward_fpn(int num_levels, const float* const* bottom_data_h
             }
             l0 = l1;
         }
-        if (rc != B200_ROI_OK && rc != 1000) return rc;
+        if (rc != B200_ROI_OK && rc != kPathDeclined) return rc;
     }
-    return rc == 1000 ? B200_ROI_EWORKSPACE : rc;
+    return rc == kPathDeclined ? B200_ROI_EWORKSPACE : rc;
 }
 
 size_t b200_nms_batched_workspace_bytes(const int* counts_host, int num_problems) {
@@ -489,7 +481,7 @@ static int nms_batched_entry(const float* boxes_dev, const int* counts_host, int
     if (total > 0 && (!boxes_dev || !keep_out_dev)) return B200_ROI_EINVAL;
     const int rc = nms_batched(boxes_dev, counts_host, num_problems, boxes_dim, nms_overlap_thresh, cython, keep_out_dev, num_out_dev,
                                workspace, workspace_bytes, (cudaStream_t)stream);
-    return rc == 1000 ? B200_ROI_EINVAL : rc;
+    return rc == kPathDeclined ? B200_ROI_EINVAL : rc;
 }
 
 int b200_nms_batched(const float* boxes_dev, const int* counts_host, int num_problems, int boxes_dim, float nms_overlap_thresh,
@@ -539,7 +531,7 @@ int b200_topk_batched(const float* const* scores_dev_ptrs_host, const int* num_a
     if (total > 0 && (!order_out_dev || !scores_out_dev)) return B200_ROI_EINVAL;
     const int rc = topk_batched(scores_dev_ptrs_host, num_anchors_host, num_cells_host, k_host, num_problems, order_out_dev, scores_out_dev,
                                 workspace, workspace_bytes, (cudaStream_t)stream);
-    return rc == 1000 ? B200_ROI_EWORKSPACE : rc;
+    return rc == kPathDeclined ? B200_ROI_EWORKSPACE : rc;
 }
 
 int b200_bbox_overlaps(const float* boxes_dev, int num_boxes, const float* query_boxes_dev, int num_query, float* overlaps_out_dev,

@@ -17,22 +17,19 @@ inline int finish_launch(int n_launches = 1) {
 
 constexpr int kNumSMs = 132;   // H100 SXM
 
+// Status of a fast path that does not apply to the shape or workspace it was given: the caller falls back to another path.
+// Neither B200_ROI_OK, a negative B200_ROI_E* code nor a CUDA runtime error (those stop at cudaErrorUnknown = 999).
+constexpr int kPathDeclined = 1000;
+
 // ---- dispatch switches -------------------------------------------------------------------------
-// A/B and test overrides of the path selection.  Each switch is read from the environment ONCE (first use) and can
-// be changed afterwards through b200_roi_ops_set_option() -- the hot path never calls getenv().
+// Test overrides of the path selection, which otherwise follows the shape.  Each switch is read from the environment ONCE
+// (first use) and can be changed afterwards through b200_roi_ops_set_option() -- the hot path never calls getenv().
 // The value is the first character of the string ('\0' = auto / default).
 enum Option {
     kOptFwdPath = 0,      // B200_ROI_ALIGN_PATH      = auto | generic | tiled | stream | quad (auto: stream first, then quad; api.cu)
     kOptBwdPath,          // B200_ROI_ALIGN_BWD_PATH  = auto | generic | nhwc | rows
     kOptBwdCpl,           // B200_ROI_ALIGN_BWD_CPL   = 4 | 2
-    kOptFwdZero,          // B200_FWD_ZERO            = dense | bins
     kOptNmsScan,          // B200_NMS_SCAN            = resolver | simple
-    kOptStreamStage,      // B200_STREAM_STAGE        = async (cp.async) | regs (LDG -> registers -> STS)
-    kOptStreamPhases,     // B200_STREAM_PHASES       = all | prepass (timing probe: the main kernel is not launched)
-    kOptFpnPath,          // B200_FPN_PATH            = fused (one launch sequence over the level table) | levels (per-level calls)
-    kOptStripRowCost,     // B200_STRIP_ROWCOST       = 0..9: cost of streaming a row in the partition model = 8 d + 4 (default 24)
-    kOptStripPdl,         // B200_STRIP_PDL           = 1 | 0: programmatic dependent launch of the main kernel behind the prepass
-    kOptBwdTrCh,          // B200_BWD_TRCH            = 2 (256) | 1 (128) | 6 (64): channels per CTA of the backward's dY transpose
     kNumOptions
 };
 int option_get(Option which);

@@ -511,7 +511,7 @@ int nms_batched(const float* boxes, const int* counts, int num_problems, int dim
         const size_t sm_r = sizeof(u64) * ((size_t)r * cb * kNmsTile + 4 * (size_t)cb) + 16;
         if (sm_r <= 224 * 1024) { reach = r; smem_res = sm_r; break; }
     }
-    if (reach == 0) return 1000;                        // a problem too large for the pipelined scan: the caller loops over b200_nms
+    if (reach == 0) return kPathDeclined;                        // a problem too large for the pipelined scan: the caller loops over b200_nms
     u64* ws = (u64*)workspace;
     if (nb.tile_off[num_problems] > 0)
         (cython ? nms_mask_batched_kernel<true> : nms_mask_batched_kernel<false>)<<<(unsigned)nb.tile_off[num_problems], kNmsTile, 0, stream>>>(

@@ -141,19 +141,19 @@ size_t roi_align_bwd_nhwc_workspace_bytes(int N, int C, int H, int W) {
     return ((size_t)N * C * H * W * sizeof(float) + 255) / 256 * 256;
 }
 
-// returns 1000 when the path does not apply (caller falls back to the generic scalar-atomic kernel)
+// returns kPathDeclined when the path does not apply (caller falls back to the generic scalar-atomic kernel)
 int roi_align_backward_nhwc(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
                             const float* rois, float* bottom_diff, const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-    if (sr < 1 || sr > 4 || PH * sr > kBwAxisMax || PW * sr > kBwAxisMax) return 1000;
-    if (workspace == nullptr || workspace_bytes < roi_align_bwd_nhwc_workspace_bytes(N, C, H, W)) return 1000;
-    if (R <= 0 || C <= 0 || N <= 0) return 1000;
+    if (sr < 1 || sr > 4 || PH * sr > kBwAxisMax || PW * sr > kBwAxisMax) return kPathDeclined;
+    if (workspace == nullptr || workspace_bytes < roi_align_bwd_nhwc_workspace_bytes(N, C, H, W)) return kPathDeclined;
+    if (R <= 0 || C <= 0 || N <= 0) return kPathDeclined;
     float* scratch = (float*)workspace;
     cudaError_t err = cudaMemsetAsync(scratch, 0, sizeof(float) * (size_t)N * C * H * W, stream);
     if (err != cudaSuccess) return (int)err;
     const int chunk = C < kBwChunk ? C : kBwChunk;
     const int c_pad = ((chunk + 3) / 4) * 4 + 4;
     const size_t smem = sizeof(float) * (size_t)PH * PW * c_pad;
-    if (smem > 200 * 1024) return 1000;
+    if (smem > 200 * 1024) return kPathDeclined;
     dim3 grid(R, (C + kBwChunk - 1) / kBwChunk);
 #define B200_LAUNCH_BW(SRV)                                                                                              \
     do {                                                                                                                 \

@@ -399,7 +399,7 @@ static int launch_rows(const RowsPlan& p, unsigned char* ws, float* dx, int N, i
     int per_sm = 0;
     err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WARPS * 32, smem);
     if (err != cudaSuccess) return (int)err;
-    if (per_sm < 1) return 1000;
+    if (per_sm < 1) return kPathDeclined;
     const int items = N * H * p.tiles_x * (C / (32 * CPL));
     const int warps_needed = items;
     int grid = kNumSMs * per_sm;
@@ -411,21 +411,19 @@ static int launch_rows(const RowsPlan& p, unsigned char* ws, float* dx, int N, i
     return B200_ROI_OK;
 }
 
-// returns 1000 when the path does not apply (caller falls back to another backward path)
+// returns kPathDeclined when the path does not apply (caller falls back to another backward path)
 int roi_align_backward_rows(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
                             const float* rois, float* bottom_diff, const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     RowsPlan p;
-    if (!rows_plan(N, R, C, H, W, PH, PW, sr, &p)) return 1000;
-    if (workspace == nullptr || workspace_bytes < p.ws_bytes) return 1000;
+    if (!rows_plan(N, R, C, H, W, PH, PW, sr, &p)) return kPathDeclined;
+    if (workspace == nullptr || workspace_bytes < p.ws_bytes) return kPathDeclined;
     unsigned char* ws = (unsigned char*)workspace;
     const int bins = PH * PW;
     int tr_ch = kTransposeChannelsMax;                       // as many channels per CTA as fit ~100 KB (two CTAs per SM)
-    const int tr_opt = option_get(kOptBwdTrCh);
-    if (tr_opt == '1') tr_ch = 128; else if (tr_opt == '6') tr_ch = 64;
     while (tr_ch > 32 && (size_t)tr_ch * (bins | 1) * sizeof(float) > 100 * 1024) tr_ch >>= 1;
     if (tr_ch > C) tr_ch = (C + 31) / 32 * 32;
     const size_t smem_tr = (size_t)tr_ch * (bins | 1) * sizeof(float);
-    if (smem_tr > 200 * 1024) return 1000;
+    if (smem_tr > 200 * 1024) return kPathDeclined;
     cudaError_t err = cudaSuccess;
     if (smem_tr > 48 * 1024) err = cudaFuncSetAttribute(roi_align_bwd_rows_tables, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tr);
     if (err != cudaSuccess) return (int)err;

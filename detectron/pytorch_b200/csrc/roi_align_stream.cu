@@ -36,10 +36,7 @@ namespace b200 {
 
 namespace {
 
-#ifndef B200_STREAM_CWARPS
-#define B200_STREAM_CWARPS 16
-#endif
-constexpr int kConsumerWarps = B200_STREAM_CWARPS;
+constexpr int kConsumerWarps = 16;
 constexpr int kProducerWarps = 4;
 constexpr int kStreamThreads = 32 * (kConsumerWarps + kProducerWarps);
 constexpr int kFragBins = 8;                                  // bins per fragment (one flush)
@@ -54,41 +51,6 @@ constexpr int kScanCap = 6144;                                // keys whose cost
 constexpr unsigned kSmemBudget = 227u * 1024u;
 
 typedef unsigned long long u64;
-
-// Debug build (-DB200_STREAM_DEBUG, tools/stream_debug.py): every warp leaves progress markers in a HOST-pinned buffer
-// registered with b200_roi_ops_debug_timing_buffer(), so that they survive a trap.  Compiled out by default.
-#ifdef B200_STREAM_DEBUG
-__device__ u64* g_stream_dbg = nullptr;
-#define SDBG(slot, val)                                                                                      \
-    do {                                                                                                     \
-        if (g_stream_dbg != nullptr && (threadIdx.x & 31) == 0) {                                            \
-            volatile u64* dbg_p = g_stream_dbg + ((size_t)blockIdx.x * 17 + (threadIdx.x >> 5)) * 8;        \
-            dbg_p[slot] = (u64)(val);                                                                        \
-            __threadfence_system();                                                                          \
-        }                                                                                                    \
-    } while (0)
-#else
-#define SDBG(slot, val) do { } while (0)
-#endif
-
-// Timing build (-DB200_STREAM_TIMING, tools/stream_timing.py): every warp leaves SM clock stamps and wait-cycle totals in a
-// DEVICE buffer registered the same way ([CTA][warp][8] u64).  Compiled out by default.
-#ifdef B200_STREAM_TIMING
-__device__ u64* g_stream_tim = nullptr;
-#define STIM_DECL u64 stim_wait = 0, stim_n0 = 0, stim_n1 = 0, stim_first = 0, stim_comp = 0, stim_c0 = 0
-#define STIM_CLOCK() ((u64)clock64())
-#define STIM(slot, val)                                                                                      \
-    do {                                                                                                     \
-        if (g_stream_tim != nullptr && (threadIdx.x & 31) == 0)                                              \
-            g_stream_tim[((size_t)blockIdx.x * (kConsumerWarps + kProducerWarps) + (threadIdx.x >> 5)) * 8 + (slot)] = (u64)(val); \
-    } while (0)
-#define STIM_DO(stmt) do { stmt; } while (0)
-#else
-#define STIM_DECL
-#define STIM_CLOCK() 0ull
-#define STIM(slot, val) do { } while (0)
-#define STIM_DO(stmt) do { } while (0)
-#endif
 
 constexpr int kMaxLevels = 6;                                 // feature maps served by one launch (FPN: P2..P6)
 constexpr int kMaxCols = 96;                                  // strip columns (level, image, strip) of one launch
@@ -436,12 +398,7 @@ __device__ __forceinline__ bool mbar_try_wait(unsigned bar, unsigned parity) {
 }
 // try_wait suspends the thread in hardware for a bounded time per attempt.  A wait that is still pending after 2^20
 // attempts (seconds) is a protocol bug: trap (surfaces as a launch failure) instead of hanging the GPU.
-#ifdef B200_STREAM_WATCH
-#define WCTX(expr) (expr)
-#else
-#define WCTX(expr) 0ull
-#endif
-__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity, unsigned tag = 0u, u64 ctx0 = 0ull, u64 ctx1 = 0ull) {
+__device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity, unsigned tag = 0u) {
     if (mbar_try_wait(bar, parity)) return;
     int spins = 0;
     while (!mbar_try_wait(bar, parity)) {
@@ -450,16 +407,9 @@ __device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity, unsigne
             // half way to the trap: say who is stuck on what (host-pinned buffer registered by the caller, else nothing)
             g_stream_dead[blockIdx.x * 32 + (threadIdx.x >> 5)] =
                 0xDEAD000000000000ull | ((u64)tag << 16) | ((u64)parity << 8) | (u64)((bar >> 3) & 0xff);
-#ifdef B200_STREAM_WATCH
-            g_stream_dead[kNumSMs * 32 + (blockIdx.x * 32 + (threadIdx.x >> 5)) * 2] = ctx0;
-            g_stream_dead[kNumSMs * 32 + (blockIdx.x * 32 + (threadIdx.x >> 5)) * 2 + 1] = ctx1;
-#endif
             __threadfence_system();
         }
-        if (spins > (1 << 20)) {
-            SDBG(6, 0xDEAD000000000000ull | ((u64)tag << 16) | ((u64)parity << 8) | (u64)((bar >> 3) & 0xff));
-            __trap();
-        }
+        if (spins > (1 << 20)) __trap();
     }
 }
 // 4-byte cp.async (LDGSTS): global -> shared without registers.
@@ -566,64 +516,40 @@ __device__ __forceinline__ float sample_val(const Taps& t, u64 hyhy, u64 lyly, u
 }
 
 // Stage row y of one (image, strip, channel group) into a ring slot: M full 32-column chunks per channel
-// (lane = column: 128-byte coalesced) plus the last column x = 32 M for all channels at once (lane = channel).
-// ASYNC: 4-byte cp.async; otherwise LDG -> registers -> STS in batches of 8 channels.
-template <int M, bool ASYNC>
+// (lane = column: 128-byte coalesced) plus the last column x = 32 M for all channels at once (lane = channel),
+// with 4-byte cp.async.
+template <int M>
 __device__ __forceinline__ void stage_row(const float* __restrict__ src_row, size_t plane, unsigned dst, int xw, int cvalid, int lane) {
     // src_row: (channel 0, row y, column x0); xw = number of valid columns from x0; cvalid = number of real channels
     constexpr int SX = 32 * M + 1;
-    if (ASYNC) {
-        if (cvalid == 32 && xw >= SX) {                       // interior: no predicates, constant offsets
-            const float* sc = src_row + lane;
-            const unsigned d = dst + (unsigned)lane * 4u;
+    if (cvalid == 32 && xw >= SX) {                           // interior: no predicates, constant offsets
+        const float* sc = src_row + lane;
+        const unsigned d = dst + (unsigned)lane * 4u;
 #pragma unroll 8
-            for (int c = 0; c < 32; ++c) {
+        for (int c = 0; c < 32; ++c) {
 #pragma unroll
-                for (int m = 0; m < M; ++m) cp_async4(d + (unsigned)(c * SX + 32 * m) * 4u, sc + 32 * m);
-                sc += plane;
-            }
-            cp_async4(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (size_t)lane * plane + 32 * M);
-        } else {
-#pragma unroll 4
-            for (int c = 0; c < 32; ++c) {
-                const bool cok = c < cvalid;
-                const float* sc = src_row + (size_t)(cok ? c : 0) * plane;
-#pragma unroll
-                for (int m = 0; m < M; ++m) {
-                    const int x = lane + 32 * m;
-                    const bool ok = cok && x < xw;
-                    cp_async4_if(dst + (unsigned)(c * SX + x) * 4u, sc + (ok ? x : 0), ok);
-                }
-            }
-            const bool ok = lane < cvalid && 32 * M < xw;
-            cp_async4_if(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (ok ? (size_t)lane * plane + 32 * M : 0), ok);
+            for (int m = 0; m < M; ++m) cp_async4(d + (unsigned)(c * SX + 32 * m) * 4u, sc + 32 * m);
+            sc += plane;
         }
+        cp_async4(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (size_t)lane * plane + 32 * M);
     } else {
-        for (int c8 = 0; c8 < 32; c8 += 8) {
-            float v[8][M];
+#pragma unroll 4
+        for (int c = 0; c < 32; ++c) {
+            const bool cok = c < cvalid;
+            const float* sc = src_row + (size_t)(cok ? c : 0) * plane;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const bool cok = c8 + j < cvalid;
-                const float* sc = src_row + (size_t)(cok ? c8 + j : 0) * plane;
-#pragma unroll
-                for (int m = 0; m < M; ++m) {
-                    const int x = lane + 32 * m;
-                    v[j][m] = (cok && x < xw) ? __ldcs(sc + x) : 0.f;
-                }
+            for (int m = 0; m < M; ++m) {
+                const int x = lane + 32 * m;
+                const bool ok = cok && x < xw;
+                cp_async4_if(dst + (unsigned)(c * SX + x) * 4u, sc + (ok ? x : 0), ok);
             }
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-#pragma unroll
-                for (int m = 0; m < M; ++m)
-                    asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + (unsigned)((c8 + j) * SX + lane + 32 * m) * 4u), "f"(v[j][m]) : "memory");
         }
         const bool ok = lane < cvalid && 32 * M < xw;
-        const float t = ok ? __ldcs(src_row + (size_t)lane * plane + 32 * M) : 0.f;
-        asm volatile("st.shared.f32 [%0], %1;" ::"r"(dst + (unsigned)(lane * SX + 32 * M) * 4u), "f"(t) : "memory");
+        cp_async4_if(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (ok ? (size_t)lane * plane + 32 * M : 0), ok);
     }
 }
 
-template <int SR, int M, bool ASYNC>
+template <int SR, int M>
 __global__ void __launch_bounds__(kStreamThreads, 1)
 roi_align_stream_fwd(const StreamArgs a) {
     constexpr int SX = 32 * M + 1;
@@ -649,9 +575,6 @@ roi_align_stream_fwd(const StreamArgs a) {
     }
     __syncthreads();
     const int L0 = __ldg(&a.piece_start[blockIdx.x]), L1 = __ldg(&a.piece_start[blockIdx.x + 1]);
-    SDBG(0, 1); SDBG(1, ((u64)(unsigned)L0 << 32) | (unsigned)L1);
-    STIM_DECL;
-    STIM(0, STIM_CLOCK()); STIM(7, ((u64)(unsigned)L0 << 32) | (unsigned)L1);
 
     if (warp >= kConsumerWarps) {
         // =============================== producers ===============================
@@ -663,7 +586,6 @@ roi_align_stream_fwd(const StreamArgs a) {
         for (int L = L0; L < L1;) {
             const Item it = decode_item(L, L1, a, lane);
             L += it.yb - it.ya;
-            SDBG(2, ((u64)it.ya << 48) | ((u64)it.yb << 32) | ((u64)it.yhi << 16) | (u64)(it.e1 - it.e0));
             if (it.e1 <= it.e0) continue;
             int slot = it.ya % a.K;
             const StreamLevel& lv = a.lv[it.lvl];
@@ -681,17 +603,11 @@ roi_align_stream_fwd(const StreamArgs a) {
                 // overtake the warp that stages it and overwrite use k - 2.  Having seen use k - 2 released here, the test
                 // for use k can only be one phase ahead (measured: K = 15, four producers, rows 2 and 17 of one item).
                 const unsigned full = bars + 8u * slot, empty = bars + 8u * (kMaxSlots + slot);
-                STIM_DO(stim_n1 = STIM_CLOCK());
-                mbar_wait(empty, (ephase >> slot) & 1u, 0x1000u + (unsigned)y,
-                          WCTX(((u64)it.ya << 48) | ((u64)it.yb << 32) | ((u64)it.yhi << 16) | (u64)(it.lvl << 12) | (u64)(it.g << 8) | (u64)it.s),
-                          WCTX(((u64)ephase << 32) | (u64)(unsigned)(L - (it.yb - it.ya))));
-                STIM_DO(stim_wait += STIM_CLOCK() - stim_n1);
+                mbar_wait(empty, (ephase >> slot) & 1u, 0x1000u + (unsigned)y);
                 if (turn == pw) {
-                    STIM_DO(++stim_n0; if (!stim_first) stim_first = STIM_CLOCK());
-                    SDBG(4, ((u64)y << 32) | (u64)slot);
-                    stage_row<M, ASYNC>(src, plane, ring + (unsigned)slot * (unsigned)RB, xw, cvalid, lane);
-                    if (slot == 0) stage_row<M, ASYNC>(src, plane, ring + (unsigned)a.K * (unsigned)RB, xw, cvalid, lane);   // mirror
-                    if (ASYNC) cp_async_arrive(full); else mbar_arrive(full);
+                    stage_row<M>(src, plane, ring + (unsigned)slot * (unsigned)RB, xw, cvalid, lane);
+                    if (slot == 0) stage_row<M>(src, plane, ring + (unsigned)a.K * (unsigned)RB, xw, cvalid, lane);   // mirror
+                    cp_async_arrive(full);
                 }
                 ephase ^= 1u << slot;
                 if (++slot == a.K) slot = 0;
@@ -699,8 +615,6 @@ roi_align_stream_fwd(const StreamArgs a) {
                 src += rowlen;
             }
         }
-        SDBG(0, 9);
-        STIM(1, stim_first); STIM(2, STIM_CLOCK()); STIM(3, stim_wait); STIM(4, stim_n0);
         return;
     }
 
@@ -716,9 +630,7 @@ roi_align_stream_fwd(const StreamArgs a) {
     for (int L = L0; L < L1;) {
         const Item it = decode_item(L, L1, a, lane);
         L += it.yb - it.ya;
-        SDBG(2, ((u64)it.ya << 48) | ((u64)it.yb << 32) | ((u64)it.yhi << 16) | (u64)(it.e1 - it.e0));
         if (it.e1 <= it.e0) continue;
-        SDBG(0, 2);
         const unsigned lc = lane_base - (unsigned)(it.s * a.WX) * 4u;
         int acq = it.ya, rel = it.ya;
         int acq_slot = it.ya % a.K, rel_slot = acq_slot;
@@ -727,11 +639,7 @@ roi_align_stream_fwd(const StreamArgs a) {
         // phase bits in step with the producers)
         auto acquire_to = [&](int row_end, unsigned tag) {
             while (acq < row_end) {
-                STIM_DO(stim_n1 = STIM_CLOCK());
-                mbar_wait(bars + 8u * acq_slot, (fphase >> acq_slot) & 1u, tag + (unsigned)acq,
-                          WCTX(((u64)it.ya << 48) | ((u64)it.yb << 32) | ((u64)it.yhi << 16) | (u64)(it.lvl << 12) | (u64)(it.g << 8) | (u64)it.s),
-                          WCTX(((u64)fphase << 32) | ((u64)(unsigned)rel << 16) | (u64)(unsigned)row_end));
-                STIM_DO(stim_wait += STIM_CLOCK() - stim_n1);
+                mbar_wait(bars + 8u * acq_slot, (fphase >> acq_slot) & 1u, tag + (unsigned)acq);
                 fphase ^= 1u << acq_slot;
                 ++acq;
                 if (++acq_slot == a.K) acq_slot = 0;
@@ -791,8 +699,6 @@ roi_align_stream_fwd(const StreamArgs a) {
                 release_to(acq);
             }
             acquire_to(end, 0x2800u);                           // rows [key, end) must be resident
-            SDBG(3, ((u64)cur.x << 32) | (u64)cur.y);
-            STIM_DO(++stim_n0; stim_c0 = STIM_CLOCK(); if (!stim_first) stim_first = stim_c0);
             const uint4 yA = lds128(tbuf + 16 * 16);
             uint4 yB = yA;
             if (SR == 2) yB = lds128(tbuf + 17 * 16);
@@ -863,22 +769,17 @@ roi_align_stream_fwd(const StreamArgs a) {
                 }
             }
             __syncwarp();
-            STIM_DO(stim_comp += STIM_CLOCK() - stim_c0);
             e = e_next;
         }
         // item tail: nothing more to read -- give back what is held, then pass the remaining rows through one by one
         // (a warp that held rows while waiting for later ones could starve the producers of slots)
-        SDBG(0, 5);
         release_to(acq);
         while (acq < it.yhi) {
             acquire_to(acq + 1, 0x3000u);
             release_to(acq);
         }
         __syncwarp();
-        SDBG(0, 6);
     }
-    SDBG(0, 9);
-    STIM(1, stim_first); STIM(2, STIM_CLOCK()); STIM(3, stim_wait); STIM(4, stim_n0); STIM(5, stim_comp);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -982,12 +883,10 @@ bool stream_device_info(int* sm_count) {
     if (!info[dev].ok) {
         const int max_dyn = (int)kSmemBudget;
         bool ok = cudaDeviceGetAttribute(&info[dev].sm_count, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess;
-#define B200_STREAM_ATTR(SRV, MV, AV) \
-        ok = ok && cudaFuncSetAttribute(roi_align_stream_fwd<SRV, MV, AV>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_dyn) == cudaSuccess
-        B200_STREAM_ATTR(1, 1, true); B200_STREAM_ATTR(1, 2, true); B200_STREAM_ATTR(1, 3, true);
-        B200_STREAM_ATTR(2, 1, true); B200_STREAM_ATTR(2, 2, true); B200_STREAM_ATTR(2, 3, true);
-        B200_STREAM_ATTR(1, 1, false); B200_STREAM_ATTR(1, 2, false); B200_STREAM_ATTR(1, 3, false);
-        B200_STREAM_ATTR(2, 1, false); B200_STREAM_ATTR(2, 2, false); B200_STREAM_ATTR(2, 3, false);
+#define B200_STREAM_ATTR(SRV, MV) \
+        ok = ok && cudaFuncSetAttribute(roi_align_stream_fwd<SRV, MV>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_dyn) == cudaSuccess
+        B200_STREAM_ATTR(1, 1); B200_STREAM_ATTR(1, 2); B200_STREAM_ATTR(1, 3);
+        B200_STREAM_ATTR(2, 1); B200_STREAM_ATTR(2, 2); B200_STREAM_ATTR(2, 3);
 #undef B200_STREAM_ATTR
         if (!ok) {
             (void)cudaGetLastError();
@@ -999,19 +898,7 @@ bool stream_device_info(int* sm_count) {
     return true;
 }
 
-}  // namespace
-
-void roi_align_stream_set_debug_buffer(unsigned long long* host_pinned) {
-#if defined(B200_STREAM_DEBUG)
-    cudaMemcpyToSymbol(g_stream_dbg, &host_pinned, sizeof(host_pinned));
-#elif defined(B200_STREAM_TIMING)
-    cudaMemcpyToSymbol(g_stream_tim, &host_pinned, sizeof(host_pinned));
-#else
-    cudaMemcpyToSymbol(g_stream_dead, &host_pinned, sizeof(host_pinned));      // [CTA][32] u64 watchdog records
-#endif
-}
-
-size_t roi_align_stream_fpn_workspace_bytes(int levels, const int* heights, const int* widths, int N, int R, int PH, int PW, int sr) {
+size_t stream_fpn_workspace_bytes(int levels, const int* heights, const int* widths, int N, int R, int PH, int PW, int sr) {
     StreamGeom g;
     StreamLayout lay;
     unsigned smem = 0;
@@ -1019,23 +906,20 @@ size_t roi_align_stream_fpn_workspace_bytes(int levels, const int* heights, cons
     return lay.ws_bytes;
 }
 
-size_t roi_align_stream_workspace_bytes(int N, int R, int H, int W, int PH, int PW, int sr) {
-    return roi_align_stream_fpn_workspace_bytes(1, &H, &W, N, R, PH, PW, sr);
-}
-
-// returns B200_ROI_OK when the streaming path ran; 1000 when it does not apply (caller falls back)
+// One launch sequence over the level table (a plain call is one level).  Returns B200_ROI_OK when the streaming path ran;
+// kPathDeclined when it does not apply (caller falls back).
 int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const int* heights, const int* widths, const float* scales,
                                  const int* level_roi_begin, int N, int R, int C, int PH, int PW, int sr, const float* rois, float* top,
                                  const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-    if (workspace == nullptr || C <= 0) return 1000;
-    if ((long long)N * C >= (1LL << 31) || (long long)R * C * PH * PW >= (1LL << 31)) return 1000;
+    if (workspace == nullptr || C <= 0) return kPathDeclined;
+    if ((long long)N * C >= (1LL << 31) || (long long)R * C * PH * PW >= (1LL << 31)) return kPathDeclined;
     int sm_count = 0;
-    if (!stream_device_info(&sm_count)) return 1000;
+    if (!stream_device_info(&sm_count)) return kPathDeclined;
     StreamGeom g;
     StreamLayout lay;
     unsigned smem = 0;
-    if (!stream_geometry(levels, bottoms, heights, widths, scales, level_roi_begin, N, R, C, PH, PW, sr, sm_count, &g, &lay, &smem)) return 1000;
-    if (workspace_bytes < lay.ws_bytes) return 1000;
+    if (!stream_geometry(levels, bottoms, heights, widths, scales, level_roi_begin, N, R, C, PH, PW, sr, sm_count, &g, &lay, &smem)) return kPathDeclined;
+    if (workspace_bytes < lay.ws_bytes) return kPathDeclined;
     unsigned char* wsb = (unsigned char*)workspace;
     StreamWs ws;
     ws.ytab = (uint4*)(wsb + lay.ytab_off);
@@ -1056,7 +940,6 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
     a.C = C; a.G = g.G; a.K = g.K; a.WX = g.WX; a.PH = PH; a.PW = PW; a.ny = g.ny; a.nx = g.nx; a.L = g.L; a.Q = g.Q;
     for (int l = 0; l < kMaxLevels; ++l) a.lv[l] = g.lv[l];
     for (int c = 0; c <= kMaxCols; ++c) a.colstart[c] = g.colstart[c];
-    const bool async = option_get(kOptStreamStage) != 'r';          // B200_STREAM_STAGE=regs selects LDG -> registers -> STS (A/B)
     const int m = (g.SX - 1) / 32;
     if (sr == 1) {
         stream_count<1><<<R, kPrepThreads, 0, stream>>>(rois, g, ws);
@@ -1065,16 +948,26 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
         stream_count<2><<<R, kPrepThreads, 0, stream>>>(rois, g, ws);
         stream_fill<2><<<R, kPrepThreads, 0, stream>>>(rois, g, ws, top, row_map);
     }
-#define B200_STREAM_LAUNCH(SRV, MV, AV) roi_align_stream_fwd<SRV, MV, AV><<<g.pieces, kStreamThreads, smem, stream>>>(a)
-#define B200_STREAM_LAUNCH_M(SRV, AV) (m == 1 ? B200_STREAM_LAUNCH(SRV, 1, AV) : m == 2 ? B200_STREAM_LAUNCH(SRV, 2, AV) : B200_STREAM_LAUNCH(SRV, 3, AV))
-    if (option_get(kOptStreamPhases) == 'p') return finish_launch(2);          // timing probe: prepass only (output undefined)
-    if (sr == 1) { if (async) B200_STREAM_LAUNCH_M(1, true); else B200_STREAM_LAUNCH_M(1, false); }
-    else         { if (async) B200_STREAM_LAUNCH_M(2, true); else B200_STREAM_LAUNCH_M(2, false); }
+#define B200_STREAM_LAUNCH(SRV, MV) roi_align_stream_fwd<SRV, MV><<<g.pieces, kStreamThreads, smem, stream>>>(a)
+#define B200_STREAM_LAUNCH_M(SRV) (m == 1 ? B200_STREAM_LAUNCH(SRV, 1) : m == 2 ? B200_STREAM_LAUNCH(SRV, 2) : B200_STREAM_LAUNCH(SRV, 3))
+    if (sr == 1) B200_STREAM_LAUNCH_M(1);
+    else         B200_STREAM_LAUNCH_M(2);
 #undef B200_STREAM_LAUNCH_M
 #undef B200_STREAM_LAUNCH
     return finish_launch(3);
 }
 
+}  // namespace
+
+void roi_align_stream_set_debug_buffer(unsigned long long* host_pinned) {
+    cudaMemcpyToSymbol(g_stream_dead, &host_pinned, sizeof(host_pinned));      // [CTA][32] u64 watchdog records
+}
+
+size_t roi_align_stream_workspace_bytes(int N, int R, int H, int W, int PH, int PW, int sr) {
+    return stream_fpn_workspace_bytes(1, &H, &W, N, R, PH, PW, sr);
+}
+
+// returns B200_ROI_OK when the streaming path ran; kPathDeclined when it does not apply (caller falls back)
 int roi_align_forward_stream(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
                              const float* rois, float* top, const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     const int begin[2] = {0, R};

@@ -18,7 +18,7 @@
 //    transposer warps (rows i mod T) wait for the slot's mbarrier, pull the row through registers (LDS.128, lane = channel)
 //    and rewrite it IN PLACE as [column][channel] (STS.32, lane = channel), then publish next[t] = their first stream row
 //    that has not landed.  128 shared-memory wavefronts per row instead of >= 512 LSU cycles for 64 four-byte cp.async;
-//  * staging by cp.async (fallback: any W, e.g. FPN P5 with W = 42; B200_STREAM_STAGE=async): every producer-side warp
+//  * staging by cp.async (fallback: any W, e.g. FPN P5 with W = 42): every producer-side warp
 //    stages rows i mod kPW with 4-byte LDGSTS, lane = column (full 128-byte lines per request: the L1 tracks outstanding
 //    misses per line), the transposing write hits 8 distinct banks per returning sector (bank = 4 x + c with the 36-word
 //    pitch); a warp's rows land in order (cp.async groups of one thread) and it publishes the same next[] word;
@@ -50,27 +50,16 @@ namespace b200 {
 
 namespace {
 
-#ifndef B200_STRIP_CONSUMERS
-#define B200_STRIP_CONSUMERS 12
-#endif
-constexpr int kCW = B200_STRIP_CONSUMERS;                     // consumer warps (<= 32: their marks are read by one warp)
-#ifndef B200_STRIP_PRODUCERS
-#define B200_STRIP_PRODUCERS 4
-#endif
-constexpr int kPW = B200_STRIP_PRODUCERS;                     // producer warps (stream row i is staged by warp i % kPW)
+constexpr int kCW = 12;                                       // consumer warps (<= 32: their marks are read by one warp)
+constexpr int kPW = 4;                                        // producer warps (stream row i is staged by warp i % kPW)
+static_assert(kPW >= 2, "TMA staging needs an issuer warp and at least one transposer warp");
 constexpr int kThreads = 32 * (kCW + kPW);
 constexpr int kFragBins = 8;                                  // bins per fragment (two passes of 4)
 // bytes per staged cell (template parameter CELL of the main kernel): 128 when rows are staged by TMA (the transposer writes
 // 128 aligned bytes per column), 144 = 32 channels + 16 B pad with cp.async producers (bank = 4 x + c for the transposing write)
 constexpr int kCellTma = 128, kCellAsync = 144;
-#ifndef B200_STRIP_DEPTH
-#define B200_STRIP_DEPTH 2
-#endif
-constexpr int kDepth = B200_STRIP_DEPTH;                      // rows every producer warp keeps in flight
-#ifndef B200_STRIP_INFLIGHT
-#define B200_STRIP_INFLIGHT 8
-#endif
-constexpr int kInflight = B200_STRIP_INFLIGHT;                // TMA mode: rows issued but not yet transposed
+constexpr int kDepth = 2;                                     // rows every producer warp keeps in flight
+constexpr int kInflight = 8;                                  // TMA mode: rows issued but not yet transposed
 constexpr int kMaxLevels = 6;
 constexpr int kMaxCols = 96;
 constexpr int kAxisMaxS = 32;
@@ -79,6 +68,7 @@ constexpr int kMaxKeys = 6144;                                // CSR scan lives 
 constexpr int kMaxK = 48;
 constexpr unsigned kSmemBudget = 227u * 1024u;
 constexpr unsigned kFragCost = 10u, kPassCost = 9u;           // cost model of the partition (units ~ 10 instructions)
+constexpr unsigned kRowCost = 44u;                            // cost of streaming one row in the same units
 
 typedef unsigned long long u64;
 
@@ -96,8 +86,6 @@ struct StripGeom {
     int ny, nx;
     int SX, WX, K, cell;                                      // columns per slot (8 XO), strip core width, ring depth, bytes per cell
     int L, Q, keys, G, pieces, max_entries, cap_r;            // cap_r: fragments one RoI can have at most
-    unsigned row_cost;
-    int stop_after;                                           // timing probe (B200_STREAM_PHASES=1|2): the prepass returns after that phase
     StripLevel lv[kMaxLevels];
     int colstart[kMaxCols + 1];
 };
@@ -279,7 +267,6 @@ strip_prep(const float* __restrict__ rois, StripGeom g, StripWs ws, float* __res
         }
         if (t == 0) ws.tmpcnt[r] = batch_ok ? n : -1;
     }
-    if (g.stop_after == 1) return;
     // ---- grid barrier (the grid is sized to be resident: see the launcher)
     __syncthreads();
     if (t == 0) {
@@ -296,7 +283,7 @@ strip_prep(const float* __restrict__ rois, StripGeom g, StripWs ws, float* __res
     // ---- phase 2: exclusive prefix of the fragment histogram and of the cost, in every CTA's shared memory
     for (int k = t; k < keys; k += kPrepThreads) {
         s_pre[k] = (unsigned)__ldcg(&ws.hist[k]);
-        s_cpre[k] = (unsigned)__ldcg(&ws.cost[k]) + g.row_cost;
+        s_cpre[k] = (unsigned)__ldcg(&ws.cost[k]) + kRowCost;
     }
     __syncthreads();
     const int chunk = ((keys + kPrepThreads - 1) / kPrepThreads) | 1;     // odd: thread-strided chunks do not collide on banks
@@ -353,7 +340,7 @@ strip_prep(const float* __restrict__ rois, StripGeom g, StripWs ws, float* __res
                 const int q = lo;
                 const int kb = g.colstart[q], Hq = g.colstart[q + 1] - kb;
                 const unsigned c0 = s_cpre[kb];
-                const unsigned colsum = s_cpre[kb + Hq] - c0;                 // >= row_cost * Hq > 0
+                const unsigned colsum = s_cpre[kb + Hq] - c0;                 // >= kRowCost * Hq > 0
                 u64 rem = target - (u64)g.G * (u64)c0;
                 int gg = (int)(rem / colsum);
                 if (gg > g.G - 1) gg = g.G - 1;
@@ -368,7 +355,6 @@ strip_prep(const float* __restrict__ rois, StripGeom g, StripWs ws, float* __res
             ws.piece_start[p] = L;
         }
     }
-    if (g.stop_after == 2) return;
     // ---- phase 3: fragment records into the CSR (position = row pointer + rank); zero-fill of the elements that are
     // accumulated with red.add (the bins of the fragments that hold a split bin's first sample)
     const int bins = g.PH * g.PW;
@@ -409,26 +395,6 @@ strip_prep(const float* __restrict__ rois, StripGeom g, StripWs ws, float* __res
 // main kernel helpers
 // ------------------------------------------------------------------------------------------------
 __device__ u64* g_strip_dead = nullptr;                       // optional host-pinned watchdog records ([CTA][32] u64)
-
-// Timing build (-DB200_STRIP_TIMING, tools/strip_timing.py): every warp leaves [start ns, first work ns, end ns, wait cycles,
-// work items, busy cycles] in a DEVICE buffer registered with b200_roi_ops_debug_timing_buffer ([CTA][warp][8] u64).
-#ifdef B200_STRIP_TIMING
-__device__ u64* g_strip_tim = nullptr;
-__device__ __forceinline__ u64 gtime_ns() { u64 t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-#define TIM_DECL u64 tim_start = gtime_ns(), tim_first = 0, tim_wait = 0, tim_n = 0, tim_busy = 0, tim_c = 0
-#define TIM_DO(stmt) do { stmt; } while (0)
-#define TIM_FLUSH()                                                                                                   \
-    do {                                                                                                              \
-        if (g_strip_tim != nullptr && (threadIdx.x & 31) == 0) {                                                      \
-            u64* tp = g_strip_tim + ((size_t)blockIdx.x * (kCW + kPW) + (threadIdx.x >> 5)) * 8;                       \
-            tp[0] = tim_start; tp[1] = tim_first; tp[2] = gtime_ns(); tp[3] = tim_wait; tp[4] = tim_n; tp[5] = tim_busy; \
-        }                                                                                                             \
-    } while (0)
-#else
-#define TIM_DECL
-#define TIM_DO(stmt) do { } while (0)
-#define TIM_FLUSH() do { } while (0)
-#endif
 
 __device__ __forceinline__ unsigned smem_addr(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void cp_async4(unsigned dst, const float* src) {
@@ -657,7 +623,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
     int L0, L1;
     asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L0) : "l"(a.piece_start + blockIdx.x) : "memory");
     asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L1) : "l"(a.piece_start + blockIdx.x + 1) : "memory");
-    TIM_DECL;
 
     if (warp >= kCW && a.tma) {
         // =============================== TMA issuer + transposers ===============================
@@ -685,7 +650,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                     // and transposition: the first rows a piece needs do not queue behind a ring-full of later ones in DRAM
                     if ((i >= a.K && low_c <= i - a.K) || (i >= kInflight && low_t <= i - kInflight)) {
                         unsigned spins = 0;
-                        TIM_DO(tim_c = clock64());
                         for (;;) {
                             const int vc = lane < kCW ? lds_acquire(pub + 4u * lane) : 0x7fffffff;
                             const int vt = lane < T ? lds_acquire(next_addr + 4u * lane) : 0x7fffffff;
@@ -696,9 +660,7 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                             if (++spins == (1u << 21)) watchdog_note(3u, ((u64)(unsigned)i << 20) | (u64)(unsigned)low_c);
                             if (spins > (1u << 22)) __trap();
                         }
-                        TIM_DO(tim_wait += clock64() - tim_c);
                     }
-                    TIM_DO(if (!tim_first) tim_first = gtime_ns(); ++tim_n);
                     if (lane == 0) {
                         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy accesses of the slot are done
                         const unsigned bar = full_bar + 8u * slot;
@@ -707,7 +669,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                     }
                 } else if (turn == role - 1) {
                     const unsigned bar = full_bar + 8u * slot;
-                    TIM_DO(tim_c = clock64());
                     if (!mbar_try_wait(bar, use_parity)) {
                         unsigned spins = 0;
                         while (!mbar_try_wait(bar, use_parity)) {
@@ -715,7 +676,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                             if (spins > (1u << 20)) __trap();
                         }
                     }
-                    TIM_DO(tim_wait += clock64() - tim_c; if (!tim_first) tim_first = gtime_ns(); ++tim_n; tim_c = clock64());
                     const unsigned sbase = ring + (unsigned)slot * (unsigned)RB;
                     const unsigned rd = sbase + (unsigned)lane * 16u, wr = sbase + (unsigned)lane * 4u;
                     const unsigned wr2 = ring + (unsigned)a.K * (unsigned)RB + (unsigned)lane * 4u;      // mirror of slot 0
@@ -745,7 +705,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                     __threadfence_block();
                     __syncwarp();
                     if (lane == 0) sts_release(next_addr + 4u * (role - 1), i + T);
-                    TIM_DO(tim_busy += clock64() - tim_c);
                 }
                 ++i;
                 if (++slot == a.K) { slot = 0; use_parity ^= 1u; }
@@ -756,7 +715,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
             __syncwarp();
             if (lane == 0) sts_release(next_addr + 4u * (role - 1), 0x7fffffff);
         }
-        TIM_FLUSH();
         return;
     }
     if (warp >= kCW) {
@@ -790,7 +748,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                         __syncwarp();
                         if (landed < committed) { landed = committed; if (lane == 0) sts_release(my_next, pw + landed * kPW); }
                         unsigned spins = 0;
-                        TIM_DO(tim_c = clock64());
                         for (;;) {
                             const int v = lane < kCW ? lds_acquire(pub + 4u * lane) : 0x7fffffff;
                             minpub = __reduce_min_sync(0xffffffffu, v);
@@ -799,9 +756,7 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                             if (++spins == (1u << 21)) watchdog_note(1u, ((u64)(unsigned)i << 20) | (u64)(unsigned)minpub);
                             if (spins > (1u << 22)) __trap();
                         }
-                        TIM_DO(tim_wait += clock64() - tim_c);
                     }
-                    TIM_DO(if (!tim_first) tim_first = gtime_ns(); ++tim_n; tim_c = clock64());
                     const bool row_ok = y < lv.H;
                     const float* srow = src + (size_t)(row_ok ? y - it.ya : 0) * lv.W;
                     const unsigned dst = ring + (unsigned)slot * (unsigned)RB + (unsigned)(lane * CELL);
@@ -817,7 +772,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                         landed = committed - kDepth;
                         if (lane == 0) sts_release(my_next, pw + landed * kPW);
                     }
-                    TIM_DO(tim_busy += clock64() - tim_c);
                 }
                 ++i;
                 if (++slot == a.K) slot = 0;
@@ -828,7 +782,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
         __threadfence_block();
         __syncwarp();
         if (lane == 0) sts_release(my_next, 0x7fffffff);
-        TIM_FLUSH();
         return;
     }
 
@@ -888,7 +841,6 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
             const int i_last = irel + end - 1;
             if (i_last >= ready_c) {
                 unsigned spins = 0;
-                TIM_DO(tim_c = clock64());
                 for (;;) {
                     const int4 nx4 = lds_acquire4(next_addr);
                     ready_c = min(min(nx4.x, nx4.y), min(nx4.z, nx4.w));
@@ -897,9 +849,7 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                     if (++spins == (1u << 20)) watchdog_note(2u, ((u64)(unsigned)i_last << 20) | (u64)(unsigned)ready_c);
                     if (spins > (1u << 21)) __trap();
                 }
-                TIM_DO(tim_wait += clock64() - tim_c);
             }
-            TIM_DO(if (!tim_first) tim_first = gtime_ns(); ++tim_n; tim_c = clock64());
             // row bases (uniform): slot of y_low; the lower tap row is the next physical slot
             unsigned rt[SR];
             u64 hh[SR], ll[SR];
@@ -963,14 +913,12 @@ roi_align_strip_fwd(const __grid_constant__ StripMaps maps, const StripArgs a) {
                     }
                 }
             }
-            TIM_DO(tim_busy += clock64() - tim_c);
             e = e_next;
         }
         ibase += it.yhi - it.ya;
     }
     __syncwarp();
     if (lane == 0) sts_volatile(pub + 4u * warp, 0x7fffffff);       // nothing more to read
-    TIM_FLUSH();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1041,8 +989,6 @@ bool strip_geometry(int levels, const float* const* bottoms, const int* heights,
     g->pieces = sm_count > 0 ? sm_count : kNumSMs;
     g->cap_r = PH * PW * sr * sr;                              // worst case: every sample its own fragment
     g->max_entries = R * g->cap_r;
-    g->row_cost = 44u;
-    g->stop_after = 0;
     size_t off = 0;
     lay->ytab_off = off; off = align_up_sz(off + (size_t)R * g->ny * 16, 256);
     lay->xtab_off = off; off = align_up_sz(off + (size_t)R * g->nx * 16, 256);
@@ -1078,7 +1024,7 @@ EncodeTiledFn encode_tiled_fn() {
 // aligned base; the innermost start coordinate is always 0, so no tile load is ever misaligned (tools/tma_probe4.cu).
 bool make_quad_map(CUtensorMap* map, const float* bottom, int N, int C, int H, int W, int SX) {
     EncodeTiledFn encode = encode_tiled_fn();
-    if (!encode || (W & 3) || ((uintptr_t)bottom & 15u) || kPW < 2) return false;
+    if (!encode || (W & 3) || ((uintptr_t)bottom & 15u)) return false;
     const cuuint64_t dims[4] = {4, (cuuint64_t)N * (cuuint64_t)C, (cuuint64_t)(W / 4), (cuuint64_t)H};
     const cuuint64_t strides[3] = {(cuuint64_t)W * (cuuint64_t)H * 4, 16, (cuuint64_t)W * 4};
     const cuuint32_t box[4] = {4, 32, (cuuint32_t)(SX / 4), 1};
@@ -1124,11 +1070,7 @@ bool strip_device_info(StripDevice* out) {
 }  // namespace
 
 void roi_align_strip_set_debug_buffer(unsigned long long* host_pinned) {
-#ifdef B200_STRIP_TIMING
-    cudaMemcpyToSymbol(g_strip_tim, &host_pinned, sizeof(host_pinned));       // device buffer [CTA][warp][8] u64
-#else
     cudaMemcpyToSymbol(g_strip_dead, &host_pinned, sizeof(host_pinned));      // [CTA][32] u64 watchdog records
-#endif
 }
 
 size_t roi_align_strip_fpn_workspace_bytes(int levels, const int* heights, const int* widths, int N, int R, int PH, int PW, int sr) {
@@ -1143,26 +1085,23 @@ size_t roi_align_strip_workspace_bytes(int N, int R, int H, int W, int PH, int P
     return roi_align_strip_fpn_workspace_bytes(1, &H, &W, N, R, PH, PW, sr);
 }
 
-// returns B200_ROI_OK when the path ran; 1000 when it does not apply (caller falls back)
+// returns B200_ROI_OK when the path ran; kPathDeclined when it does not apply (caller falls back)
 int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const int* heights, const int* widths, const float* scales,
                                 const int* level_roi_begin, int N, int R, int C, int PH, int PW, int sr, const float* rois, float* top,
                                 const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-    if (workspace == nullptr || C <= 0) return 1000;
-    if ((long long)N * C >= (1LL << 31) || (long long)R * C * PH * PW >= (1LL << 31)) return 1000;
+    if (workspace == nullptr || C <= 0) return kPathDeclined;
+    if ((long long)N * C >= (1LL << 31) || (long long)R * C * PH * PW >= (1LL << 31)) return kPathDeclined;
     StripDevice dev;
-    if (!strip_device_info(&dev)) return 1000;
+    if (!strip_device_info(&dev)) return kPathDeclined;
     StripGeom g;
     StripLayout lay;
     unsigned smem = 0;
     // rows by TMA when every level has an x-quad view (W % 4 == 0, 16-byte aligned base) -- else cp.async producers
-    bool tma = option_get(kOptStreamStage) != 'a' && encode_tiled_fn() != nullptr && kPW >= 2;      // B200_STREAM_STAGE=async: A/B
+    bool tma = encode_tiled_fn() != nullptr;
     for (int l = 0; tma && l < levels; ++l) tma = (widths[l] & 3) == 0 && ((uintptr_t)bottoms[l] & 15u) == 0;
     if (!strip_geometry(levels, bottoms, heights, widths, scales, level_roi_begin, N, R, C, PH, PW, sr, dev.sm_count,
-                        tma ? kCellTma : kCellAsync, &g, &lay, &smem)) return 1000;
-    if (workspace_bytes < lay.ws_bytes) return 1000;
-    const int rc_opt = option_get(kOptStripRowCost);
-    if (rc_opt >= '0' && rc_opt <= '9') g.row_cost = 8u * (unsigned)(rc_opt - '0') + 4u;      // B200_STRIP_ROWCOST=0..9 (tuning)
-    if (option_get(kOptStreamPhases) == '1') g.stop_after = 1; else if (option_get(kOptStreamPhases) == '2') g.stop_after = 2;
+                        tma ? kCellTma : kCellAsync, &g, &lay, &smem)) return kPathDeclined;
+    if (workspace_bytes < lay.ws_bytes) return kPathDeclined;
     unsigned char* wsb = (unsigned char*)workspace;
     StripWs ws;
     ws.ytab = (uint4*)(wsb + lay.ytab_off);
@@ -1181,7 +1120,7 @@ int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const i
     int per_sm = 0;
     cudaError_t err = sr == 1 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, strip_prep<1>, kPrepThreads, prep_dyn)
                               : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, strip_prep<2>, kPrepThreads, prep_dyn);
-    if (err != cudaSuccess || per_sm < 1) { (void)cudaGetLastError(); return 1000; }
+    if (err != cudaSuccess || per_sm < 1) { (void)cudaGetLastError(); return kPathDeclined; }
     long long cap = (long long)per_sm * dev.sm_count;
     const int prep_grid = (int)(R < cap ? R : cap);
 
@@ -1189,7 +1128,6 @@ int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const i
     if (err != cudaSuccess) return (int)err;
     if (sr == 1) strip_prep<1><<<prep_grid, kPrepThreads, prep_dyn, stream>>>(rois, g, ws, top, row_map);
     else         strip_prep<2><<<prep_grid, kPrepThreads, prep_dyn, stream>>>(rois, g, ws, top, row_map);
-    if (option_get(kOptStreamPhases) == 'p' || g.stop_after) return finish_launch(1);          // timing probe: prepass only (output undefined)
 
     StripArgs a;
     a.ytab = ws.ytab; a.xtab = ws.xtab; a.entries = ws.entries; a.rowptr = ws.rowptr; a.maxend = ws.maxend;
@@ -1199,7 +1137,7 @@ int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const i
     StripMaps maps;
     memset(&maps, 0, sizeof(maps));
     for (int l = 0; tma && l < levels; ++l)
-        if (!make_quad_map(&maps.m[l], bottoms[l], N, C, heights[l], widths[l], g.SX)) return 1000;      // (the geometry was sized for TMA cells)
+        if (!make_quad_map(&maps.m[l], bottoms[l], N, C, heights[l], widths[l], g.SX)) return kPathDeclined;      // (the geometry was sized for TMA cells)
     a.tma = tma ? 1 : 0;
     for (int l = 0; l < kMaxLevels; ++l) a.lv[l] = g.lv[l];
     for (int c = 0; c <= kMaxCols; ++c) a.colstart[c] = g.colstart[c];
@@ -1214,7 +1152,7 @@ int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const i
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = option_get(kOptStripPdl) == '0' ? 0 : 1;                    // B200_STRIP_PDL=0: plain stream order
+    cfg.numAttrs = 1;
     const int xo = g.SX / 8;
 #define B200_STRIP_LAUNCH(SRV, XOV) \
     err = tma ? cudaLaunchKernelEx(&cfg, roi_align_strip_fwd<SRV, XOV, kCellTma>, maps, a) : cudaLaunchKernelEx(&cfg, roi_align_strip_fwd<SRV, XOV, kCellAsync>, maps, a)

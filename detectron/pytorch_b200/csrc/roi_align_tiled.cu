@@ -31,15 +31,6 @@
 
 namespace b200 {
 
-// Optional phase timing (tools/fwd_phase_probe.py; build with -DB200_FWD_TIMING): when a buffer is registered,
-// lane 0 of every warp adds its clock64 deltas per phase.  Compiled out by default (it costs registers).
-__device__ unsigned long long* g_fwd_timing = nullptr;
-#ifdef B200_FWD_TIMING
-#define B200_TIMING_PTR g_fwd_timing
-#else
-#define B200_TIMING_PTR ((unsigned long long*)nullptr)
-#endif
-
 // ------------------------------------------------------------------------------------------------
 // prepass
 // ------------------------------------------------------------------------------------------------
@@ -156,9 +147,6 @@ roi_align_tiled_fwd(const float* __restrict__ bottom, const AxisEntry* __restric
         // the NEXT item is claimed now, so the global atomic's latency hides behind this item
         int next_work = 0;
         if (tid == 0) { next_work = atomicAdd(work_counter, 1); misc[1] = 0; }
-        unsigned long long* const timing = B200_TIMING_PTR;
-        long long t_start = 0, t_staged = 0, t_done = 0;
-        if (timing) t_start = clock64();
         const int tile_id = work / n_cgroups;             // consecutive items share a tile (same list, tables hit L2)
         const int c0 = (work - tile_id * n_cgroups) * kCG;
         const int n_list = tile_count[tile_id];
@@ -211,8 +199,6 @@ roi_align_tiled_fwd(const float* __restrict__ bottom, const AxisEntry* __restric
             }
         }
         __syncthreads();
-        if (timing) t_staged = clock64();
-        int n_items = 0, n_kb = 0;
 
         // ---- warps pull RoIs of this tile; the axis tables of the NEXT RoI are fetched into registers
         //      while the current one is processed
@@ -267,9 +253,7 @@ roi_align_tiled_fwd(const float* __restrict__ bottom, const AxisEntry* __restric
             const unsigned div_m = 65536u / (unsigned)npw + 1u;          // b / npw == (b * div_m) >> 16 for b < 1024
             float* out_r = out + (size_t)(row_map ? row_map[r_cur] : r_cur) * C * bins + (size_t)c0 * bins;
             const float* tbase = tile + 4 * i;
-            ++n_items;
             if (kb < nb) {                                   // always true for entries the prepass wrote
-                ++n_kb;
 #pragma unroll
                 for (int jj = 0; jj < kStageBins / 4; ++jj) {
                     const int b = kb + jj * 4 + q;
@@ -330,23 +314,9 @@ roi_align_tiled_fwd(const float* __restrict__ bottom, const AxisEntry* __restric
                 __syncwarp();
             }
         }
-        if (timing) t_done = clock64();
         __syncthreads();                                  // every warp has read misc[0] and is done with the tile
-        if (timing && lane == 0) {
-            atomicAdd(&timing[0], (unsigned long long)(t_staged - t_start));
-            atomicAdd(&timing[1], (unsigned long long)(t_done - t_staged));
-            atomicAdd(&timing[2], (unsigned long long)(clock64() - t_done));
-            atomicAdd(&timing[3], 1ull);
-            atomicAdd(&timing[4], (unsigned long long)n_items);
-            atomicAdd(&timing[5], (unsigned long long)n_kb);
-            atomicMax(&timing[6], (unsigned long long)(t_done - t_staged));
-        }
         if (tid == 0) misc[0] = next_work;
     }
-}
-
-void roi_align_tiled_set_timing_buffer(unsigned long long* buf) {
-    cudaMemcpyToSymbol(g_fwd_timing, &buf, sizeof(buf));
 }
 
 size_t roi_align_tiled_workspace_bytes(int N, int R, int H, int W, int PH, int PW, int sr) {
@@ -355,12 +325,12 @@ size_t roi_align_tiled_workspace_bytes(int N, int R, int H, int W, int PH, int P
     return p.ws_bytes;
 }
 
-// returns B200_ROI_OK when the fast path ran; 1000 when it does not apply (caller falls back)
+// returns B200_ROI_OK when the fast path ran; kPathDeclined when it does not apply (caller falls back)
 int roi_align_forward_tiled(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
                             const float* rois, float* top, const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     TiledPlan p;
-    if (!roi_align_tiled_plan(N, R, H, W, C, PH, PW, sr, &p)) return 1000;
-    if (workspace == nullptr || workspace_bytes < p.ws_bytes) return 1000;
+    if (!roi_align_tiled_plan(N, R, H, W, C, PH, PW, sr, &p)) return kPathDeclined;
+    if (workspace == nullptr || workspace_bytes < p.ws_bytes) return kPathDeclined;
     unsigned char* ws = (unsigned char*)workspace;
     RoiHeader* hdr = (RoiHeader*)(ws + p.hdr_off);
     AxisEntry* ytab = (AxisEntry*)(ws + p.ytab_off);
@@ -374,7 +344,7 @@ int roi_align_forward_tiled(const float* bottom, float scale, int N, int R, int 
     static bool attr_set[64] = {false};     // per device: the attribute lives in the device's context
     static int sm_count[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 1000;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kPathDeclined;
     std::unique_lock<std::mutex> attr_lock(attr_mu);
     if (!attr_set[dev]) {
         cudaError_t e = cudaFuncSetAttribute(roi_align_tiled_fwd<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (228 * 1024 - kTiledCtasPerSM * 1024) / kTiledCtasPerSM);
@@ -391,8 +361,8 @@ int roi_align_forward_tiled(const float* bottom, float scale, int N, int R, int 
     if (err != cudaSuccess) return (int)err;
     // The bins the main kernel accumulates into must start at zero.  With a dense output one memset of the whole tensor
     // (25.7 MB at cfg2) is cheaper than the prepass storing ~1.3 M scattered zeros; the indexed variant shares
-    // its output tensor with other calls and zero-fills exactly its own split bins.  B200_FWD_ZERO=bins forces the latter.
-    const bool whole = row_map == nullptr && option_get(kOptFwdZero) != 'b';
+    // its output tensor with other calls and zero-fills exactly its own split bins.
+    const bool whole = row_map == nullptr;
     if (whole) {
         err = cudaMemsetAsync(top, 0, sizeof(float) * (size_t)R * C * PH * PW, stream);
         if (err != cudaSuccess) return (int)err;

@@ -146,7 +146,7 @@ roi_crop_bwd_nhwc_scatter(const float* __restrict__ go, const float* __restrict_
     }
 }
 
-// returns 1000 when the path does not apply
+// returns kPathDeclined when the path does not apply
 static bool crop_nhwc_applies(int N, int C, int H, int W, int R, int oh, int ow) {
     if ((C & 3) || C < 16 || N <= 0 || R <= 0 || (R % N) != 0) return false;
     const long long taps = 4LL * R * oh * ow * C;
@@ -160,16 +160,16 @@ size_t roi_crop_backward_workspace_bytes(int N, int C, int H, int W, int R, int 
 
 static int roi_crop_backward_nhwc(const float* grad_output, const float* grids, int N, int C, int H, int W, int R, int oh, int ow,
                                   float* grad_image, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-    if (!crop_nhwc_applies(N, C, H, W, R, oh, ow)) return 1000;
+    if (!crop_nhwc_applies(N, C, H, W, R, oh, ow)) return kPathDeclined;
     const int chunk = C < kCropChunk ? C : kCropChunk;
-    if (chunk & 3) return 1000;                                // thread = (pixel lane, quad): 256 / quads pixel lanes, the rest idle
+    if (chunk & 3) return kPathDeclined;                                // thread = (pixel lane, quad): 256 / quads pixel lanes, the rest idle
     const int c_pad = chunk + 4;
     const size_t smem = sizeof(float) * (size_t)oh * ow * c_pad;
-    if (smem > 200 * 1024) return 1000;
+    if (smem > 200 * 1024) return kPathDeclined;
     const size_t bytes = sizeof(float) * (size_t)N * C * H * W;
     float* scratch = (float*)workspace;
     const bool own = scratch == nullptr || workspace_bytes < bytes;      // no caller scratch: stream-ordered allocation
-    if (own && cudaMallocAsync((void**)&scratch, bytes, stream) != cudaSuccess) { (void)cudaGetLastError(); return 1000; }
+    if (own && cudaMallocAsync((void**)&scratch, bytes, stream) != cudaSuccess) { (void)cudaGetLastError(); return kPathDeclined; }
     cudaError_t err = cudaMemsetAsync(scratch, 0, bytes, stream);
     if (err == cudaSuccess && smem > 48 * 1024)
         err = cudaFuncSetAttribute(roi_crop_bwd_nhwc_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -191,7 +191,7 @@ int roi_crop_backward(const float* grad_output, const float* grids, int N, int C
     }
     if ((long)R * oh * ow > 0 && C > 0 && option_get(kOptBwdPath) != 'g') {      // B200_ROI_ALIGN_BWD_PATH=generic: scalar atomics (A/B)
         const int rc = roi_crop_backward_nhwc(grad_output, grids, N, C, H, W, R, oh, ow, grad_image, workspace, workspace_bytes, stream);
-        if (rc != 1000) return rc;
+        if (rc != kPathDeclined) return rc;
     }
     cudaError_t err = cudaMemsetAsync(grad_image, 0, sizeof(float) * (size_t)N * C * H * W, stream);
     if (err != cudaSuccess) return (int)err;

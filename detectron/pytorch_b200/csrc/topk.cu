@@ -197,18 +197,18 @@ size_t topk_batched_workspace_bytes(int num_problems) {
     return (size_t)num_problems * 3 * kBins * sizeof(int);
 }
 
-// returns 1000 when the batch does not fit the kernel's limits (caller falls back)
+// returns kPathDeclined when the batch does not fit the kernel's limits (caller falls back)
 int topk_batched(const float* const* scores_dev_ptrs_host, const int* A_host, const int* HW_host, const int* k_host, int num_problems,
                  long long* order_out, float* scores_out, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-    if (num_problems < 1 || num_problems > kTopkMaxProblems) return 1000;
-    if (workspace == nullptr || workspace_bytes < topk_batched_workspace_bytes(num_problems)) return 1000;
+    if (num_problems < 1 || num_problems > kTopkMaxProblems) return kPathDeclined;
+    if (workspace == nullptr || workspace_bytes < topk_batched_workspace_bytes(num_problems)) return kPathDeclined;
     TopkBatch tb;
     memset(&tb, 0, sizeof(tb));
     tb.count = num_problems;
     int off = 0, chunks = 0, kmax = 0;
     for (int p = 0; p < num_problems; ++p) {
         const long long n = (long long)A_host[p] * HW_host[p];
-        if (A_host[p] < 1 || HW_host[p] < 1 || n >= (1LL << 30) || k_host[p] < 0 || k_host[p] > n || k_host[p] > kTopkMaxK) return 1000;
+        if (A_host[p] < 1 || HW_host[p] < 1 || n >= (1LL << 30) || k_host[p] < 0 || k_host[p] > n || k_host[p] > kTopkMaxK) return kPathDeclined;
         tb.src[p] = scores_dev_ptrs_host[p]; tb.A[p] = A_host[p]; tb.HW[p] = HW_host[p]; tb.k[p] = k_host[p];
         tb.out_off[p] = off; off += k_host[p];
         tb.chunk_off[p] = chunks; chunks += (int)((n + kChunk - 1) / kChunk);
@@ -227,7 +227,7 @@ int topk_batched(const float* const* scores_dev_ptrs_host, const int* A_host, co
     const size_t smem = (size_t)m2 * sizeof(u64);
     static bool attr_done[64] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 1000;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kPathDeclined;
     if (!__atomic_load_n(&attr_done[dev], __ATOMIC_ACQUIRE)) {
         if (cudaFuncSetAttribute(topk_collect_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTopkMaxK * (int)sizeof(u64)) != cudaSuccess)
             return (int)cudaGetLastError();

@@ -175,10 +175,10 @@ B200_API int b200_nms(const float* boxes_dev, int boxes_num, int boxes_dim, floa
  * RoIs of all levels stored level-major in bottom_rois (level l owns rows level_roi_begin_host[l] .. [l + 1]), and
  * top_rows[r] = the row of top_data RoI r is written to (the inverse of the reference's restore permutation; NULL:
  * identity).  The four *_host arrays and bottom_data_host (device pointers of the maps) are HOST arrays read during the
- * call.  One streaming kernel walks the strip columns of every level; results are bit-identical to per-level
+ * call.  The quad-strip kernel walks the strip columns of every level; results are bit-identical to per-level
  * b200_roi_align_forward calls.  b200_roi_align_fpn_workspace_bytes(...) == 0 means "not applicable" (sampling_ratio
- * outside {1, 2}, too many strip columns, path switched off): loop over b200_roi_align_forward_indexed instead;
- * b200_roi_align_forward_fpn then returns B200_ROI_EWORKSPACE. */
+ * outside {1, 2}, too many strip columns, B200_ROI_ALIGN_PATH other than auto or quad): loop over
+ * b200_roi_align_forward_indexed instead; b200_roi_align_forward_fpn then returns B200_ROI_EWORKSPACE. */
 B200_API size_t b200_roi_align_fpn_workspace_bytes(int num_levels, const int* heights_host, const int* widths_host,
                                                    int batch_size, int num_rois, int aligned_height, int aligned_width,
                                                    int sampling_ratio);
@@ -277,16 +277,16 @@ B200_API int b200_nms_oks(const float* xy_preds_dev, const float* rois_dev, int 
 /* ---- introspection used by the benchmark / tests (no compute) ----------------------------------
  * Number of kernel launches the library has enqueued since load (all entry points). */
 B200_API unsigned long long b200_roi_ops_launch_count(void);
-/* Path-selection switches (A/B runs and tests): name is one of "B200_ROI_ALIGN_PATH" (auto|generic|tiled|stream|quad),
- * "B200_ROI_ALIGN_BWD_PATH" (auto|generic|nhwc|rows), "B200_ROI_ALIGN_BWD_CPL" (4|2), "B200_FWD_ZERO" (dense|bins),
- * "B200_NMS_SCAN" (resolver|simple), "B200_STREAM_STAGE" (tma|async|regs), "B200_STREAM_PHASES" (all|prepass: timing probe), "B200_STRIP_ROWCOST" (0..9),
- * "B200_STRIP_PDL" (1|0), "B200_FPN_PATH" (fused|levels);
+/* Path-selection switches (A/B runs and tests reach paths the dispatch otherwise picks by shape): name is one of
+ * "B200_ROI_ALIGN_PATH" (auto|generic|tiled|stream|quad), "B200_ROI_ALIGN_BWD_PATH" (auto|generic|nhwc|rows),
+ * "B200_ROI_ALIGN_BWD_CPL" (4|2), "B200_NMS_SCAN" (resolver|simple);
  * value NULL or "" restores the default.  Each switch takes its initial value from the
  * environment variable of the same name, read once at first use -- no entry point calls getenv() on the hot path.
  * Returns 0, or B200_ROI_EINVAL for an unknown name. */
 B200_API int b200_roi_ops_set_option(const char* name, const char* value);
-/* Debug: register (or clear with NULL) a device buffer of 8 x uint64 into which the tiled RoIAlign forward
- * adds per-warp clock64 deltas [staging, compute, end-of-item wait, warp-items, RoI items, 8-bin groups, max compute]. */
+/* Debug: register (or clear with NULL) one buffer with two uses.  The NMS kernels add their phase clock deltas to its
+ * first 16 uint64 words.  The two streaming RoIAlign forwards write a watchdog record into [CTA][32] uint64 (one word per
+ * warp) when a wait has spun half way to its trap; host-pinned memory keeps those records readable after the trap. */
 B200_API void b200_roi_ops_debug_timing_buffer(void* device_u64x16);
 
 /* ---- RPN proposal decode (SURVEY.md 8f N1: the GPU-resident proposal layer) --------------------------------

@@ -95,7 +95,6 @@ def test_workspace_sizing_is_host_arithmetic(lib_option):
     lib_option("B200_ROI_ALIGN_BWD_PATH", "generic")
     assert lib.b200_roi_align_backward_workspace_bytes(1, 512, 256, 200, 272, 7, 7, 2) == 0
     lib_option("B200_ROI_ALIGN_BWD_PATH", None)
-    assert lib.b200_roi_ops_set_option(b"NO_SUCH_SWITCH", b"x") == -1
     assert lib.b200_roi_align_backward_workspace_bytes(0, 512, 256, 200, 272, 7, 7, 2) == 0
     assert lib.b200_roi_align_backward_workspace_bytes(1, 512, 252, 200, 272, 7, 7, 2) == 252 * 200 * 272 * 4     # C % 64 != 0 -> NHWC path
     assert lib.b200_roi_align_backward_workspace_bytes(1, 8, 256, 200, 272, 7, 7, 2) == 0      # tiny gather volume -> scalar atomics
@@ -107,6 +106,26 @@ def test_workspace_sizing_is_host_arithmetic(lib_option):
     # NULL workspace is legal for the _ws entry points (generic kernels run); bad dims are still rejected first
     assert lib.b200_roi_align_forward_ws(None, 0.25, 1, 4, 10, 10, 3, 0, 7, 2, None, None, None, 0, None) == -1
     assert lib.b200_roi_align_backward_ws(None, 0.25, 1, 4, 10, -1, 3, 7, 7, 2, None, None, None, 0, None) == -1
+
+
+KEPT_SWITCHES = {"B200_ROI_ALIGN_PATH": b"generic", "B200_ROI_ALIGN_BWD_PATH": b"generic", "B200_ROI_ALIGN_BWD_CPL": b"2",
+                 "B200_NMS_SCAN": b"simple"}
+# tuning and timing switches of earlier versions (variants the dispatch never chose, probes with undefined output)
+RETIRED_SWITCHES = ["B200_" + s for s in ("STREAM_STAGE", "STREAM_PHASES", "STRIP_ROWCOST", "STRIP_PDL", "FWD_ZERO", "BWD_TRCH", "FPN_PATH")]
+
+
+@pytest.mark.parametrize("name", ["NO_SUCH_SWITCH"] + RETIRED_SWITCHES + sorted(KEPT_SWITCHES))
+def test_set_option_accepts_only_path_switches(name):
+    """b200_roi_ops_set_option knows the four switches that force a path the dispatch otherwise picks by shape; any other
+    name, including the retired tuning and timing switches, is B200_ROI_EINVAL."""
+    lib = _lib.load()
+    if name not in KEPT_SWITCHES:
+        assert lib.b200_roi_ops_set_option(name.encode(), b"x") == -1
+        return
+    try:
+        assert lib.b200_roi_ops_set_option(name.encode(), KEPT_SWITCHES[name]) == 0
+    finally:
+        assert lib.b200_roi_ops_set_option(name.encode(), None) == 0        # back to the default
 
 
 def test_round2_entry_points_validate_arguments_without_gpu():

@@ -279,6 +279,13 @@ def test_roi_align_fpn_equals_per_level_loop_cat_and_restore(bwd, lib_option):
             assert a.grad is not None and torch.count_nonzero(a.grad) == 0
 
 
+def test_roi_align_fpn_forced_stream_path_takes_per_level_loop(lib_option):
+    """The pyramid call runs the quad strips only.  With the forward forced onto the streaming-strip path it sizes no
+    workspace, so RoIAlignFPNFunction takes the per-level loop and still equals the reference flow."""
+    lib_option("B200_ROI_ALIGN_PATH", "stream")
+    test_roi_align_fpn_equals_per_level_loop_cat_and_restore("auto", lib_option)
+
+
 def test_roi_align_fpn_single_launch_sequence_bit_exact():
     """SURVEY 8f N2, second step: the whole pyramid in ONE launch sequence (count + fill + one streaming kernel over the strip
     columns of every level) -- bit-identical to the per-level calls, 3 kernel launches instead of 3 per level."""

@@ -2,7 +2,7 @@
 
     python tools/fwd_ab.py [--iters 60] [--paths quad,stream,tiled] [--check]
 
-Per path: whole call (prepass + main) and prepass only (B200_STREAM_PHASES=prepass), rotating over input sets larger than L2.
+Per path: time of the whole call (prepass + main), rotating over input sets larger than L2.
 --check compares every path's output with the generic kernel's (bit-exact share).
 """
 import argparse
@@ -43,18 +43,15 @@ def main():
         for path in args.paths.split(","):
             _lib.set_option("B200_ROI_ALIGN_PATH", path)
             row = {}
-            for phases in ("all", "prepass"):
-                _lib.set_option("B200_STREAM_PHASES", phases)
-                for i in range(5):
-                    ops.roi_align_forward(feats[i % nset], rois[i % nset], P, P, s, sr)
-                torch.cuda.synchronize()
-                e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for i in range(args.iters):
-                    ops.roi_align_forward(feats[i % nset], rois[i % nset], P, P, s, sr)
-                e1.record(); torch.cuda.synchronize()
-                row[phases + "_us"] = round(e0.elapsed_time(e1) * 1e3 / args.iters, 2)
-            _lib.set_option("B200_STREAM_PHASES", "all")
+            for i in range(5):
+                ops.roi_align_forward(feats[i % nset], rois[i % nset], P, P, s, sr)
+            torch.cuda.synchronize()
+            e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for i in range(args.iters):
+                ops.roi_align_forward(feats[i % nset], rois[i % nset], P, P, s, sr)
+            e1.record(); torch.cuda.synchronize()
+            row["all_us"] = round(e0.elapsed_time(e1) * 1e3 / args.iters, 2)
             if ref is not None:
                 out = ops.roi_align_forward(feats[0], rois[0], P, P, s, sr).cpu().numpy()
                 row["exact_share"] = float(np.mean(out == ref))
