@@ -41,7 +41,11 @@ roi_align_tiled_prep(const float* __restrict__ rois, float scale, int N, int R, 
                      int* __restrict__ tile_count, unsigned* __restrict__ tile_list, int groups_max, float* __restrict__ out,
                      const int* __restrict__ row_map, int zero_split) {
     __shared__ int s_ty[kAxisMax], s_tx[kAxisMax];
-    __shared__ int s_nbin_y[kAxisMax], s_nbin_x[kAxisMax];     // bin rows / cols this RoI has in tile row ty0+k / col tx0+k
+    // the tile rows / cols that hold samples of this RoI (at most one per sample; the RoI's tile rectangle can span many
+    // more), and the bin rows / cols the RoI has in each
+    __shared__ int s_tile_y[kAxisMax], s_tile_x[kAxisMax];
+    __shared__ int s_nbin_y[kAxisMax], s_nbin_x[kAxisMax];
+    __shared__ int s_nty, s_ntx;
     __shared__ unsigned short s_split[kAxisMax * kAxisMax];
     __shared__ int s_nsplit;
     const int r = blockIdx.x;
@@ -68,26 +72,32 @@ roi_align_tiled_prep(const float* __restrict__ rois, float scale, int N, int R, 
     }
     // Work entries: one per (tile, 8-bin group of this RoI in that tile), so that no warp of the main kernel is
     // ever stuck with more than 8 bins while its CTA waits.  The bin rectangle of a tile is derived exactly as
-    // the main kernel derives it: [first sample in tile / sr, last sample in tile / sr] per axis.
-    const int nty = ty1 - ty0 + 1, ntx = tx1 - tx0 + 1;
-    if (t < nty + ntx) {
-        const bool isy = t < nty;
-        const int want = isy ? ty0 + t : tx0 + (t - nty);
+    // the main kernel derives it: [first sample in tile / sr, last sample in tile / sr] per axis.  Tiles without a
+    // sample of the RoI get no entry; a tall or wide RoI can span more than kAxisMax tile rows / cols, but only the
+    // (at most ny / nx) tiles that hold samples are listed, in ascending order.
+    if (t < ny + nx) {
+        const bool isy = t < ny;
+        const int s = isy ? t : t - ny;
         const int* arr = isy ? s_ty : s_tx;
         const int cnt = isy ? ny : nx;
-        int first = -1, last = -1;
-        for (int s = 0; s < cnt; ++s) if (arr[s] == want) { if (first < 0) first = s; last = s; }
-        const int nbin = first < 0 ? 0 : last / sr - first / sr + 1;
-        if (isy) s_nbin_y[t] = nbin; else s_nbin_x[t - nty] = nbin;
+        if (s == 0 || arr[s] != arr[s - 1]) {                 // first sample of its tile (lows are monotone along an axis)
+            int rank = 0;
+            for (int j = 1; j <= s; ++j) rank += arr[j] != arr[j - 1];
+            int last = s;
+            while (last + 1 < cnt && arr[last + 1] == arr[s]) ++last;
+            const int nbin = last / sr - s / sr + 1;
+            if (isy) { s_tile_y[rank] = arr[s]; s_nbin_y[rank] = nbin; } else { s_tile_x[rank] = arr[s]; s_nbin_x[rank] = nbin; }
+            if (last == cnt - 1) { if (isy) s_nty = rank + 1; else s_ntx = rank + 1; }
+        }
     }
     __syncthreads();
+    const int nty = s_nty, ntx = s_ntx;
     if (batch_ok) {
         for (int k = t; k < nty * ntx; k += blockDim.x) {
             const int ky = k / ntx, kx = k - ky * ntx;
             const int nb = s_nbin_y[ky] * s_nbin_x[kx];
-            if (nb == 0) continue;
             const int ngroups = (nb + kStageBins - 1) / kStageBins;
-            const int tile = (g.batch * tiles_y + ty0 + ky) * tiles_x + tx0 + kx;
+            const int tile = (g.batch * tiles_y + s_tile_y[ky]) * tiles_x + s_tile_x[kx];
             const int pos = atomicAdd(&tile_count[tile], ngroups);
             unsigned* dst = tile_list + (size_t)tile * R * groups_max + pos;
             for (int gI = 0; gI < ngroups; ++gI) dst[gI] = (unsigned)r | ((unsigned)gI << 16);

@@ -2,6 +2,7 @@
 `make -C oracle ref REFERENCE=<reference checkout>` from its unmodified sources).  Needs a GPU and oracle/liboracle.so:
 
     python tests/golden/make_golden.py OUT_DIR          # then copy OUT_DIR/*.npz into tests/golden/
+    python tests/golden/make_golden.py OUT_DIR geometry # only roi_align_geometry_sm90a.npz (tests/geometry_cases.py)
 
 Inputs are the seeded cases of tests/cases.py and synthetic.py, so only the reference OUTPUTS are stored.  Outputs of the
 full-size configurations are stored as a fixed, seeded sample of positions (roi_align_full_size.npz,
@@ -63,11 +64,30 @@ def full_size(out_dir, t):
     np.savez_compressed(os.path.join(out_dir, "roi_align_bwd_spread.npz"), **g)
 
 
-def main(out_dir):
+def geometry(out_dir, t):
+    """The reference kernel's forward and dX on the rectangular-bin cases of tests/geometry_cases.py, from its sm_90a build
+    (roi_align_geometry_sm90a.npz): a fixed, seeded sample of output positions and of non-zero dX positions per case."""
+    from tests import geometry_cases as GC
+    g = {}
+    for i, name in enumerate(GC.RECT_CASES):
+        c, f, r, dy = GC.geometry_case(name)
+        PH, PW, s, sr = c["PH"], c["PW"], c["scale"], c["sr"]
+        out = G.roi_align_forward(t(f), t(r), PH, PW, s, sr).cpu().numpy()
+        dx = G.roi_align_backward(t(dy), t(r), c["shape"], PH, PW, s, sr).cpu().numpy()
+        io, idx = GC.golden_positions(out.size, 100 + i), GC.golden_positions(dx.size, 200 + i, nonzero_of=dx)
+        g.update({name + "/out_idx": io, name + "/out": out.reshape(-1)[io], name + "/dx_idx": idx, name + "/dx": dx.reshape(-1)[idx]})
+    np.savez_compressed(os.path.join(out_dir, "roi_align_geometry_sm%d%da.npz" % torch.cuda.get_device_capability()), **g)
+
+
+def main(out_dir, steps=None):
     os.makedirs(out_dir, exist_ok=True)
     assert torch.cuda.is_available() and G.available()
     dev = torch.device("cuda:0")
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)   # noqa: E731
+    if steps == ["geometry"]:
+        geometry(out_dir, t)
+        print("golden written to", out_dir, sorted(os.listdir(out_dir)))
+        return
     xfrom = {}
     for name in sorted(cases.ROI_CASES):
         c, f, r, dy = cases.roi_case(name)
@@ -96,11 +116,12 @@ def main(out_dir):
         keeps["keep_%d" % n] = G.nms_gpu(t(cases.nms_case(n)), 0.7).cpu().numpy().reshape(-1).astype(np.int32)
     np.savez_compressed(os.path.join(out_dir, "nms.npz"), **keeps)
     full_size(out_dir, t)
+    geometry(out_dir, t)
     torch.cuda.synchronize()
     print("golden written to", out_dir, sorted(os.listdir(out_dir)))
 
 
 if __name__ == "__main__":
-    if len(sys.argv) != 2:
-        raise SystemExit("usage: python tests/golden/make_golden.py OUT_DIR")
-    main(sys.argv[1])
+    if len(sys.argv) not in (2, 3) or sys.argv[2:] not in ([], ["geometry"]):
+        raise SystemExit("usage: python tests/golden/make_golden.py OUT_DIR [geometry]")
+    main(sys.argv[1], sys.argv[2:] or None)
