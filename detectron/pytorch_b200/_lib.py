@@ -107,6 +107,16 @@ _SIGNATURES = {
     # (xy_preds, rois, D, K, thresh, keep, num_keep, stream)
     "b200_nms_oks": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_void_p, ctypes.c_void_p,
                                     _stream_t]),
+    # (L, F_host, A_host, N, num_gt)
+    "b200_rpn_targets_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int]),
+    # (L, F_host, A_host, strides_host, cell_host, N, im_sizes_host, gt_begin_host, gt, straddle, pos, neg, counts, ws, ws_bytes, stream)
+    "b200_rpn_labels": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int] + [ctypes.c_void_p] * 2 +
+                        [_c_float_p, ctypes.c_double, ctypes.c_float, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t,
+                         _stream_t]),
+    # (L, F_host, A_host, strides_host, cell_host, N, im_sizes_host, gt_begin_host, gt, straddle, counts, dis, dis_begin_host, en,
+    #  en_begin_host, ws, ws_bytes, labels_host, targets_host, inside_host, outside_host, stream)
+    "b200_rpn_emit": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int] + [ctypes.c_void_p] * 2 +
+                      [_c_float_p, ctypes.c_double] + [ctypes.c_void_p] * 6 + [ctypes.c_size_t] + [ctypes.c_void_p] * 4 + [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

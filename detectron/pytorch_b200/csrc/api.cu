@@ -77,6 +77,13 @@ bool keypoints_args_ok(int, int, int, int);
 bool nms_oks_args_ok(int, int);
 int heatmaps_to_keypoints(const float*, const float*, int, int, int, int, float*, cudaStream_t);
 int nms_oks(const float*, const float*, int, double, int*, int*, cudaStream_t);
+int rpn_total_anchors(int, const int*, const int*);
+size_t rpn_workspace_bytes(int, int, int);
+int rpn_labels(int, const int*, const int*, const double*, const double*, int, const double*, const int*, const float*, double, float, float,
+               int*, void*, size_t, cudaStream_t);
+int rpn_emit(int, const int*, const int*, const double*, const double*, int, const double*, const int*, const float*, double, const int*,
+             const int*, const int*, const int*, const int*, void*, size_t, int* const*, float* const*, float* const*, float* const*,
+             cudaStream_t);
 
 // B200_ROI_ALIGN_PATH=generic|tiled|stream|auto (default auto) -- test/benchmark override of the forward dispatch
 //   0 auto: streaming-strip path -> quad-strip path -> tiled path -> generic, each when it applies.  On H100 the streaming
@@ -622,6 +629,33 @@ int b200_nms_oks(const float* xy_preds_dev, const float* rois_dev, int num_rois,
     if (num_rois == 0) return B200_ROI_OK;
     if (!xy_preds_dev || !rois_dev || !keep_dev || !num_keep_dev) return B200_ROI_EINVAL;
     return nms_oks(xy_preds_dev, rois_dev, num_rois, thresh, keep_dev, num_keep_dev, (cudaStream_t)stream);
+}
+
+size_t b200_rpn_targets_workspace_bytes(int num_levels, const int* field_sizes_host, const int* num_cell_anchors_host, int num_images,
+                                        int num_gt_total) {
+    const int total = rpn_total_anchors(num_levels, field_sizes_host, num_cell_anchors_host);
+    return total < 0 ? 0 : rpn_workspace_bytes(num_images, total, num_gt_total);
+}
+
+int b200_rpn_labels(int num_levels, const int* field_sizes_host, const int* num_cell_anchors_host, const double* strides_host,
+                    const double* cell_anchors_host, int num_images, const double* im_sizes_host, const int* gt_begin_host,
+                    const float* gt_boxes_dev, double straddle_thresh, float positive_overlap, float negative_overlap, int* counts_out_dev,
+                    void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+    return rpn_labels(num_levels, field_sizes_host, num_cell_anchors_host, strides_host, cell_anchors_host, num_images, im_sizes_host,
+                      gt_begin_host, gt_boxes_dev, straddle_thresh, positive_overlap, negative_overlap, counts_out_dev, workspace,
+                      workspace_bytes, (cudaStream_t)stream);
+}
+
+int b200_rpn_emit(int num_levels, const int* field_sizes_host, const int* num_cell_anchors_host, const double* strides_host,
+                  const double* cell_anchors_host, int num_images, const double* im_sizes_host, const int* gt_begin_host,
+                  const float* gt_boxes_dev, double straddle_thresh, const int* counts_dev, const int* fg_disable_dev,
+                  const int* fg_disable_begin_host, const int* bg_enable_dev, const int* bg_enable_begin_host, void* workspace,
+                  size_t workspace_bytes, int* const* labels_out_host, float* const* bbox_targets_out_host,
+                  float* const* inside_weights_out_host, float* const* outside_weights_out_host, b200_stream_t stream) {
+    return rpn_emit(num_levels, field_sizes_host, num_cell_anchors_host, strides_host, cell_anchors_host, num_images, im_sizes_host,
+                    gt_begin_host, gt_boxes_dev, straddle_thresh, counts_dev, fg_disable_dev, fg_disable_begin_host, bg_enable_dev,
+                    bg_enable_begin_host, workspace, workspace_bytes, labels_out_host, bbox_targets_out_host, inside_weights_out_host,
+                    outside_weights_out_host, (cudaStream_t)stream);
 }
 
 }  // extern "C"

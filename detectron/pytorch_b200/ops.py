@@ -599,6 +599,79 @@ def heatmaps_to_keypoints_raw(maps, rois, min_size=0):
     return out
 
 
+def rpn_targets_raw(gt_boxes, gt_counts, im_sizes, levels, draw, straddle_thresh=0, positive_overlap=0.7, negative_overlap=0.3):
+    """RPN anchor labels and regression targets for N images and all anchor levels (lib/roi_data/rpn.py:115-259).
+    gt_boxes: float32 CUDA (sum G, 4), image n's (scaled) ground truth in rows sum(gt_counts[:n]) ...; gt_counts: host ints, each
+    >= 1; im_sizes: host (N, 2) = (im_height, im_width); levels: one (field_size, stride, cell_anchors (A, 4) float64) per level.
+    draw(counts) is called once with the (N, 3) host array (#fg candidates, #bg candidates, #inside anchors) -- the one host read
+    of the call -- and returns, per image, (fg positions to disable, bg positions to enable): int sequences or CUDA tensors.
+    Returns one (labels int32 (N, A, F, F), bbox_targets, inside_weights, outside_weights float32 (N, 4A, F, F)) per level."""
+    import ctypes
+    import numpy as np
+    _need_cuda_f32(gt_boxes, "gt_boxes")
+    if gt_boxes.dim() != 2 or gt_boxes.size(1) != 4:
+        raise ValueError("gt_boxes must be (G, 4) = [x1, y1, x2, y2], got %s" % (tuple(gt_boxes.shape),))
+    gt_counts = [int(c) for c in gt_counts]
+    N, L = len(gt_counts), len(levels)
+    im_sizes = np.ascontiguousarray(im_sizes, dtype=np.float64).reshape(-1, 2)
+    if im_sizes.shape[0] != N or sum(gt_counts) != gt_boxes.size(0):
+        raise ValueError("rpn_targets_raw: %d images, %d image sizes, %d ground-truth rows for counts %s"
+                         % (N, im_sizes.shape[0], gt_boxes.size(0), gt_counts))
+    dev = gt_boxes.device
+    gt_boxes = gt_boxes.contiguous()
+    Fs = [int(F) for F, _, _ in levels]
+    cells = [np.asarray(c, dtype=np.float64).reshape(-1, 4) for _, _, c in levels]
+    As = [c.shape[0] for c in cells]
+
+    def arr(ctype, vals):
+        a = (ctype * max(len(vals), 1))(*vals)
+        return ctypes.cast(a, ctypes.c_void_p), a             # the array object keeps the memory alive during the call
+
+    F_p, F_a = arr(ctypes.c_int, Fs)
+    A_p, A_a = arr(ctypes.c_int, As)
+    S_p, S_a = arr(ctypes.c_double, [float(s) for _, s, _ in levels])
+    C_p, C_a = arr(ctypes.c_double, np.concatenate(cells).ravel().tolist() if cells else [])
+    I_p, I_a = arr(ctypes.c_double, im_sizes.ravel().tolist())
+    G_p, G_a = arr(ctypes.c_int, np.concatenate([[0], np.cumsum(gt_counts)]).astype(int).tolist())
+    lib = _lib.load()
+    ws_bytes = int(lib.b200_rpn_targets_workspace_bytes(L, F_p, A_p, N, gt_boxes.size(0)))
+    if ws_bytes == 0:
+        raise ValueError("rpn_targets_raw: unsupported geometry (1..8 levels, <= 32 cell anchors, 1..64 images)")
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    counts = torch.empty((N, 3), dtype=torch.int32, device=dev)
+    common = (L, F_p, A_p, S_p, C_p, N, I_p, G_p, gt_boxes.data_ptr(), float(straddle_thresh))
+    with torch.cuda.device(dev):
+        _lib.check(lib.b200_rpn_labels(*common, float(positive_overlap), float(negative_overlap), counts.data_ptr(), ws.data_ptr(), ws_bytes,
+                                       _stream()), "b200_rpn_labels")
+        picks = draw(counts.cpu().numpy())
+        dis_parts, en_parts = [], []
+        for dis, en in picks:
+            dis_parts.append(torch.as_tensor(np.asarray(dis) if not torch.is_tensor(dis) else dis).reshape(-1))
+            en_parts.append(torch.as_tensor(np.asarray(en) if not torch.is_tensor(en) else en).reshape(-1))
+        if len(dis_parts) != N:
+            raise ValueError("draw returned %d entries for %d images" % (len(dis_parts), N))
+        D_p, D_a = arr(ctypes.c_int, np.concatenate([[0], np.cumsum([d.numel() for d in dis_parts])]).astype(int).tolist())
+        E_p, E_a = arr(ctypes.c_int, np.concatenate([[0], np.cumsum([e.numel() for e in en_parts])]).astype(int).tolist())
+        # one int32 device buffer for both draws (a single upload when they come from the host)
+        parts = dis_parts + en_parts
+        if all(not p.is_cuda for p in parts):
+            flat = torch.cat([p.to(torch.int32) for p in parts]).to(dev) if parts else torch.empty((0,), dtype=torch.int32, device=dev)
+        else:
+            flat = torch.cat([p.to(device=dev, dtype=torch.int32) for p in parts])
+        flat = torch.cat([flat, flat.new_zeros((1,))])            # never empty: a valid pointer even without draws
+        n_dis = sum(d.numel() for d in dis_parts)
+        outs = []
+        for F, A in zip(Fs, As):
+            outs.append((torch.empty((N, A, F, F), dtype=torch.int32, device=dev),
+                         torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev),
+                         torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev),
+                         torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev)))
+        tables = [arr(ctypes.c_void_p, [o[k].data_ptr() for o in outs]) for k in range(4)]
+        _lib.check(lib.b200_rpn_emit(*common, counts.data_ptr(), flat.data_ptr(), D_p, flat.data_ptr() + 4 * n_dis, E_p, ws.data_ptr(),
+                                     ws_bytes, *[t[0] for t in tables], _stream()), "b200_rpn_emit")
+    return outs
+
+
 def nms_oks_raw(xy_preds, rois, thresh):
     """Greedy OKS NMS of lib/utils/keypoints.py:225-266 on (D, 4, 17) predictions and their (D, >=4) boxes, float32 CUDA.
     Returns (keep int32 (D,), num_keep int32 (1,)) on the device, no host sync: keep[:num_keep] are the kept indices in

@@ -336,6 +336,46 @@ B200_API int b200_fast_rcnn_targets(const float* boxes_dev, const float* gt_boxe
                                     float* rois_out_dev, float* bbox_targets_out_dev, float* inside_weights_out_dev,
                                     float* outside_weights_out_dev, b200_stream_t stream);
 
+/* ---- RPN anchor labels and box-regression targets (training, lib/roi_data/rpn.py:40-261) -------------------------------
+ * add_rpn_blobs / _get_rpn_blobs for all images and all anchor levels of a step, in a fixed number of launches.
+ * Level table (HOST arrays, 1 <= num_levels <= 8): field_sizes_host[l] = F_l, num_cell_anchors_host[l] = A_l (sum <= 32),
+ *   strides_host[l], cell_anchors_host (sum A_l, 4) float64 = generate_anchors(stride_l, sizes_l, ratios).  Anchor i of the
+ *   call is the reference's concatenated order: level, then (h, w, a); it is float32(cell anchor + (w, h, w, h) * stride), the
+ *   rounding of data_utils.py:69-93, computed where it is needed.
+ * Image table (HOST arrays, 1 <= num_images <= 64): im_sizes_host (N, 2) float64 = (im_height, im_width); image n's ground
+ *   truth is rows gt_begin_host[n] .. gt_begin_host[n + 1] - 1 of gt_boxes_dev (float32 (x1, y1, x2, y2), already scaled), and
+ *   every image needs at least one (the reference fails without, rpn.py:144-186).
+ * b200_rpn_labels  rpn.py:115-170 + the candidate sets of :174 / :186: inside test (straddle_thresh < 0 keeps every anchor;
+ *   x1, y1 >= float32(-straddle), x2 < im_width + straddle and y2 < im_height + straddle in float64), IoU with
+ *   cython_bbox.bbox_overlaps' arithmetic, fg candidates = anchors whose row equals some ground-truth box's maximum over the
+ *   inside anchors or whose row maximum is >= positive_overlap, bg candidates = row maximum < negative_overlap (fg included).
+ *   counts_out_dev int32 (N, 3) = (#fg candidates, #bg candidates, #inside anchors).  memset + 3 launches.
+ * The caller reads the counts once and draws: per image, positions into the ascending fg candidate list to disable
+ *   (npr.choice(fg_inds, #fg - num_fg, replace=False), rpn.py:175-179) and positions into the ascending bg candidate list to
+ *   enable (npr.randint(#bg, size=num_bg), :185-189, only when #bg > num_bg).
+ * b200_rpn_emit  rpn.py:176-259 with that draw: fg_disable_dev / bg_enable_dev int32, image n's positions at
+ *   [*_begin_host[n], *_begin_host[n + 1]) (HOST tables, N + 1 entries; positions out of range are ignored).  Disables first,
+ *   then enables; targets (utils/boxes.py:199-230, weights 1) for the fg set left by the disable draw, even where the enable
+ *   draw relabels one of them 0; inside weights 1 where the final label is 1; outside weights float32(1.0 / #labels >= 0)
+ *   where it is >= 0.  Writes EVERY element of level l's blobs, the four device pointers of the *_out_host tables:
+ *   labels int32 (N, A_l, F_l, F_l), bbox targets / inside / outside weights float32 (N, 4 A_l, F_l, F_l); anchors outside
+ *   the image get -1 / 0.  Blobs with F_l * F_l % 4 == 0 must be 16-byte aligned.  3 launches.
+ * Both take the same tables, `counts_dev` is the labelling call's output, and the workspace (b200_rpn_targets_workspace_bytes
+ * bytes, about 13 bytes per (image, anchor)) carries the labelling state to the emit call.  Bad sizes, tables or null pointers:
+ * B200_ROI_EINVAL before any launch; a missing or small workspace: B200_ROI_EWORKSPACE. */
+B200_API size_t b200_rpn_targets_workspace_bytes(int num_levels, const int* field_sizes_host, const int* num_cell_anchors_host, int num_images,
+                                                 int num_gt_total);
+B200_API int b200_rpn_labels(int num_levels, const int* field_sizes_host, const int* num_cell_anchors_host, const double* strides_host,
+                             const double* cell_anchors_host, int num_images, const double* im_sizes_host, const int* gt_begin_host,
+                             const float* gt_boxes_dev, double straddle_thresh, float positive_overlap, float negative_overlap,
+                             int* counts_out_dev, void* workspace, size_t workspace_bytes, b200_stream_t stream);
+B200_API int b200_rpn_emit(int num_levels, const int* field_sizes_host, const int* num_cell_anchors_host, const double* strides_host,
+                           const double* cell_anchors_host, int num_images, const double* im_sizes_host, const int* gt_begin_host,
+                           const float* gt_boxes_dev, double straddle_thresh, const int* counts_dev, const int* fg_disable_dev,
+                           const int* fg_disable_begin_host, const int* bg_enable_dev, const int* bg_enable_begin_host, void* workspace,
+                           size_t workspace_bytes, int* const* labels_out_host, float* const* bbox_targets_out_host,
+                           float* const* inside_weights_out_host, float* const* outside_weights_out_host, b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
