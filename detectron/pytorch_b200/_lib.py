@@ -117,6 +117,11 @@ _SIGNATURES = {
     #  en_begin_host, ws, ws_bytes, labels_host, targets_host, inside_host, outside_host, stream)
     "b200_rpn_emit": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 4 + [ctypes.c_int] + [ctypes.c_void_p] * 2 +
                       [_c_float_p, ctypes.c_double] + [ctypes.c_void_p] * 6 + [ctypes.c_size_t] + [ctypes.c_void_p] * 4 + [_stream_t]),
+    # (rois, roi_image, roi_class, R, N, obj_begin_host, num_polys, poly_begin, num_coords, coord_begin, coords, M, num_classes,
+    #  obj_boxes, masks, stream)
+    "b200_mask_targets": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                         ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 2 +
+                          [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

@@ -84,6 +84,8 @@ int rpn_labels(int, const int*, const int*, const double*, const double*, int, c
 int rpn_emit(int, const int*, const int*, const double*, const double*, int, const double*, const int*, const float*, double, const int*,
              const int*, const int*, const int*, const int*, void*, size_t, int* const*, float* const*, float* const*, float* const*,
              cudaStream_t);
+int mask_targets(const float*, const int*, const int*, int, int, const int*, int, const int*, int, const int*, const float*, int, int,
+                 float*, int*, cudaStream_t);
 
 // B200_ROI_ALIGN_PATH=generic|tiled|stream|auto (default auto) -- test/benchmark override of the forward dispatch
 //   0 auto: streaming-strip path -> quad-strip path -> tiled path -> generic, each when it applies.  On H100 the streaming
@@ -656,6 +658,14 @@ int b200_rpn_emit(int num_levels, const int* field_sizes_host, const int* num_ce
                     gt_begin_host, gt_boxes_dev, straddle_thresh, counts_dev, fg_disable_dev, fg_disable_begin_host, bg_enable_dev,
                     bg_enable_begin_host, workspace, workspace_bytes, labels_out_host, bbox_targets_out_host, inside_weights_out_host,
                     outside_weights_out_host, (cudaStream_t)stream);
+}
+
+int b200_mask_targets(const float* rois_dev, const int* roi_image_dev, const int* roi_class_dev, int num_rois, int num_images,
+                      const int* obj_begin_host, int num_polys, const int* poly_begin_dev, int num_coords, const int* coord_begin_dev,
+                      const float* coords_dev, int resolution, int num_classes, float* obj_boxes_out_dev, int* masks_out_dev,
+                      b200_stream_t stream) {
+    return mask_targets(rois_dev, roi_image_dev, roi_class_dev, num_rois, num_images, obj_begin_host, num_polys, poly_begin_dev, num_coords,
+                        coord_begin_dev, coords_dev, resolution, num_classes, obj_boxes_out_dev, masks_out_dev, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -15,8 +15,9 @@ Training branch (:49-63).  The reference "reuses the data loader code": json_dat
 merged into every roidb entry behind its ground-truth boxes, best-gt assignment through cython_bbox.bbox_overlaps,
 crowd_thresh = 0 so nothing is filtered) and roi_data.fast_rcnn.add_fast_rcnn_blobs (_sample_rois per image, concatenation,
 _add_multilevel_rois).  Here the same blobs are produced on the device with roi_data/fast_rcnn.py (SURVEY.md 8f N4); the
-random draws are inputs (`choices`), see there.  Mask / keypoint blobs are not produced (MASK_ON / KEYPOINTS_ON models keep
-the host path for those).
+random draws are inputs (`choices`), see there.  With MODEL.MASK_ON the mask blobs (mask_rois, roi_has_mask_int32,
+masks_int32 and the mask_rois FPN blobs) come from roi_data/mask_rcnn.py, on the device too; keypoint blobs are not produced
+(KEYPOINTS_ON models keep the host path for those).
 """
 import torch
 from torch import nn
@@ -78,7 +79,9 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
         Training (module in training mode): roidb = one dict per image with the ground truth ('boxes' (G, 4) unscaled,
         'gt_classes' (G,); numpy or tensors), im_info = (N, 3) [height, width, scale]; `train` = the TRAIN / MODEL keys
         (dict, or taken from `cfg`): BATCH_SIZE_PER_IM, FG_FRACTION, FG_THRESH, BG_THRESH_HI, BG_THRESH_LO, NUM_CLASSES,
-        BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG; choices = per image (fg_choice, bg_choice) or None (device randperm)."""
+        BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG, and for Mask R-CNN MASK_ON, MRCNN_RESOLUTION (default 14), CLS_SPECIFIC_MASK
+        (default True), with the roidb entries' 'segms' and 'is_crowd'; choices = per image (fg_choice, bg_choice) or None
+        (device randperm)."""
         p = self._params()
         n = p["rpn_max"] - p["rpn_min"] + 1
         topn = int(p["topn"] * p["scale"] + 0.5)
@@ -96,10 +99,13 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
             t = dict(BATCH_SIZE_PER_IM=c.TRAIN.BATCH_SIZE_PER_IM, FG_FRACTION=c.TRAIN.FG_FRACTION, FG_THRESH=c.TRAIN.FG_THRESH,
                      BG_THRESH_HI=c.TRAIN.BG_THRESH_HI, BG_THRESH_LO=c.TRAIN.BG_THRESH_LO, NUM_CLASSES=c.MODEL.NUM_CLASSES,
                      BBOX_REG_WEIGHTS=c.MODEL.BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG=c.MODEL.CLS_AGNOSTIC_BBOX_REG)
+            if getattr(c.MODEL, "MASK_ON", False):
+                t.update(MASK_ON=True, MRCNN_RESOLUTION=c.MRCNN.RESOLUTION, CLS_SPECIFIC_MASK=c.MRCNN.CLS_SPECIFIC_MASK)
         dev = rois.device
         im_info = torch.as_tensor(im_info, dtype=torch.float32)
         scales = im_info[:, 2].cpu()
-        per_image = []
+        mask_on = bool(t.get("MASK_ON", False))
+        per_image, sampled, num_fg = [], [], []
         for i, entry in enumerate(roidb):
             gt = torch.as_tensor(entry["boxes"], dtype=torch.float32).to(dev).reshape(-1, 4)
             gcls = torch.as_tensor(entry["gt_classes"]).to(device=dev, dtype=torch.int32).reshape(-1)
@@ -109,11 +115,13 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
             props = rois[rois[:, 0] == i][:, 1:5] * inv                              # add_proposals: back to image coordinates
             boxes = torch.cat([gt, props]).contiguous()
             fg_c, bg_c = (choices[i] if choices is not None else (None, None))
-            per_image.append(FR.sample_rois(boxes, gt, gcls, float(scales[i]), i, t["NUM_CLASSES"],
-                                            batch_size_per_im=t["BATCH_SIZE_PER_IM"], fg_fraction=t["FG_FRACTION"],
-                                            fg_thresh=t["FG_THRESH"], bg_thresh_hi=t["BG_THRESH_HI"], bg_thresh_lo=t["BG_THRESH_LO"],
-                                            bbox_reg_weights=t["BBOX_REG_WEIGHTS"], cls_agnostic_bbox_reg=t["CLS_AGNOSTIC_BBOX_REG"],
-                                            fg_choice=fg_c, bg_choice=bg_c))
+            b, nf = FR._sample_rois(boxes, gt, gcls, float(scales[i]), i, t["NUM_CLASSES"], t["BATCH_SIZE_PER_IM"], t["FG_FRACTION"],
+                                    t["FG_THRESH"], t["BG_THRESH_HI"], t["BG_THRESH_LO"], t["BBOX_REG_WEIGHTS"],
+                                    t["CLS_AGNOSTIC_BBOX_REG"], fg_c, bg_c, None)
+            per_image.append(b)
+            if mask_on:                                                              # add_mask_rcnn_blobs' sampled_boxes (unscaled)
+                sampled.append(boxes[b["keep_inds"].long()])
+                num_fg.append(nf)
         blobs = {k: torch.cat([b[k] for b in per_image]) for k in
                  ("labels_int32", "rois", "bbox_targets", "bbox_inside_weights", "bbox_outside_weights")}
         # roi_data/fast_rcnn.py:251-283 (_add_multilevel_rois): the sampled rois go to their FPN levels
@@ -121,4 +129,14 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
         for k, v in d.items():
             if k != "rois":
                 blobs[k] = v
+        if mask_on:
+            # roi_data/mask_rcnn.py:34-122 per image, concatenated, then fast_rcnn.py:275-276: mask_rois to their FPN levels
+            from detectron.pytorch_b200.roi_data import mask_rcnn as MR
+            mb = MR.mask_rcnn_blobs([b["labels_int32"] for b in per_image], [b["rois"] for b in per_image], sampled, num_fg, roidb,
+                                    t.get("MRCNN_RESOLUTION", 14), t.get("CLS_SPECIFIC_MASK", True), t["NUM_CLASSES"])
+            blobs.update(mb)
+            d = distribute(mb["mask_rois"], p["roi_min"], p["roi_max"], p["s0"], p["k0"])
+            for k, v in d.items():
+                if k not in ("rois", "counts"):
+                    blobs["mask_" + k] = v
         return blobs

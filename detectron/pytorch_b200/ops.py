@@ -672,6 +672,79 @@ def rpn_targets_raw(gt_boxes, gt_counts, im_sizes, levels, draw, straddle_thresh
     return outs
 
 
+MASK_COORD_LIMIT = float(2 ** 20)
+
+
+def pack_polygons(objects_per_image):
+    """Host packer for mask_targets_raw.  objects_per_image: per image, the list of its objects' polygon segmentations (roidb
+    `segms` entries: a list of polygons, each a flat [x0, y0, x1, y1, ...] coordinate list).  Returns numpy tables
+    (obj_begin (N + 1,), poly_begin (O + 1,), coord_begin (P + 1,) int32; coords (2V,) float32).
+    ValueError for an object without polygons, a polygon with fewer than 6 values or an odd count, non-finite coordinates and
+    coordinates beyond +-2^20.  The reference's pycocotools frPyObjects dispatches on the first polygon's length: 4 values
+    read every polygon of the object as [x, y, w, h] boxes, fewer fail, and an odd count silently drops the last value --
+    none of which is a polygon mask, so all are rejected here."""
+    import numpy as np
+    obj_begin, poly_begin, coord_begin, parts = [0], [0], [0], []
+    for objs in objects_per_image:
+        for polys in objs:
+            if isinstance(polys, dict) or not isinstance(polys, (list, tuple)) or len(polys) == 0:
+                raise ValueError("a non-crowd object needs a non-empty list of polygons, got %r" % (type(polys),))
+            for p in polys:
+                a = np.asarray(p, dtype=np.float64).reshape(-1)
+                if a.size < 6 or a.size % 2:
+                    raise ValueError("a polygon needs an even number (>= 6) of coordinates, got %d" % a.size)
+                if not np.isfinite(a).all():
+                    raise ValueError("non-finite polygon coordinate")
+                if np.abs(a).max() > MASK_COORD_LIMIT:
+                    raise ValueError("polygon coordinate beyond +-2^20")
+                parts.append(a.astype(np.float32))
+                coord_begin.append(coord_begin[-1] + a.size)
+            poly_begin.append(len(coord_begin) - 1)
+        obj_begin.append(len(poly_begin) - 1)
+    coords = np.concatenate(parts) if parts else np.zeros((0,), np.float32)
+    return (np.asarray(obj_begin, np.int32), np.asarray(poly_begin, np.int32), np.asarray(coord_begin, np.int32), coords)
+
+
+def mask_targets_raw(rois, roi_image, roi_class, packed, resolution, num_classes):
+    """Mask R-CNN training mask targets (lib/roi_data/mask_rcnn.py:34-122) for all RoIs of a step in one call (2 launches, no
+    device-to-host read).  rois: float32 CUDA (R, 4) unscaled (x1, y1, x2, y2); roi_image: host ints (R,) (image index);
+    roi_class: int32 CUDA (R,) -- a class <= 0 gives an all -1 row; packed: pack_polygons' tables; num_classes: 0 for
+    class-agnostic masks.  Returns masks_int32 (R, max(num_classes, 1) * M * M) on the device."""
+    import ctypes
+    import numpy as np
+    _need_cuda_f32(rois, "rois")
+    if rois.dim() != 2 or rois.size(1) != 4:
+        raise ValueError("rois must be (R, 4) = [x1, y1, x2, y2], got %s" % (tuple(rois.shape),))
+    if roi_class.dtype != torch.int32 or not roi_class.is_cuda:
+        raise TypeError("roi_class must be an int32 CUDA tensor")
+    obj_begin, poly_begin, coord_begin, coords = packed
+    R, M, K = rois.size(0), int(resolution), int(num_classes)
+    roi_image = np.asarray(roi_image, np.int32).reshape(-1)
+    if R == 0 or roi_image.size != R or roi_class.numel() != R:
+        raise ValueError("mask_targets_raw: %d RoIs, %d image indices, %d classes" % (R, roi_image.size, roi_class.numel()))
+    if not 1 <= M <= 64 or K < 0 or not 1 <= obj_begin.size - 1 <= 64:
+        raise ValueError("mask_targets_raw: resolution %d (1..64), num_classes %d (>= 0), %d images (1..64)" % (M, K, obj_begin.size - 1))
+    dev = rois.device
+    rois = rois.contiguous()
+    if rois.data_ptr() % 16:
+        rois = rois.clone()                                              # the kernel reads a RoI with one 16-byte load
+    roi_class = roi_class.contiguous()
+    O, P, C = poly_begin.size - 1, coord_begin.size - 1, coords.size
+    # one upload: roi_image | poly_begin | coord_begin | coords (as int32 bits)
+    host = np.concatenate([roi_image, poly_begin, coord_begin, coords.view(np.int32)])
+    buf = torch.from_numpy(host).pin_memory().to(dev, non_blocking=True)
+    ptr, i4 = buf.data_ptr(), 4
+    boxes = torch.empty((max(O, 1), 4), dtype=torch.float32, device=dev)
+    masks = torch.empty((R, max(K, 1) * M * M), dtype=torch.int32, device=dev)
+    ob = (ctypes.c_int * obj_begin.size)(*obj_begin.tolist())
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().b200_mask_targets(rois.data_ptr(), ptr, roi_class.data_ptr(), R,
+                                                 obj_begin.size - 1, ob, P, ptr + i4 * R, C, ptr + i4 * (R + O + 1),
+                                                 ptr + i4 * (R + O + P + 2), M, K, boxes.data_ptr(), masks.data_ptr(), _stream()),
+                   "b200_mask_targets")
+    return masks
+
+
 def nms_oks_raw(xy_preds, rois, thresh):
     """Greedy OKS NMS of lib/utils/keypoints.py:225-266 on (D, 4, 17) predictions and their (D, >=4) boxes, float32 CUDA.
     Returns (keep int32 (D,), num_keep int32 (1,)) on the device, no host sync: keep[:num_keep] are the kept indices in

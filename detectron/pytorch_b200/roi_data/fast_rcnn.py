@@ -4,7 +4,7 @@ Mirrors, for proposals that already live on the GPU, what the reference does per
   * `bbox_overlaps`          lib/utils/cython_bbox.pyx:32-73
   * `assign_rois`            lib/datasets/json_dataset.py:429-490 (_merge_proposal_boxes_into_roidb) + :514-531
   * `sample_rois`            lib/roi_data/fast_rcnn.py:129-200 (_sample_rois), :203-248 (_compute_targets, _expand_bbox_targets)
-Mask / keypoint targets (polygon rasterisation through pycocotools) stay on the host as in the reference.
+Mask targets are in roi_data/mask_rcnn.py (device polygon rasteriser); keypoint targets stay on the host as in the reference.
 
 The random choice of the reference (`npr.choice(inds, size, replace=False)` = a permutation prefix) is an INPUT here: pass
 the positions it picked (`fg_choice`, `bg_choice`, e.g. from the same numpy RandomState) for a bit-identical minibatch, or
@@ -78,6 +78,13 @@ def sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, b
     coordinates).  Returns the reference's blob dict with CUDA tensors: labels_int32, rois, bbox_targets,
     bbox_inside_weights, bbox_outside_weights (+ keep_inds, the rows of `boxes` that were sampled).
     assignment: (max_overlaps, box_to_gt_ind, max_classes) when the caller already has them (assign_rois)."""
+    return _sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, batch_size_per_im, fg_fraction, fg_thresh,
+                        bg_thresh_hi, bg_thresh_lo, bbox_reg_weights, cls_agnostic_bbox_reg, fg_choice, bg_choice, assignment)[0]
+
+
+def _sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, batch_size_per_im, fg_fraction, fg_thresh, bg_thresh_hi,
+                 bg_thresh_lo, bbox_reg_weights, cls_agnostic_bbox_reg, fg_choice, bg_choice, assignment):
+    """sample_rois' blobs and the number of fg rows (a host int; they come first)."""
     boxes = _boxes4(boxes, "boxes")
     dev = boxes.device
     if assignment is None:
@@ -120,4 +127,4 @@ def sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, b
                                                       labels.data_ptr(), rois.data_ptr(), targets.data_ptr(), inside.data_ptr(),
                                                       outside.data_ptr(), _stream()), "b200_fast_rcnn_targets")
     return dict(labels_int32=labels, rois=rois, bbox_targets=targets, bbox_inside_weights=inside, bbox_outside_weights=outside,
-                keep_inds=keep)
+                keep_inds=keep), n_fg

@@ -376,6 +376,28 @@ B200_API int b200_rpn_emit(int num_levels, const int* field_sizes_host, const in
                            size_t workspace_bytes, int* const* labels_out_host, float* const* bbox_targets_out_host,
                            float* const* inside_weights_out_host, float* const* outside_weights_out_host, b200_stream_t stream);
 
+/* ---- Mask R-CNN mask targets (training, lib/roi_data/mask_rcnn.py:34-122 with lib/utils/segms.py:93-131) -------------------
+ * add_mask_rcnn_blobs' masks_int32 for all images of a step, in 2 launches whatever the image, RoI, object or vertex count.
+ * RoIs: rois_dev (R, 4) float32 (x1, y1, x2, y2) in UNSCALED image coordinates (16-byte aligned), roi_image_dev (R,) int32
+ *   image index, roi_class_dev (R,) int32 class; R >= 1.  A RoI with class <= 0 (the reference's empty-fg fallback row), with
+ *   class >= num_classes (class-specific), or in an image without objects gets an all -1 row.
+ * Objects (HOST table, 1 <= num_images <= 64): image n's non-crowd objects are obj_begin_host[n] .. obj_begin_host[n + 1] - 1
+ *   (obj_begin_host[0] = 0, non-decreasing).  Object o's polygons are poly_begin_dev[o] .. poly_begin_dev[o + 1] - 1 (at least
+ *   one), polygon p's coordinates coords_dev[coord_begin_dev[p] .. coord_begin_dev[p + 1]) as float32 x, y pairs, packed in
+ *   order (coord_begin_dev[0] = 0, even, non-decreasing; num_polys + 1 and num_objects + 1 entries).  Coordinates must lie
+ *   within +-2^20 so the upsampled positions stay in int32.
+ * Per RoI with a class: the object whose tight polygon box (segms.py:120-131, written to obj_boxes_out_dev (num_objects, 4),
+ *   16-byte aligned) has the first maximum cython_bbox IoU (mask_rcnn.py:57-64); its polygons normalised to the RoI in float32
+ *   ((p - x1) * M / max(x2 - x1, 1), segms.py:104-110) and rasterised as pycocotools' rleFrPoly + decode on an M x M grid,
+ *   union over the polygons (segms.py:112-117).
+ * masks_out_dev int32 (R, num_classes * M * M), or (R, M * M) for num_classes = 0 (class-agnostic): the RoI's class slice
+ *   holds the [y][x] mask (0 / 1), every other element -1 (mask_rcnn.py:108-122).  16-byte aligned when the row length is a
+ *   multiple of 4.  1 <= resolution (M) <= 64.  Bad sizes, host tables or null pointers: B200_ROI_EINVAL before any launch. */
+B200_API int b200_mask_targets(const float* rois_dev, const int* roi_image_dev, const int* roi_class_dev, int num_rois, int num_images,
+                               const int* obj_begin_host, int num_polys, const int* poly_begin_dev, int num_coords, const int* coord_begin_dev,
+                               const float* coords_dev, int resolution, int num_classes, float* obj_boxes_out_dev, int* masks_out_dev,
+                               b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
