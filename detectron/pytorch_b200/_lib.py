@@ -122,6 +122,14 @@ _SIGNATURES = {
     "b200_mask_targets": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                          ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_int, ctypes.c_int] + [ctypes.c_void_p] * 2 +
                           [_stream_t]),
+    # (boxes, max_overlaps, box_to_gt, N, box_begin_host, gt_inds, gt_begin_host, keypoints, person_begin_host, K, fg_thresh,
+    #  candidates, counts, stream)
+    "b200_keypoint_candidates": (ctypes.c_int, [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 5 + [ctypes.c_int, ctypes.c_float] +
+                                 [ctypes.c_void_p] * 2 + [_stream_t]),
+    # (boxes, box_to_gt, N, box_begin_host, gt_inds, gt_begin_host, keypoints, person_begin_host, K, HS, candidates, counts, picks,
+    #  roi_begin_host, im_scales_host, batch_index_host, rois, locations, weights, stream)
+    "b200_keypoint_targets": (ctypes.c_int, [ctypes.c_void_p] * 2 + [ctypes.c_int] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 2 +
+                              [ctypes.c_void_p] * 9 + [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

@@ -86,6 +86,10 @@ int rpn_emit(int, const int*, const int*, const double*, const double*, int, con
              cudaStream_t);
 int mask_targets(const float*, const int*, const int*, int, int, const int*, int, const int*, int, const int*, const float*, int, int,
                  float*, int*, cudaStream_t);
+int keypoint_candidates(const float*, const float*, const int*, int, const int*, const int*, const int*, const int*, const int*, int, float,
+                        int*, int*, cudaStream_t);
+int keypoint_targets(const float*, const int*, int, const int*, const int*, const int*, const int*, const int*, int, int, const int*,
+                     const int*, const int*, const int*, const float*, const float*, float*, int*, float*, cudaStream_t);
 
 // B200_ROI_ALIGN_PATH=generic|tiled|stream|auto (default auto) -- test/benchmark override of the forward dispatch
 //   0 auto: streaming-strip path -> quad-strip path -> tiled path -> generic, each when it applies.  On H100 the streaming
@@ -666,6 +670,25 @@ int b200_mask_targets(const float* rois_dev, const int* roi_image_dev, const int
                       b200_stream_t stream) {
     return mask_targets(rois_dev, roi_image_dev, roi_class_dev, num_rois, num_images, obj_begin_host, num_polys, poly_begin_dev, num_coords,
                         coord_begin_dev, coords_dev, resolution, num_classes, obj_boxes_out_dev, masks_out_dev, (cudaStream_t)stream);
+}
+
+int b200_keypoint_candidates(const float* boxes_dev, const float* max_overlaps_dev, const int* box_to_gt_dev, int num_images,
+                             const int* box_begin_host, const int* gt_inds_dev, const int* gt_begin_host, const int* keypoints_dev,
+                             const int* person_begin_host, int num_keypoints, float fg_thresh, int* candidates_out_dev,
+                             int* counts_out_dev, b200_stream_t stream) {
+    return keypoint_candidates(boxes_dev, max_overlaps_dev, box_to_gt_dev, num_images, box_begin_host, gt_inds_dev, gt_begin_host,
+                               keypoints_dev, person_begin_host, num_keypoints, fg_thresh, candidates_out_dev, counts_out_dev,
+                               (cudaStream_t)stream);
+}
+
+int b200_keypoint_targets(const float* boxes_dev, const int* box_to_gt_dev, int num_images, const int* box_begin_host,
+                          const int* gt_inds_dev, const int* gt_begin_host, const int* keypoints_dev, const int* person_begin_host,
+                          int num_keypoints, int heatmap_size, const int* candidates_dev, const int* counts_dev, const int* picks_dev,
+                          const int* roi_begin_host, const float* im_scales_host, const float* batch_index_host, float* rois_out_dev,
+                          int* locations_out_dev, float* weights_out_dev, b200_stream_t stream) {
+    return keypoint_targets(boxes_dev, box_to_gt_dev, num_images, box_begin_host, gt_inds_dev, gt_begin_host, keypoints_dev,
+                            person_begin_host, num_keypoints, heatmap_size, candidates_dev, counts_dev, picks_dev, roi_begin_host,
+                            im_scales_host, batch_index_host, rois_out_dev, locations_out_dev, weights_out_dev, (cudaStream_t)stream);
 }
 
 }  // extern "C"

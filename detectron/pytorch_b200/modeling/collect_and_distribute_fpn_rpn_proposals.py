@@ -16,9 +16,13 @@ merged into every roidb entry behind its ground-truth boxes, best-gt assignment 
 crowd_thresh = 0 so nothing is filtered) and roi_data.fast_rcnn.add_fast_rcnn_blobs (_sample_rois per image, concatenation,
 _add_multilevel_rois).  Here the same blobs are produced on the device with roi_data/fast_rcnn.py (SURVEY.md 8f N4); the
 random draws are inputs (`choices`), see there.  With MODEL.MASK_ON the mask blobs (mask_rois, roi_has_mask_int32,
-masks_int32 and the mask_rois FPN blobs) come from roi_data/mask_rcnn.py, on the device too; keypoint blobs are not produced
-(KEYPOINTS_ON models keep the host path for those).
+masks_int32 and the mask_rois FPN blobs) come from roi_data/mask_rcnn.py, and with MODEL.KEYPOINTS_ON the keypoint blobs
+(keypoint_rois, keypoint_locations_int32, keypoint_weights, keypoint_loss_normalizer and the keypoint_rois FPN blobs) from
+roi_data/keypoint_rcnn.py, on the device too.  The keypoint candidates see the reference's merged roidb: a proposal keeps the
+assignment assign_rois gives it (the same one the Fast R-CNN blobs use), a ground-truth row maps to itself with overlap 1,
+or -1 when it is a crowd object.
 """
+import numpy as np
 import torch
 from torch import nn
 
@@ -80,8 +84,10 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
         'gt_classes' (G,); numpy or tensors), im_info = (N, 3) [height, width, scale]; `train` = the TRAIN / MODEL keys
         (dict, or taken from `cfg`): BATCH_SIZE_PER_IM, FG_FRACTION, FG_THRESH, BG_THRESH_HI, BG_THRESH_LO, NUM_CLASSES,
         BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG, and for Mask R-CNN MASK_ON, MRCNN_RESOLUTION (default 14), CLS_SPECIFIC_MASK
-        (default True), with the roidb entries' 'segms' and 'is_crowd'; choices = per image (fg_choice, bg_choice) or None
-        (device randperm)."""
+        (default True), with the roidb entries' 'segms' and 'is_crowd'; for Keypoint R-CNN KEYPOINTS_ON, HEATMAP_SIZE,
+        NUM_KEYPOINTS, IMS_PER_BATCH (default 2), MIN_KEYPOINT_COUNT (default 20), with the roidb entries' 'gt_keypoints'
+        (G, 3, K) and 'is_crowd' (where crowd objects exist); choices = per image (fg_choice, bg_choice) or, with keypoints,
+        (fg_choice, bg_choice, keypoint_choice), or None (device randperm)."""
         p = self._params()
         n = p["rpn_max"] - p["rpn_min"] + 1
         topn = int(p["topn"] * p["scale"] + 0.5)
@@ -101,11 +107,16 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
                      BBOX_REG_WEIGHTS=c.MODEL.BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG=c.MODEL.CLS_AGNOSTIC_BBOX_REG)
             if getattr(c.MODEL, "MASK_ON", False):
                 t.update(MASK_ON=True, MRCNN_RESOLUTION=c.MRCNN.RESOLUTION, CLS_SPECIFIC_MASK=c.MRCNN.CLS_SPECIFIC_MASK)
+            if getattr(c.MODEL, "KEYPOINTS_ON", False):
+                t.update(KEYPOINTS_ON=True, HEATMAP_SIZE=c.KRCNN.HEATMAP_SIZE, NUM_KEYPOINTS=c.KRCNN.NUM_KEYPOINTS,
+                         IMS_PER_BATCH=c.TRAIN.IMS_PER_BATCH, MIN_KEYPOINT_COUNT=c.KRCNN.MIN_KEYPOINT_COUNT_FOR_VALID_MINIBATCH)
         dev = rois.device
         im_info = torch.as_tensor(im_info, dtype=torch.float32)
         scales = im_info[:, 2].cpu()
         mask_on = bool(t.get("MASK_ON", False))
+        kp_on = bool(t.get("KEYPOINTS_ON", False))
         per_image, sampled, num_fg = [], [], []
+        kp_boxes, kp_overlaps, kp_map, kp_choices = [], [], [], []
         for i, entry in enumerate(roidb):
             gt = torch.as_tensor(entry["boxes"], dtype=torch.float32).to(dev).reshape(-1, 4)
             gcls = torch.as_tensor(entry["gt_classes"]).to(device=dev, dtype=torch.int32).reshape(-1)
@@ -114,10 +125,25 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
             inv = (torch.ones((), dtype=torch.float32) / scales[i]).item()           # json_dataset.py:420: 1. / scales[i] in float32
             props = rois[rois[:, 0] == i][:, 1:5] * inv                              # add_proposals: back to image coordinates
             boxes = torch.cat([gt, props]).contiguous()
-            fg_c, bg_c = (choices[i] if choices is not None else (None, None))
+            ch = tuple(choices[i]) if choices is not None else (None, None)
+            fg_c, bg_c = ch[0], ch[1]
+            assignment = FR.assign_rois(boxes, gt, gcls) if kp_on else None
             b, nf = FR._sample_rois(boxes, gt, gcls, float(scales[i]), i, t["NUM_CLASSES"], t["BATCH_SIZE_PER_IM"], t["FG_FRACTION"],
                                     t["FG_THRESH"], t["BG_THRESH_HI"], t["BG_THRESH_LO"], t["BBOX_REG_WEIGHTS"],
-                                    t["CLS_AGNOSTIC_BBOX_REG"], fg_c, bg_c, None)
+                                    t["CLS_AGNOSTIC_BBOX_REG"], fg_c, bg_c, assignment)
+            if kp_on:
+                # json_dataset.py:429-490 + :513-531 as add_keypoint_rcnn_blobs reads them: gt rows map to themselves (their roidb
+                # row) with overlap 1 (-1 for crowd), proposals to gt_inds[argmax] with their max IoU, -1 without overlap
+                cls_h = np.asarray(entry["gt_classes"]).reshape(-1)
+                gt_inds = np.where(cls_h > 0)[0]
+                crowd = np.asarray(entry["is_crowd"]).reshape(-1)[gt_inds] if "is_crowd" in entry else np.zeros(gt_inds.size, bool)
+                gi = torch.from_numpy(gt_inds.astype(np.int32)).to(dev)
+                G = gt_inds.size
+                mo, am = assignment[0][G:], assignment[1][G:]
+                kp_boxes.append(boxes)
+                kp_overlaps.append(torch.cat([torch.from_numpy(np.where(crowd != 0, -1.0, 1.0).astype(np.float32)).to(dev), mo]))
+                kp_map.append(torch.cat([gi, torch.where(am >= 0, gi[am.clamp(min=0).long()] if G else am, torch.full_like(am, -1))]))
+                kp_choices.append(ch[2] if len(ch) > 2 else None)
             per_image.append(b)
             if mask_on:                                                              # add_mask_rcnn_blobs' sampled_boxes (unscaled)
                 sampled.append(boxes[b["keep_inds"].long()])
@@ -139,4 +165,20 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
             for k, v in d.items():
                 if k not in ("rois", "counts"):
                     blobs["mask_" + k] = v
+        if kp_on:
+            # roi_data/keypoint_rcnn.py:33-96 for every image in one device call, then fast_rcnn.py:277-278: keypoint_rois to their
+            # FPN levels
+            from detectron.pytorch_b200.roi_data import keypoint_rcnn as KR
+            box_begin = np.concatenate([[0], np.cumsum([bx.size(0) for bx in kp_boxes])])
+            kb = KR.keypoint_rcnn_blobs(torch.cat(kp_boxes), box_begin, torch.cat(kp_overlaps), torch.cat(kp_map), roidb,
+                                        [float(s) for s in scales], int(round(t["FG_FRACTION"] * int(t["BATCH_SIZE_PER_IM"]))),
+                                        t["HEATMAP_SIZE"], t["NUM_KEYPOINTS"], t["FG_THRESH"], choices=kp_choices)
+            KR.finalize_keypoint_minibatch(kb, True, ims_per_batch=t.get("IMS_PER_BATCH", 2), batch_size_per_im=t["BATCH_SIZE_PER_IM"],
+                                           fg_fraction=t["FG_FRACTION"], num_keypoints=t["NUM_KEYPOINTS"],
+                                           min_count=t.get("MIN_KEYPOINT_COUNT", 20))
+            blobs.update(kb)
+            d = distribute(kb["keypoint_rois"], p["roi_min"], p["roi_max"], p["s0"], p["k0"])
+            for k, v in d.items():
+                if k not in ("rois", "counts"):
+                    blobs["keypoint_" + k] = v
         return blobs

@@ -745,6 +745,169 @@ def mask_targets_raw(rois, roi_image, roi_class, packed, resolution, num_classes
     return masks
 
 
+def _host_or_device(x, dtype, dev, name):
+    """A host array (returned as numpy, for the one upload) or a CUDA tensor of `dtype` (returned as is, contiguous)."""
+    import numpy as np
+    if torch.is_tensor(x):
+        if not x.is_cuda:
+            raise NotImplementedError("%s must be a CUDA tensor or a host array, not a CPU tensor" % name)
+        return x.to(device=dev, dtype=dtype).reshape(-1).contiguous()
+    return np.ascontiguousarray(np.asarray(x).reshape(-1).astype(np.float32 if dtype == torch.float32 else np.int32))
+
+
+def keypoint_targets_raw(boxes, box_begin, max_overlaps, box_to_gt_ind_map, gt_inds, gt_keypoints, im_scales, fg_rois_per_image, draw,
+                         heatmap_size, fg_thresh=0.5, batch_index=None, device=None):
+    """Keypoint R-CNN training targets (lib/roi_data/keypoint_rcnn.py:33-82 with lib/utils/keypoints.py:160-211) for N images
+    in one call: 2 launches and one host read, the N candidate counts.
+    boxes (B, 4) float32, max_overlaps (B,) float32, box_to_gt_ind_map (B,) int32: the merged roidb's (ground truth first, then
+    proposals; unscaled), image n's in rows box_begin[n] .. box_begin[n + 1] - 1 (host ints); each a CUDA tensor or a host
+    array.  gt_inds: per image, np.where(gt_classes > 0); gt_keypoints: per image (G_n, 3, K) int32 (x, y, v) host arrays.
+    im_scales: host (N,); batch_index: host (N,), default 0 .. N - 1.
+    draw(counts) is called once with the (N,) host candidate counts and returns, per image, None (the first
+    min(fg_rois_per_image, count) candidates in ascending order) or the positions in the candidate list that np.random.choice
+    picked (host ints or a CUDA tensor, min(fg_rois_per_image, count) of them).
+    A host box_to_gt_ind_map is checked against gt_inds first (numpy's IndexError becomes ValueError); a device one is read
+    with the same bounds, an out-of-range entry meaning no person.  Returns (keypoint_rois (R, 5) float32,
+    keypoint_locations_int32 (R * K,) int32, keypoint_weights (R * K,) float32, all CUDA; counts (N,) numpy)."""
+    import ctypes
+    import numpy as np
+    box_begin = np.asarray(box_begin, np.int64).reshape(-1)
+    N = box_begin.size - 1
+    if not 1 <= N <= 64 or box_begin[0] != 0 or (np.diff(box_begin) < 0).any():
+        raise ValueError("keypoint_targets_raw: box_begin must start at 0 and not decrease over 1..64 images, got %s" % box_begin.tolist())
+    if len(gt_inds) != N or len(gt_keypoints) != N or np.asarray(im_scales).size != N:
+        raise ValueError("keypoint_targets_raw: %d images but %d gt_inds, %d gt_keypoints, %d im_scales"
+                         % (N, len(gt_inds), len(gt_keypoints), np.asarray(im_scales).size))
+    HS, fg = int(heatmap_size), int(fg_rois_per_image)
+    kps = [np.asarray(k) for k in gt_keypoints]
+    K = kps[0].shape[2] if kps[0].ndim == 3 else -1
+    if any(k.ndim != 3 or k.shape[1] != 3 or k.shape[2] != K for k in kps) or not 1 <= K <= 64:
+        raise ValueError("gt_keypoints must be (G, 3, K) arrays with the same K in 1..64, got %s" % [k.shape for k in kps])
+    if not 1 <= HS <= 4096:
+        raise ValueError("heatmap_size %d outside 1..4096" % HS)
+    gis = [np.asarray(g, np.int64).reshape(-1) for g in gt_inds]
+    for n, (g, k) in enumerate(zip(gis, kps)):
+        if g.size and (g.min() < 0 or g.max() >= k.shape[0]):
+            raise ValueError("image %d: gt_inds out of range for %d keypoint rows" % (n, k.shape[0]))
+    B = int(box_begin[-1])
+    dev = device if device is not None else next((t.device for t in (boxes, max_overlaps, box_to_gt_ind_map) if torch.is_tensor(t)),
+                                                 torch.device("cuda", torch.cuda.current_device()))
+    bx = _host_or_device(boxes, torch.float32, dev, "boxes")
+    mo = _host_or_device(max_overlaps, torch.float32, dev, "max_overlaps")
+    bm = _host_or_device(box_to_gt_ind_map, torch.int32, dev, "box_to_gt_ind_map")
+    def size(a):
+        return a.numel() if torch.is_tensor(a) else a.size
+    if size(bx) != 4 * B:
+        raise ValueError("boxes must be (%d, 4)" % B)
+    if size(mo) != B or size(bm) != B:
+        raise ValueError("max_overlaps and box_to_gt_ind_map must have %d entries" % B)
+    if not torch.is_tensor(bm):
+        for n in range(N):
+            m, G = bm[box_begin[n]:box_begin[n + 1]], gis[n].size
+            if m.size and (m.min() < -G or m.max() >= G):
+                raise ValueError("image %d: box_to_gt_ind_map indexes gt_inds of size %d out of range (numpy: IndexError)" % (n, G))
+    # one upload: the host-side inputs, gt_inds, the keypoints (float32 as int32 bits), one pad so no part is at the very end
+    parts, offs = [], {}
+
+    def put(name, a):
+        offs[name] = sum(p.size for p in parts)
+        parts.append(a.view(np.int32) if a.dtype == np.float32 else a.astype(np.int32))
+    for name, a in (("boxes", bx), ("mo", mo), ("map", bm)):
+        if not torch.is_tensor(a):
+            put(name, a)
+    put("gt_inds", np.concatenate(gis) if any(g.size for g in gis) else np.zeros((0,), np.int32))
+    put("kps", np.concatenate([k.astype(np.int32).reshape(-1) for k in kps]))
+    parts.append(np.zeros((1,), np.int32))
+    buf = torch.from_numpy(np.concatenate(parts)).pin_memory().to(dev, non_blocking=True)
+    base = buf.data_ptr()
+
+    def ptr(name, a):
+        return a.data_ptr() if torch.is_tensor(a) else base + 4 * offs[name]
+
+    def tab(vals):
+        return (ctypes.c_int * len(vals))(*[int(v) for v in vals])
+    bb = tab(box_begin)
+    gb = tab(np.concatenate([[0], np.cumsum([g.size for g in gis])]))
+    pb = tab(np.concatenate([[0], np.cumsum([k.shape[0] for k in kps])]))
+    cand =torch.empty((max(B, 1),), dtype=torch.int32, device=dev)
+    counts = torch.empty((N,), dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        _lib.check(lib.b200_keypoint_candidates(ptr("boxes", bx), ptr("mo", mo), ptr("map", bm), N, bb, base + 4 * offs["gt_inds"], gb,
+                                                base + 4 * offs["kps"], pb, K, float(fg_thresh), cand.data_ptr(), counts.data_ptr(),
+                                                _stream()), "b200_keypoint_candidates")
+        counts_h = counts.cpu().numpy()
+        picks = list(draw(counts_h))
+        if len(picks) != N:
+            raise ValueError("draw returned %d entries for %d images" % (len(picks), N))
+        sizes = [min(fg, int(c)) for c in counts_h]
+        sel = []
+        for n, (pk, size) in enumerate(zip(picks, sizes)):
+            if pk is None:
+                sel.append(torch.arange(size, dtype=torch.int32))
+                continue
+            pk = pk.reshape(-1) if torch.is_tensor(pk) else torch.from_numpy(np.asarray(pk, np.int64).reshape(-1))
+            if pk.numel() != size:
+                raise ValueError("image %d: %d keypoint draw positions, the minibatch takes %d" % (n, pk.numel(), size))
+            if not pk.is_cuda and size and (int(pk.min()) < 0 or int(pk.max()) >= int(counts_h[n])):
+                raise ValueError("image %d: keypoint draw positions outside 0..%d" % (n, int(counts_h[n]) - 1))
+            sel.append(pk)
+        if all(not p.is_cuda for p in sel):
+            flat = torch.cat([p.to(torch.int32) for p in sel] + [torch.zeros((1,), dtype=torch.int32)]).to(dev)
+        else:
+            flat = torch.cat([p.to(device=dev, dtype=torch.int32) for p in sel] + [torch.zeros((1,), dtype=torch.int32, device=dev)])
+        R = sum(sizes)
+        rb = tab(np.concatenate([[0], np.cumsum(sizes)]))
+        sc = (ctypes.c_float * N)(*[float(np.float32(s)) for s in np.asarray(im_scales).reshape(-1)])
+        bi = (ctypes.c_float * N)(*[float(np.float32(b)) for b in (np.arange(N) if batch_index is None else np.asarray(batch_index).reshape(-1))])
+        rois = torch.empty((max(R, 1), 5), dtype=torch.float32, device=dev)
+        loc = torch.empty((max(R * K, 1),), dtype=torch.int32, device=dev)
+        w = torch.empty((max(R * K, 1),), dtype=torch.float32, device=dev)
+        _lib.check(lib.b200_keypoint_targets(ptr("boxes", bx), ptr("map", bm), N, bb, base + 4 * offs["gt_inds"], gb, base + 4 * offs["kps"],
+                                             pb, K, HS, cand.data_ptr(), counts.data_ptr(), flat.data_ptr(), rb, sc, bi, rois.data_ptr(),
+                                             loc.data_ptr(), w.data_ptr(), _stream()), "b200_keypoint_targets")
+    return rois[:R], loc[:R * K], w[:R * K], counts_h
+
+
+def keypoints_to_heatmap_labels_raw(keypoints, rois, heatmap_size):
+    """keypoints_to_heatmap_labels (lib/utils/keypoints.py:160-211) for R given RoIs: keypoints (R, 3, K) int32 (host array or
+    CUDA tensor), rois CUDA float32 (R, >=4) = [x1, y1, x2, y2].  Returns (heats (R, K) int32 = the reference's result after
+    `.astype(np.int32)`, weights (R, K) float32), CUDA.  One launch (the emit of keypoint_targets_raw, each RoI its own
+    candidate)."""
+    import ctypes
+    import numpy as np
+    _need_cuda_f32(rois, "rois")
+    if rois.dim() != 2 or rois.size(1) < 4:
+        raise ValueError("rois must be (R, >=4) = [x1, y1, x2, y2, ...], got %s" % (tuple(rois.shape),))
+    dev = rois.device
+    kp = keypoints.to(device=dev, dtype=torch.int32) if torch.is_tensor(keypoints) else \
+        torch.from_numpy(np.ascontiguousarray(np.asarray(keypoints).astype(np.int32))).to(dev)
+    R = rois.size(0)
+    if kp.dim() != 3 or kp.size(0) != R or kp.size(1) != 3 or not 1 <= kp.size(2) <= 64:
+        raise ValueError("keypoints must be (%d, 3, K) with K in 1..64, got %s" % (R, tuple(kp.shape)))
+    K, HS = kp.size(2), int(heatmap_size)
+    if not 1 <= HS <= 4096:
+        raise ValueError("heatmap_size %d outside 1..4096" % HS)
+    if R == 0:
+        return torch.empty((0, K), dtype=torch.int32, device=dev), torch.empty((0, K), dtype=torch.float32, device=dev)
+    boxes = rois[:, :4].contiguous()
+    kp = kp.contiguous()
+    ident = torch.arange(R + 1, dtype=torch.int32, device=dev)            # map, gt_inds, candidates and picks; ident[R] = count
+    ident[R] = R
+    tab = (ctypes.c_int * 2)(0, R)
+    one = (ctypes.c_float * 1)(1.0)
+    zero = (ctypes.c_float * 1)(0.0)
+    rows = torch.empty((R, 5), dtype=torch.float32, device=dev)
+    heats = torch.empty((R, K), dtype=torch.int32, device=dev)
+    weights = torch.empty((R, K), dtype=torch.float32, device=dev)
+    p = ident.data_ptr()
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().b200_keypoint_targets(boxes.data_ptr(), p, 1, tab, p, tab, kp.data_ptr(), tab, K, HS, p, p + 4 * R, p, tab, one,
+                                                     zero, rows.data_ptr(), heats.data_ptr(), weights.data_ptr(), _stream()),
+                   "b200_keypoint_targets")
+    return heats, weights
+
+
 def nms_oks_raw(xy_preds, rois, thresh):
     """Greedy OKS NMS of lib/utils/keypoints.py:225-266 on (D, 4, 17) predictions and their (D, >=4) boxes, float32 CUDA.
     Returns (keep int32 (D,), num_keep int32 (1,)) on the device, no host sync: keep[:num_keep] are the kept indices in

@@ -4,7 +4,7 @@ Mirrors, for proposals that already live on the GPU, what the reference does per
   * `bbox_overlaps`          lib/utils/cython_bbox.pyx:32-73
   * `assign_rois`            lib/datasets/json_dataset.py:429-490 (_merge_proposal_boxes_into_roidb) + :514-531
   * `sample_rois`            lib/roi_data/fast_rcnn.py:129-200 (_sample_rois), :203-248 (_compute_targets, _expand_bbox_targets)
-Mask targets are in roi_data/mask_rcnn.py (device polygon rasteriser); keypoint targets stay on the host as in the reference.
+Mask targets are in roi_data/mask_rcnn.py (device polygon rasteriser), keypoint targets in roi_data/keypoint_rcnn.py.
 
 The random choice of the reference (`npr.choice(inds, size, replace=False)` = a permutation prefix) is an INPUT here: pass
 the positions it picked (`fg_choice`, `bg_choice`, e.g. from the same numpy RandomState) for a bit-identical minibatch, or

@@ -1,6 +1,8 @@
 """Host-array front door of the device keypoint extraction, named like the reference's `utils.keypoints`
 (lib/utils/keypoints.py): `heatmaps_to_keypoints(maps, rois)` (:103-157) and `nms_oks(kp_predictions, rois, thresh)`
 (:225-266).  Both take numpy arrays like the reference's or CUDA tensors, and return numpy results.
+`keypoints_to_heatmap_labels(keypoints, rois)` (:160-211), the training-time labels, returns CUDA tensors (the loss reads
+them on the device).
 
 The resize, argmax and coordinates reproduce the reference's numpy 2 / cv2 float32 INTER_CUBIC arithmetic bit for bit;
 prob (the spatial softmax at the maximum) is summed in double on the device where numpy sums float32 pairwise, so it
@@ -39,3 +41,16 @@ def nms_oks(kp_predictions, rois, thresh):
     dev = _device_of(kp_predictions, rois)
     keep, num_keep = ops.nms_oks_raw(_f32(kp_predictions, dev), _f32(rois, dev), thresh)
     return keep[:int(num_keep.item())].cpu().tolist()
+
+
+def keypoints_to_heatmap_labels(keypoints, rois, heatmap_size=None, cfg=None):
+    """The training-time labels of lib/utils/keypoints.py:160-211 on the device: keypoints (R, 3, K) int32 (x, y, v), rois (R, >=4)
+    float32 [x1, y1, x2, y2] (numpy or CUDA; computed in float32 as the reference's float32 roidb boxes are).  heatmap_size is
+    KRCNN.HEATMAP_SIZE (or taken from cfg).  Returns (heats, weights) as CUDA (R, K) tensors: heats int32 -- the reference's
+    float32 labels after the caller's `.astype(np.int32)`, INT_MIN where they are NaN -- and weights float32 (0 / 1)."""
+    if heatmap_size is None:
+        if cfg is None:
+            raise ValueError("keypoints_to_heatmap_labels needs heatmap_size (or cfg=)")
+        heatmap_size = cfg.KRCNN.HEATMAP_SIZE
+    dev = _device_of(keypoints, rois)
+    return ops.keypoints_to_heatmap_labels_raw(keypoints, _f32(rois, dev), heatmap_size)

@@ -398,6 +398,39 @@ B200_API int b200_mask_targets(const float* rois_dev, const int* roi_image_dev, 
                                const float* coords_dev, int resolution, int num_classes, float* obj_boxes_out_dev, int* masks_out_dev,
                                b200_stream_t stream);
 
+/* ---- Keypoint R-CNN keypoint targets (training, lib/roi_data/keypoint_rcnn.py:33-82 with lib/utils/keypoints.py:160-211) ---
+ * add_keypoint_rcnn_blobs for all images of a step in 2 launches (one per call) whatever the image, box or person count, with
+ * the caller's draw in between.  Shared inputs (1 <= num_images <= 64, HOST tables starting at 0 and non-decreasing):
+ *   boxes_dev (B, 4) float32 (x1, y1, x2, y2) UNSCALED, image n's merged roidb boxes in rows box_begin_host[n] .. [n + 1] - 1
+ *   (ground truth first, then proposals; B <= 2^29); box_to_gt_dev (B,) int32 = roidb['box_to_gt_ind_map'] (an index into the
+ *   image's gt_inds, numpy-style: -1 is the last entry; out of range: no person); gt_inds_dev = each image's
+ *   np.where(gt_classes > 0), rows gt_begin_host[n] .. [n + 1] - 1, values indexing the image's keypoint rows;
+ *   keypoints_dev (P, 3, K) int32 = every image's gt_keypoints (x, y, v rows), image n's in rows person_begin_host[n] .. [n + 1]
+ *   - 1.  1 <= num_keypoints (K) <= 64.
+ * b200_keypoint_candidates (keypoint_rcnn.py:37-51): box b of image n is a candidate when max_overlaps_dev[b] >= fg_thresh
+ *   (float32) and its person has a keypoint with v > 0 inside the box, ends included, compared in double (_within_box).
+ *   candidates_out_dev (B,) int32: image n's candidates as ascending image-relative box indices from row box_begin_host[n];
+ *   counts_out_dev (N,) int32: their number per image.  Nothing else is written.
+ * b200_keypoint_targets (keypoint_rcnn.py:59-82): image n's selected RoIs are rows roi_begin_host[n] .. [n + 1] - 1 (never more
+ *   than the image's boxes); picks_dev[r] is the position of RoI r in its image's candidate list (< counts_dev[n], else the row
+ *   is unspecified).  Per (RoI r, keypoint k), with the person's keypoints (all -1 when box_to_gt < 0), in float32:
+ *   s = HS / (x2 - x1), floor((x - x1) * s), HS - 1 when x == x2 (the same for y); valid = 0 <= x, y < HS and v > 0;
+ *   locations_out_dev[r * K + k] int32 = y * HS + x when valid, else 0, or INT_MIN where that product is not finite (numpy's
+ *   astype(int32) of NaN); weights_out_dev[r * K + k] float32 = valid.  rois_out_dev (R, 5) float32 = batch_index_host[n], then
+ *   the box times im_scales_host[n] (float32 multiply).  1 <= heatmap_size (HS) <= 4096, R * K < 2^31.  Every output element is
+ *   written once; with R = 0 the launch writes nothing (the pointers must still be valid).
+ * Bad sizes, host tables or null pointers: B200_ROI_EINVAL before any launch. */
+B200_API int b200_keypoint_candidates(const float* boxes_dev, const float* max_overlaps_dev, const int* box_to_gt_dev, int num_images,
+                                      const int* box_begin_host, const int* gt_inds_dev, const int* gt_begin_host, const int* keypoints_dev,
+                                      const int* person_begin_host, int num_keypoints, float fg_thresh, int* candidates_out_dev,
+                                      int* counts_out_dev, b200_stream_t stream);
+B200_API int b200_keypoint_targets(const float* boxes_dev, const int* box_to_gt_dev, int num_images, const int* box_begin_host,
+                                   const int* gt_inds_dev, const int* gt_begin_host, const int* keypoints_dev, const int* person_begin_host,
+                                   int num_keypoints, int heatmap_size, const int* candidates_dev, const int* counts_dev,
+                                   const int* picks_dev, const int* roi_begin_host, const float* im_scales_host,
+                                   const float* batch_index_host, float* rois_out_dev, int* locations_out_dev, float* weights_out_dev,
+                                   b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
