@@ -130,6 +130,9 @@ _SIGNATURES = {
     #  roi_begin_host, im_scales_host, batch_index_host, rois, locations, weights, stream)
     "b200_keypoint_targets": (ctypes.c_int, [ctypes.c_void_p] * 2 + [ctypes.c_int] + [ctypes.c_void_p] * 5 + [ctypes.c_int] * 2 +
                               [ctypes.c_void_p] * 9 + [_stream_t]),
+    # (src, descs, N, mean_table, blob_h, blob_w, out, stream)
+    "b200_image_blob": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
+                                       _c_float_p, _stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

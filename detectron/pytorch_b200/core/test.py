@@ -29,6 +29,9 @@ read of the per-detection sizes; the result is the reference's list of COCO RLE 
 `keypoint_results(cls_boxes, pred_heatmaps, ref_boxes)` is the Keypoint R-CNN step (lib/core/test.py:850-866): every
 detection's 17 heatmaps are resized, searched for their maximum and soft-maxed on the device in one launch (plus one for
 the optional OKS NMS), with one host read of the (R, 4, 17) result; the result is the reference's cls_keyps.
+
+`get_blobs(im, rois, target_scale, target_max_size)` is _get_blobs with _get_rois_blob (lib/core/test.py:869-929): the `data` blob
+is built on the device from the uint8 image (utils/blob.py).
 """
 import numpy as np
 import torch
@@ -221,3 +224,17 @@ def keypoint_results(cls_boxes, pred_heatmaps, ref_boxes, cfg=None, **kw):
         cls_boxes[PERSON_CLASS_INDEX] = cls_boxes[PERSON_CLASS_INDEX][keep, :]
     cls_keyps[PERSON_CLASS_INDEX] = [xy_preds[i] for i in range(xy_preds.shape[0])]
     return cls_keyps
+
+
+def get_blobs(im, rois, target_scale, target_max_size, cfg=None, **kw):
+    """_get_blobs with _get_rois_blob (lib/core/test.py:869-929): blobs['data'] is the device image blob (utils/blob.py),
+    blobs['im_info'] the float32 (1, 3) numpy (Hp, Wp, im_scale); with rois (R, 4) in image coordinates, blobs['rois'] is
+    the float32 (R, 5) [0, x1, y1, x2, y2] projection, multiplied in float64 like _project_im_rois.  Returns (blobs, im_scale)."""
+    from ..utils import blob as blob_utils
+    blobs = {}
+    blobs["data"], im_scale, blobs["im_info"] = blob_utils.get_image_blob(im, target_scale, target_max_size, cfg, **kw)
+    if rois is not None:
+        r = np.asarray(rois).astype(np.float64, copy=False) * im_scale
+        levels = np.zeros((r.shape[0], 1), dtype=np.int64)
+        blobs["rois"] = np.hstack((levels, r)).astype(np.float32, copy=False)
+    return blobs, im_scale

@@ -90,6 +90,7 @@ int keypoint_candidates(const float*, const float*, const int*, int, const int*,
                         int*, int*, cudaStream_t);
 int keypoint_targets(const float*, const int*, int, const int*, const int*, const int*, const int*, const int*, int, int, const int*,
                      const int*, const int*, const int*, const float*, const float*, float*, int*, float*, cudaStream_t);
+int image_blob(const unsigned char*, const b200_image_blob_desc*, int, const float*, int, int, float*, cudaStream_t);
 
 // B200_ROI_ALIGN_PATH=generic|tiled|stream|auto (default auto) -- test/benchmark override of the forward dispatch
 //   0 auto: streaming-strip path -> quad-strip path -> tiled path -> generic, each when it applies.  On H100 the streaming
@@ -689,6 +690,11 @@ int b200_keypoint_targets(const float* boxes_dev, const int* box_to_gt_dev, int 
     return keypoint_targets(boxes_dev, box_to_gt_dev, num_images, box_begin_host, gt_inds_dev, gt_begin_host, keypoints_dev,
                             person_begin_host, num_keypoints, heatmap_size, candidates_dev, counts_dev, picks_dev, roi_begin_host,
                             im_scales_host, batch_index_host, rois_out_dev, locations_out_dev, weights_out_dev, (cudaStream_t)stream);
+}
+
+int b200_image_blob(const unsigned char* src_dev, const b200_image_blob_desc* descs_dev, int num_images, const float* mean_table_dev,
+                    int blob_h, int blob_w, float* out_dev, b200_stream_t stream) {
+    return image_blob(src_dev, descs_dev, num_images, mean_table_dev, blob_h, blob_w, out_dev, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -92,6 +92,32 @@ __device__ __forceinline__ AxisTap xfrom_axis(float v, int size) {
     return t;
 }
 
+// ---- one axis of cv2.resize's float32 INTER_LINEAR (imgproc resize.cpp, IPP off) ----------------------------------------
+// Output index d, scale = 1 / inv_scale in double: f = float((d + .5) * scale - .5), s = floor(f), f -= s.  On the x axis
+// (clamp) a position before the first / past the last source column is clamped to it with f = 0; on the y axis f is kept
+// and both indices s, s + 1 are clipped into [0, src).  Weights w0 = 1 - f, w1 = f.
+struct Cv2Tap {
+    int s0, s1;
+    float w0, w1;
+};
+
+__device__ __forceinline__ Cv2Tap cv2_linear_tap(long long d, double scale, int src, bool clamp) {
+    float f = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, .5), scale), .5));
+    const float fl = floorf(f);
+    int s = (int)fl;
+    f = __fsub_rn(f, fl);
+    if (clamp) {
+        if (s < 0) { f = 0.f; s = 0; }
+        if (s >= src - 1) { f = 0.f; s = src - 1; }
+    }
+    Cv2Tap t;
+    t.s0 = s < 0 ? 0 : (s > src - 1 ? src - 1 : s);
+    t.s1 = s + 1 < 0 ? 0 : (s + 1 > src - 1 ? src - 1 : s + 1);
+    t.w0 = __fsub_rn(1.f, f);
+    t.w1 = f;
+    return t;
+}
+
 // ---- IoU exactly as the reference's compiled Cython computes it (lib/utils/cython_bbox.pyx:52-72) ----------------------
 // The generated C adds the literal 1.0 as a DOUBLE: widths / heights are (double)(float difference) + 1.0, their products and the
 // union are formed in double (separate multiply and add: x86-64 baseline has no FMA) and rounded to float once on assignment

@@ -62,28 +62,11 @@ __device__ SegmGeom segm_geom(const float* __restrict__ box, int M, int im_h, in
     return g;
 }
 
-struct Tap {
-    int s0, s1;
-    float w0, w1;
-};
+using Tap = Cv2Tap;
 
-// one axis of cv2's INTER_LINEAR: output index d of dst, source length src
+// one axis of cv2's INTER_LINEAR resized to a size (dsize): output index d of dst, source length src
 __device__ __forceinline__ Tap linear_tap(long long d, long long dst, int src, bool clamp) {
-    const double scale = __ddiv_rn(1.0, __ddiv_rn((double)dst, (double)src));
-    float f = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, .5), scale), .5));
-    const float fl = floorf(f);
-    int s = (int)fl;
-    f = __fsub_rn(f, fl);
-    if (clamp) {
-        if (s < 0) { f = 0.f; s = 0; }
-        if (s >= src - 1) { f = 0.f; s = src - 1; }
-    }
-    Tap t;
-    t.s0 = s < 0 ? 0 : (s > src - 1 ? src - 1 : s);
-    t.s1 = s + 1 < 0 ? 0 : (s + 1 > src - 1 ? src - 1 : s + 1);
-    t.w0 = __fsub_rn(1.f, f);
-    t.w1 = f;
-    return t;
+    return cv2_linear_tap(d, __ddiv_rn(1.0, __ddiv_rn((double)dst, (double)src)), src, clamp);
 }
 
 // resized value at window pixel (dx, dy) of the box (tx: the x tap of column dx, unused on the 2x path)

@@ -927,3 +927,104 @@ def nms_oks_raw(xy_preds, rois, thresh):
                                             _stream()),
                    "b200_nms_oks")
     return keep, num_keep
+
+
+# ------------------------------------------------------------------------------------------------
+# Input image blob (lib/utils/blob.py:37-148, lib/roi_data/minibatch.py:47-79)
+# ------------------------------------------------------------------------------------------------
+# b200_image_blob_desc of include/b200_roi_ops.h
+_BLOB_DESC = [("src_offset", "<i8"), ("row_pitch", "<i8"), ("inv_scale", "<f8"), ("height", "<i4"), ("width", "<i4"),
+              ("out_h", "<i4"), ("out_w", "<i4"), ("flipped", "<i4"), ("area2x", "<i4"), ("slot", "<i4"), ("reserved", "<i4")]
+
+
+def pixel_mean_table(pixel_means):
+    """(3, 256) float32: channel c of a uint8 value v after the reference's `im = im.astype(np.float32); im -= pixel_means`
+    (with the default float64 means, float32(float64(v) - mean)), evaluated by numpy itself."""
+    import numpy as np
+    t = np.empty((256, 1, 3), np.float32)
+    t[...] = np.arange(256, dtype=np.float32).reshape(256, 1, 1)
+    t -= np.asarray(pixel_means)
+    return np.ascontiguousarray(t.reshape(256, 3).T)
+
+
+def resized_size(h, w, im_scale):
+    """cv2.resize's output size for fx = fy = im_scale: (rint(h * s), rint(w * s)), half to even.  A zero side raises
+    ValueError where cv2 raises."""
+    import numpy as np
+    oh, ow = int(np.rint(h * float(im_scale))), int(np.rint(w * float(im_scale)))
+    if oh <= 0 or ow <= 0:
+        raise ValueError("resizing a %d x %d image by %r leaves an empty side (cv2.resize raises)" % (h, w, im_scale))
+    return oh, ow
+
+
+def image_blob_raw(images, scales, flipped, pixel_means, stride, out=None):
+    """The network's input blob for all images of a call in one launch: image i (uint8 (H, W, 3) BGR, a host array or a CUDA
+    tensor) flipped when flipped[i] (im[:, ::-1, :]), minus pixel_means, resized by scales[i] like cv2.resize(fx = fy,
+    INTER_LINEAR) with IPP off, zero-padded to the largest resized size (rounded up to a multiple of `stride` when it is not
+    None: FPN.COARSEST_STRIDE) and stored NCHW.  Host images go up in one asynchronous copy from one pinned buffer; CUDA
+    images are read where they are.  Returns (blob float32 CUDA (N, 3, Hp, Wp), [(h, w) resized size per image]).
+    `out`: an optional float32 CUDA tensor of that shape to write into (every element is written)."""
+    import numpy as np
+    N = len(images)
+    if N < 1 or len(scales) != N or len(flipped) != N:
+        raise ValueError("image_blob_raw: %d images, %d scales, %d flip flags" % (N, len(scales), len(flipped)))
+    dev = next((im.device for im in images if torch.is_tensor(im) and im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
+    descs = np.zeros((N,), dtype=_BLOB_DESC)
+    host, host_bytes, cuda_ims, sizes = [], 0, [], []
+    for i, im in enumerate(images):
+        on_dev = torch.is_tensor(im) and im.is_cuda
+        if not on_dev:
+            im = np.ascontiguousarray(im.numpy() if torch.is_tensor(im) else im)
+        dtype_ok = im.dtype == torch.uint8 if on_dev else im.dtype == np.uint8
+        if not dtype_ok or len(im.shape) != 3 or im.shape[2] != 3 or im.shape[0] < 1 or im.shape[1] < 1:
+            raise ValueError("image %d must be a uint8 (H, W, 3) image, got %s %s" % (i, im.dtype, tuple(im.shape)))
+        if on_dev:
+            if im.device != dev:
+                raise ValueError("image_blob_raw: images on %s and %s" % (dev, im.device))
+            if im.stride(2) != 1 or im.stride(1) != 3:
+                im = im.contiguous()
+            cuda_ims.append((i, im))
+        else:
+            host.append((i, im, host_bytes))
+            host_bytes += (im.nbytes + 15) & ~15
+        H, W = int(im.shape[0]), int(im.shape[1])
+        s = float(scales[i])
+        oh, ow = resized_size(H, W, s)
+        d = descs[i]
+        d["height"], d["width"], d["out_h"], d["out_w"] = H, W, oh, ow
+        d["row_pitch"] = im.stride(0) if on_dev else im.strides[0]
+        d["inv_scale"] = 1.0 if (oh, ow) == (H, W) else 1.0 / s          # an unchanged size is a copy in cv2
+        d["area2x"] = int(1.0 / s == 2.0)
+        d["flipped"] = int(bool(flipped[i]))
+        d["slot"] = i
+        sizes.append((oh, ow))
+    Hp, Wp = max(h for h, _ in sizes), max(w for _, w in sizes)
+    if stride:
+        Hp, Wp = int(np.ceil(Hp / float(stride)) * stride), int(np.ceil(Wp / float(stride)) * stride)
+    if out is None:
+        out = torch.empty((N, 3, Hp, Wp), dtype=torch.float32, device=dev)
+    elif not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (N, 3, Hp, Wp) and out.device == dev):
+        raise ValueError("out must be a contiguous float32 CUDA tensor of shape %s on %s" % ((N, 3, Hp, Wp), dev))
+    # one pinned staging buffer -- descriptors | mean table | host images, 16-byte aligned -- and one H2D copy into `buf`;
+    # CUDA images are addressed relative to buf's base
+    table = pixel_mean_table(pixel_means)
+    head = descs.nbytes + table.nbytes
+    buf = torch.empty((head + host_bytes,), dtype=torch.uint8, device=dev)
+    base = buf.data_ptr()
+    for i, im, off in host:
+        descs[i]["src_offset"] = head + off
+    for i, im in cuda_ims:
+        descs[i]["src_offset"] = im.data_ptr() - base
+    staging = torch.empty((head + host_bytes,), dtype=torch.uint8, pin_memory=True)
+    st = staging.numpy()
+    st[:descs.nbytes] = descs.view(np.uint8)
+    st[descs.nbytes:head] = table.view(np.uint8).reshape(-1)
+    for i, im, off in host:
+        st[head + off:head + off + im.nbytes] = im.reshape(-1)
+    with torch.cuda.device(dev):
+        # Asynchronous: torch's pinned-memory allocator records this copy on the stream and does not hand `staging` out again
+        # before it has completed, so dropping the last reference on return is safe.
+        buf.copy_(staging, non_blocking=True)
+        _lib.check(_lib.load().b200_image_blob(base, base, N, base + descs.nbytes, Hp, Wp, out.data_ptr(), _stream()),
+                   "b200_image_blob")
+    return out, sizes

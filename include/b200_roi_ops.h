@@ -431,6 +431,35 @@ B200_API int b200_keypoint_targets(const float* boxes_dev, const int* box_to_gt_
                                    const float* batch_index_host, float* rois_out_dev, int* locations_out_dev, float* weights_out_dev,
                                    b200_stream_t stream);
 
+/* ---- input image blob (lib/utils/blob.py:37-148, lib/roi_data/minibatch.py:47-79, lib/roi_data/loader.py:251-260) ----------
+ * The network's `data` blob for all images of a call in ONE launch, whatever their number and sizes: per image the decoded
+ * uint8 BGR image, optionally flipped (im[:, ::-1, :]), minus PIXEL_MEANS, resized like cv2.resize(fx = fy = im_scale,
+ * INTER_LINEAR) with IPP off, zero-padded and transposed to NCHW.
+ * Image i is described by descs_dev[i] (a DEVICE array of num_images entries, 1 <= num_images <= 65535):
+ *   src_offset   byte offset of its first pixel from src_dev; pixel (y, x) channel c is src_dev[src_offset + y * row_pitch + 3 x + c];
+ *   height, width  its size (>= 1); row_pitch >= 3 * width;
+ *   out_h, out_w   the resized size, cv2's (rint(height * im_scale), rint(width * im_scale)), at most blob_h x blob_w;
+ *   inv_scale    1 / im_scale in double (cv2's scale; 1.0 when the resized size equals the input size: cv2 copies);
+ *   flipped      non-zero: read source column width - 1 - s where the unflipped image reads s;
+ *   area2x       non-zero when inv_scale == 2.0 exactly: cv2's fast INTER_AREA path;
+ *   slot         its index in the output batch.  The slots of the call must be 0 .. num_images - 1, each once.
+ * mean_table_dev (3, 256) float32: channel c of a pixel of value v after `im -= PIXEL_MEANS` (numpy's float32(float64(v) - mean)).
+ * out_dev (num_images, 3, blob_h, blob_w) float32: every element written once, 0 outside each image's out_h x out_w; 16-byte
+ *   stores when blob_w % 4 == 0 and out_dev is 16-byte aligned.  blob_h * blob_w < 2^31.
+ * Bad sizes or null pointers: B200_ROI_EINVAL before any launch (the descriptors live on the device and are not read by the host). */
+typedef struct b200_image_blob_desc {
+    long long src_offset;
+    long long row_pitch;
+    double inv_scale;
+    int height, width;
+    int out_h, out_w;
+    int flipped, area2x;
+    int slot, reserved;
+} b200_image_blob_desc;
+
+B200_API int b200_image_blob(const unsigned char* src_dev, const b200_image_blob_desc* descs_dev, int num_images, const float* mean_table_dev,
+                             int blob_h, int blob_w, float* out_dev, b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
