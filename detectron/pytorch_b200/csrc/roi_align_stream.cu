@@ -19,17 +19,21 @@
 // output element is computed by one lane in the reference's own operation order and written exactly once
 // with a plain store: bit-identical to the reference kernel, deterministic, no zero-fill of the output.
 // Only bins whose samples cannot be resident together (x-span beyond the strip halo, y-span beyond the
-// ring) are cut into per-sample fragments that accumulate with red.global.add onto elements the fill
-// kernel zeroed (at most two partial sums per element -> still deterministic).
+// ring) are cut into per-sample fragments that accumulate with red.global.add onto elements the
+// prepass zeroed (at most two partial sums per element -> still deterministic).
 //
-// Prepass (channel independent, two small kernels): `count` builds the per-RoI axis tables (all IEEE
-// divisions; ring-slot byte offsets precomputed) and a histogram of fragments per (image, strip, row); its
-// last CTA scans the histogram (CSR row pointers) and cuts the linear space into one piece per SM of equal
-// estimated cost; `fill` writes the 8-byte fragment records into the CSR.
+// Prepass (channel independent): `clear` zeroes the counters; `prep`, ONE kernel launched as its programmatic
+// dependent, builds the per-RoI axis tables (all IEEE divisions; ring-slot byte offsets precomputed), lists the
+// fragments and takes each one's rank within its (image, strip, row) key with a returning atomic, passes a grid
+// barrier, scans the histogram in every CTA's shared memory (CSR row pointers), writes the 8-byte fragment records
+// at row pointer + rank and cuts the linear space into one piece per SM of equal estimated cost.  The main kernel
+// is launched as the prepass's programmatic dependent: its ring and barrier set-up overlaps the prepass.
 //
 // Semantics: lib/modeling/roi_xfrom/roi_align/src/roi_align_kernel.cu (reference) :16-63, :65-121.
 #include "common.cuh"
+#include "strip_prep.cuh"
 #include <mutex>
+#include <string.h>
 #include <stdlib.h>
 
 namespace b200 {
@@ -47,8 +51,8 @@ constexpr int kMaxSlots = 32;                                 // ring depth K <=
 constexpr int kAxisMaxS = 32;                                 // P * sampling_ratio per axis
 constexpr int kPrepThreads = 128;
 constexpr unsigned kRowCost = 8u;                             // cost of streaming one row (16 acquires + staging), in bins
-constexpr int kScanCap = 6144;                                // keys whose cost prefix is kept in shared memory by the scan
 constexpr unsigned kSmemBudget = 227u * 1024u;
+constexpr unsigned kPrepSmemMax = 200u * 1024u;               // dynamic shared memory of the prepass: scan of the keys + one RoI's fragment list
 
 typedef unsigned long long u64;
 
@@ -73,7 +77,7 @@ struct StreamGeom {
     int Q, keys;                // strip columns, keys = sum over columns of their rows
     int G;                      // 32-channel groups
     int pieces;                 // persistent CTAs
-    int max_entries;
+    int max_entries, cap_r;     // cap_r: fragments one RoI can have at most
     StreamLevel lv[kMaxLevels];
     int colstart[kMaxCols + 1]; // first key of every column (its rows are consecutive keys); colstart[Q] = keys
 };
@@ -90,13 +94,13 @@ struct StreamWs {
     uint4* xtab;                // [R][nx] {hx, lx, x_low * 4, 0}
     int* hist;                  // [keys] fragments per key                           (zero block)
     int* cost;                  // [keys] estimated cost per key                      (zero block)
-    int* cursor;                // [keys] fill cursors                                (zero block)
     int* maxend;                // [keys] max over the key's fragments of `end`       (zero block)
-    int* ticket;                // [4]                                                (zero block)
+    int* ticket;                // [4] grid barrier of the prepass                    (zero block)
     int* rowptr;                // [keys + 1] CSR offsets into entries
-    unsigned* cpre;             // [keys + 1] exclusive prefix of the cost
     int* piece_start;           // [pieces + 1] linear start index of every piece
     uint2* entries;             // fragment records
+    uint4* tmp;                 // [R][cap_r] {key index, rank within the key, record}: phase 1 -> phase 3 of the prepass
+    int* tmpcnt;                // [R] fragments of the RoI (-1: batch index out of range)
 };
 
 // fragment record: x = r | ph << 16 | pw0 << 21 | (npw - 1) << 26 | red << 29 ; y = key | (end - key) << 16 | smask << 24
@@ -177,199 +181,136 @@ __device__ __forceinline__ void enum_row(const int* yl, const int* yh, const int
 }
 
 // ------------------------------------------------------------------------------------------------
-// prepass 1: tables + histogram; last CTA: scan + partition
+// prepass: clear of the counters, then ONE kernel: tables + fragment list | grid barrier | CSR scan (every CTA) | records,
+// zero-fill, pieces
 // ------------------------------------------------------------------------------------------------
-template <int SR>
+// The counters the prepass accumulates into must start at zero.  A kernel instead of a memset: the prepass is launched as
+// its programmatic dependent, so that its tables and fragment lists are computed while this runs.
 __global__ void __launch_bounds__(kPrepThreads)
-stream_count(const float* __restrict__ rois, StreamGeom g, StreamWs ws) {
-    __shared__ int s_yl[kAxisMaxS], s_yh[kAxisMaxS], s_xl[kAxisMaxS];
-    __shared__ int s_last;
-    __shared__ unsigned s_h[kPrepThreads], s_c[kPrepThreads];
-    const int r = blockIdx.x, t = threadIdx.x;
-    const StreamLevel& lv = g.lv[level_of_roi(g, r)];
-    const XfromRoi geo = xfrom_roi(rois + 5 * (size_t)r, lv.scale, g.PH, g.PW, g.sr);
-    if (t < g.ny + g.nx) {
-        const bool isy = t < g.ny;
-        const int s = isy ? t : t - g.ny;
-        if (isy) {
-            // rows exactly as the reference takes them (low == high == H - 1 on the clamped last row, weights (1, 0)): the
-            // lower tap then reads whatever the next ring slot holds with weight 0 -- always finite, the ring starts zeroed
-            const AxisTap a = xfrom_axis(xfrom_coord(geo.start_h, geo.bin_h, s / SR, s % SR, SR), lv.H);
-            s_yl[s] = a.low; s_yh[s] = a.high;
-            uint4 e;
-            e.x = __float_as_uint(a.valid ? a.h : 0.f); e.y = __float_as_uint(a.valid ? a.l : 0.f);
-            e.z = (unsigned)((a.low % g.K) * g.row_bytes);
-            e.w = 0u;
-            ws.ytab[(size_t)r * g.ny + s] = e;
-        } else {
-            const AdjTap a = adj_axis(xfrom_coord(geo.start_w, geo.bin_w, s / SR, s % SR, SR), lv.W);
-            s_xl[s] = a.low;
-            uint4 e;
-            e.x = __float_as_uint(a.h); e.y = __float_as_uint(a.l);
-            e.z = (unsigned)(a.low * 4); e.w = 0u;
-            ws.xtab[(size_t)r * g.nx + s] = e;
-        }
-    }
-    __syncthreads();
-    const bool batch_ok = geo.batch >= 0 && geo.batch < g.N;
-    if (batch_ok && t < g.PH) {
-        const int cbase = lv.q_base + geo.batch * lv.S;
-        enum_row<SR>(s_yl, s_yh, s_xl, t, g, lv.S, [&](int s, int key, int end, int pw0, int npw, unsigned smask, int red, bool owner) {
-            const int k = g.colstart[cbase + s] + key;
-            atomicAdd(&ws.hist[k], 1);
-            atomicAdd(&ws.cost[k], 2 + npw);
-            (void)end; (void)pw0; (void)smask; (void)red; (void)owner;
-        });
-    }
-    // ---- last CTA: CSR row pointers, cost prefix, piece boundaries
-    __threadfence();
-    __syncthreads();
-    if (t == 0) s_last = (atomicAdd(&ws.ticket[0], 1) == (int)gridDim.x - 1) ? 1 : 0;
-    __syncthreads();
-    if (!s_last) return;
-    __threadfence();
-    // Everything below is latency bound (one CTA): the histogram is pulled into shared memory with all loads of a
-    // chunk in flight, scanned there, and the piece boundaries are binary-searched in the shared copy of the prefix.
-    __shared__ unsigned s_pre[kScanCap + 1];                  // exclusive cost prefix (keys <= kScanCap)
-    __shared__ unsigned s_carry[2];
-    const int keys = g.keys;
-    const bool in_smem = keys <= kScanCap;
-    if (t == 0) { s_carry[0] = 0u; s_carry[1] = 0u; }
-    __syncthreads();
-    constexpr int kPer = 8, kChunk = kPrepThreads * kPer;
-    for (int base = 0; base < keys; base += kChunk) {
-        unsigned h[kPer], c[kPer];
-#pragma unroll
-        for (int j = 0; j < kPer; ++j) {                      // thread t owns keys base + t * kPer + j; loads are independent
-            const int k = base + t * kPer + j;
-            h[j] = k < keys ? (unsigned)__ldcg(&ws.hist[k]) : 0u;
-            c[j] = k < keys ? (unsigned)__ldcg(&ws.cost[k]) + kRowCost : 0u;
-        }
-        unsigned sh = 0, sc = 0;
-#pragma unroll
-        for (int j = 0; j < kPer; ++j) { sh += h[j]; sc += c[j]; }
-        s_h[t] = sh; s_c[t] = sc;
-        __syncthreads();
-        if (t < 32) {                                         // exclusive scan of the 128 thread sums by one warp (4 per lane)
-            unsigned vh[4], vc[4], th = 0, tc = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { vh[j] = s_h[t * 4 + j]; vc[j] = s_c[t * 4 + j]; th += vh[j]; tc += vc[j]; }
-            unsigned ih = th, ic = tc;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const unsigned uh = __shfl_up_sync(0xffffffffu, ih, d), uc = __shfl_up_sync(0xffffffffu, ic, d);
-                if (t >= d) { ih += uh; ic += uc; }
-            }
-            unsigned rh = ih - th + s_carry[0], rc = ic - tc + s_carry[1];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { s_h[t * 4 + j] = rh; s_c[t * 4 + j] = rc; rh += vh[j]; rc += vc[j]; }
-            __syncwarp();
-            if (t == 31) { s_carry[0] = rh; s_carry[1] = rc; }
-        }
-        __syncthreads();
-        unsigned rh = s_h[t], rc = s_c[t];
-#pragma unroll
-        for (int j = 0; j < kPer; ++j) {
-            const int k = base + t * kPer + j;
-            if (k < keys) {
-                ws.rowptr[k] = (int)rh; ws.cpre[k] = rc;
-                if (in_smem) s_pre[k] = rc;
-            }
-            rh += h[j]; rc += c[j];
-        }
-        __syncthreads();
-    }
-    if (t == 0) {
-        ws.rowptr[keys] = (int)s_carry[0]; ws.cpre[keys] = s_carry[1];
-        if (in_smem) s_pre[keys] = s_carry[1];
-    }
-    __threadfence();
-    __syncthreads();
-    // piece p starts where the cumulative cost over the linear order (column q, channel group, row) reaches p/pieces
-    auto pre = [&](size_t k) -> unsigned { return in_smem ? s_pre[k] : __ldcg(&ws.cpre[k]); };
-    const unsigned total = s_carry[1];
-    const u64 grand = (u64)total * (u64)g.G;
-    for (int p = t; p <= g.pieces; p += kPrepThreads) {
-        int L;
-        if (p == 0) L = 0;
-        else if (p == g.pieces) L = g.G * g.keys;
-        else {
-            const u64 target = grand / (u64)g.pieces * (u64)p + (grand % (u64)g.pieces) * (u64)p / (u64)g.pieces;
-            int lo = 0, hi = g.Q - 1;
-            while (lo < hi) {
-                const int mid = (lo + hi + 1) >> 1;
-                if ((u64)g.G * (u64)pre((size_t)g.colstart[mid]) <= target) lo = mid; else hi = mid - 1;
-            }
-            const int q = lo;
-            const int k0 = g.colstart[q], Hq = g.colstart[q + 1] - k0;
-            const unsigned c0 = pre((size_t)k0);
-            const unsigned colsum = pre((size_t)k0 + Hq) - c0;              // >= kRowCost * Hq > 0
-            u64 rem = target - (u64)g.G * (u64)c0;
-            int gg = (int)(rem / colsum);
-            if (gg > g.G - 1) gg = g.G - 1;
-            rem -= (u64)gg * colsum;
-            int ylo = 0, yhi = Hq - 1;
-            while (ylo < yhi) {
-                const int mid = (ylo + yhi + 1) >> 1;
-                if ((u64)(pre((size_t)k0 + mid) - c0) <= rem) ylo = mid; else yhi = mid - 1;
-            }
-            L = g.G * k0 + gg * Hq + ylo;                                   // linear order: (column, channel group, row)
-        }
-        ws.piece_start[p] = L;
-    }
+stream_clear(int4* __restrict__ zero, int n16) {
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    for (int i = blockIdx.x * kPrepThreads + threadIdx.x; i < n16; i += gridDim.x * kPrepThreads) zero[i] = make_int4(0, 0, 0, 0);
 }
 
-// ------------------------------------------------------------------------------------------------
-// prepass 2: fragment records into the CSR; zero-fill of the elements that are accumulated with red.add
-// ------------------------------------------------------------------------------------------------
 template <int SR>
 __global__ void __launch_bounds__(kPrepThreads)
-stream_fill(const float* __restrict__ rois, StreamGeom g, StreamWs ws, float* __restrict__ out, const int* __restrict__ row_map) {
+stream_prep(const float* __restrict__ rois, StreamGeom g, StreamWs ws, float* __restrict__ out, const int* __restrict__ row_map) {
+    extern __shared__ unsigned s_dyn[];                       // [keys + 1] fragment prefix, [keys + 1] cost prefix, [cap_r][3] fragment list
+    __shared__ int s_nlist;
     __shared__ int s_yl[kAxisMaxS], s_yh[kAxisMaxS], s_xl[kAxisMaxS];
     __shared__ unsigned short s_zero[kAxisMaxS * kAxisMaxS];
     __shared__ int s_nzero;
-    const int r = blockIdx.x, t = threadIdx.x;
-    const StreamLevel& lv = g.lv[level_of_roi(g, r)];
-    const XfromRoi geo = xfrom_roi(rois + 5 * (size_t)r, lv.scale, g.PH, g.PW, g.sr);
-    if (t == 0) s_nzero = 0;
-    if (t < g.ny + g.nx) {
-        const bool isy = t < g.ny;
-        const int s = isy ? t : t - g.ny;
-        if (isy) {
-            const AxisTap a = xfrom_axis(xfrom_coord(geo.start_h, geo.bin_h, s / SR, s % SR, SR), lv.H);
-            s_yl[s] = a.low; s_yh[s] = a.high;
-        } else {
-            s_xl[s] = adj_axis(xfrom_coord(geo.start_w, geo.bin_w, s / SR, s % SR, SR), lv.W).low;
+    __shared__ unsigned s_ph[kPrepThreads], s_pc[kPrepThreads];
+    const int t = threadIdx.x;
+    const int keys = g.keys;
+    unsigned* s_pre = s_dyn;
+    unsigned* s_cpre = s_dyn + (keys + 1);
+    unsigned* s_list = s_dyn + 2 * (keys + 1);               // {key index, record.x, record.y} per fragment of the current RoI
+    // the main kernel may start its prologue (ring, barriers) on every SM this grid leaves room on; it waits for all of
+    // this grid's results before it reads any of them
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+
+    // ---- phase 1: per RoI (the grid loops over them when R exceeds the resident grid): axis tables (all IEEE divisions live
+    // here), the fragments listed in shared memory by the bin-row threads; then ALL threads take one fragment each: rank
+    // within its key (one returning atomic, its latency hides behind the grid barrier), cost / extent atomics, and a
+    // temporary record that phase 3 only has to drop into the CSR
+    for (int r = blockIdx.x; r < g.R; r += gridDim.x) {
+        __syncthreads();                                      // s_yl / s_yh / s_xl / s_list of the previous RoI are no longer read
+        const StreamLevel& lv = g.lv[level_of_roi(g, r)];
+        const XfromRoi geo = xfrom_roi(rois + 5 * (size_t)r, lv.scale, g.PH, g.PW, g.sr);
+        if (t == 0) s_nlist = 0;
+        if (t < g.ny + g.nx) {
+            const bool isy = t < g.ny;
+            const int s = isy ? t : t - g.ny;
+            if (isy) {
+                // rows exactly as the reference takes them (low == high == H - 1 on the clamped last row, weights (1, 0)): the
+                // lower tap then reads whatever the next ring slot holds with weight 0 -- always finite, the ring starts zeroed
+                const AxisTap a = xfrom_axis(xfrom_coord(geo.start_h, geo.bin_h, s / SR, s % SR, SR), lv.H);
+                s_yl[s] = a.low; s_yh[s] = a.high;
+                uint4 e;
+                e.x = __float_as_uint(a.valid ? a.h : 0.f); e.y = __float_as_uint(a.valid ? a.l : 0.f);
+                e.z = (unsigned)((a.low % g.K) * g.row_bytes);
+                e.w = 0u;
+                ws.ytab[(size_t)r * g.ny + s] = e;
+            } else {
+                const AdjTap a = adj_axis(xfrom_coord(geo.start_w, geo.bin_w, s / SR, s % SR, SR), lv.W);
+                s_xl[s] = a.low;
+                uint4 e;
+                e.x = __float_as_uint(a.h); e.y = __float_as_uint(a.l);
+                e.z = (unsigned)(a.low * 4); e.w = 0u;
+                ws.xtab[(size_t)r * g.nx + s] = e;
+            }
         }
-    }
-    __syncthreads();
-    const bool batch_ok = geo.batch >= 0 && geo.batch < g.N;
-    const int bins = g.PH * g.PW;
-    if (batch_ok) {
-        if (t < g.PH) {
+        __syncthreads();
+        const bool batch_ok = geo.batch >= 0 && geo.batch < g.N;
+        if (batch_ok && t < g.PH) {
             const int cbase = lv.q_base + geo.batch * lv.S;
             enum_row<SR>(s_yl, s_yh, s_xl, t, g, lv.S, [&](int s, int key, int end, int pw0, int npw, unsigned smask, int red, bool owner) {
-                const int k = g.colstart[cbase + s] + key;
-                const int pos = ws.rowptr[k] + atomicAdd(&ws.cursor[k], 1);
-                if (pos < g.max_entries) ws.entries[pos] = pack_entry(r, t, pw0, npw, red, key, end, smask);
-                atomicMax(&ws.maxend[k], end);
-                if (owner) {
-                    const int z = atomicAdd(&s_nzero, npw);
-                    for (int i = 0; i < npw; ++i) s_zero[z + i] = (unsigned short)(t * g.PW + pw0 + i);
-                }
+                const int idx = atomicAdd(&s_nlist, 1);
+                const uint2 e = pack_entry(r, t, pw0, npw, red, key, end, smask);
+                s_list[3 * idx] = (unsigned)(g.colstart[cbase + s] + key); s_list[3 * idx + 1] = e.x; s_list[3 * idx + 2] = e.y;
+                (void)owner;
             });
         }
-    } else {
-        for (int i = t; i < bins; i += kPrepThreads) s_zero[i] = (unsigned short)i;       // the reference would read out of bounds
-        if (t == 0) s_nzero = bins;
+        __syncthreads();
+        // the counters are cleared by the kernel this one depends on: wait for it before the first atomic (returns at once
+        // from the second RoI on)
+        asm volatile("griddepcontrol.wait;" ::: "memory");
+        const int n = s_nlist;
+        for (int idx = t; idx < n; idx += kPrepThreads) {
+            const unsigned k = s_list[3 * idx], ex = s_list[3 * idx + 1], ey = s_list[3 * idx + 2];
+            const int npw = (int)((ex >> 26) & 7u) + 1, end = (int)(ey & 0xffffu) + (int)((ey >> 16) & 0xffu);
+            const int rank = atomicAdd(&ws.hist[k], 1);
+            atomicAdd(&ws.cost[k], 2 + npw);
+            atomicMax(&ws.maxend[k], end);
+            ws.tmp[(size_t)r * g.cap_r + idx] = make_uint4(k, (unsigned)rank, ex, ey);
+        }
+        if (t == 0) ws.tmpcnt[r] = batch_ok ? n : -1;
     }
-    __syncthreads();
-    const int nz = s_nzero;
-    if (nz == 0) return;
-    float* out_r = out + (size_t)(row_map ? row_map[r] : r) * g.C * bins;
-    for (int idx = t; idx < g.C * nz; idx += kPrepThreads) {
-        const int c = idx / nz, k = idx - c * nz;
-        out_r[(size_t)c * bins + s_zero[k]] = 0.f;
+    asm volatile("griddepcontrol.wait;" ::: "memory");      // a CTA without a RoI still arrives on a cleared ticket
+    // ---- grid barrier (the grid is sized to be resident: see the launcher)
+    prepass::grid_barrier(ws.ticket);
+    // ---- phase 2: exclusive prefix of the fragment histogram and of the cost, in every CTA's shared memory
+    prepass::scan_keys<kPrepThreads>(ws.hist, ws.cost, kRowCost, keys, s_pre, s_cpre, s_ph, s_pc);
+    // row pointers for the main kernel: every CTA writes a slice
+    for (int k = blockIdx.x * kPrepThreads + t; k <= keys; k += gridDim.x * kPrepThreads) ws.rowptr[k] = (int)s_pre[k];
+    // piece boundaries: every CTA holds the whole prefix, so they are spread over the grid (one per CTA, thread 0)
+    if (t == 0)
+        for (int p = blockIdx.x; p <= g.pieces; p += gridDim.x)
+            ws.piece_start[p] = prepass::piece_start(p, g.pieces, g.G, keys, g.Q, g.colstart, s_cpre);
+    // ---- phase 3: fragment records into the CSR (position = row pointer + rank); zero-fill of the elements that are
+    // accumulated with red.add (the bins of the fragments that hold a split bin's first sample)
+    const int bins = g.PH * g.PW;
+    for (int r = blockIdx.x; r < g.R; r += gridDim.x) {
+        __syncthreads();
+        if (t == 0) s_nzero = 0;
+        __syncthreads();
+        const int n = __ldcg(&ws.tmpcnt[r]);
+        if (n >= 0) {
+            for (int idx = t; idx < n; idx += kPrepThreads) {
+                const uint4 rec = __ldcg(&ws.tmp[(size_t)r * g.cap_r + idx]);
+                const int pos = (int)s_pre[rec.x] + (int)rec.y;
+                if (pos < g.max_entries) ws.entries[pos] = make_uint2(rec.z, rec.w);
+                const bool owner = ((rec.z >> 29) & 1u) && ((rec.w >> 24) & 1u);
+                if (owner) {
+                    const int ph = (rec.z >> 16) & 31u, pw0 = (rec.z >> 21) & 31u, npw = (int)((rec.z >> 26) & 7u) + 1;
+                    const int z = atomicAdd(&s_nzero, npw);
+                    for (int i = 0; i < npw; ++i) s_zero[z + i] = (unsigned short)(ph * g.PW + pw0 + i);
+                }
+            }
+        } else {
+            for (int i = t; i < bins; i += kPrepThreads) s_zero[i] = (unsigned short)i;       // the reference would read out of bounds
+            if (t == 0) s_nzero = bins;
+        }
+        __syncthreads();
+        const int nz = s_nzero;
+        if (nz > 0) {
+            float* out_r = out + (size_t)(row_map ? row_map[r] : r) * g.C * bins;
+            for (int idx = t; idx < g.C * nz; idx += kPrepThreads) {
+                const int c = idx / nz, k = idx - c * nz;
+                out_r[(size_t)c * bins + s_zero[k]] = 0.f;
+            }
+        }
     }
 }
 
@@ -470,11 +411,11 @@ __device__ __forceinline__ Item decode_item(int L, int L1, const StreamArgs& a, 
     const int qq = q - a.lv[l].q_base;
     it.n = qq / a.lv[l].S;
     it.s = qq - it.n * a.lv[l].S;
-    it.e0 = __ldg(&a.rowptr[it.kbase + it.ya]);
-    it.e1 = __ldg(&a.rowptr[it.kbase + it.yb]);
+    it.e0 = __ldcg(&a.rowptr[it.kbase + it.ya]);
+    it.e1 = __ldcg(&a.rowptr[it.kbase + it.yb]);
     int m = 0;
     if (it.e1 > it.e0) {
-        for (int y = it.ya + lane; y < it.yb; y += 32) m = max(m, __ldg(&a.maxend[it.kbase + y]));
+        for (int y = it.ya + lane; y < it.yb; y += 32) m = max(m, __ldcg(&a.maxend[it.kbase + y]));
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
     }
@@ -574,7 +515,12 @@ roi_align_stream_fwd(const StreamArgs a) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    const int L0 = __ldg(&a.piece_start[blockIdx.x]), L1 = __ldg(&a.piece_start[blockIdx.x + 1]);
+    asm volatile("griddepcontrol.wait;" ::: "memory");             // the prepass's results are visible from here on
+    // Everything the prepass wrote is read with ld.volatile / ld.cg from here on, never __ldg: a read-only (.nc) load carries
+    // no dependence on the wait above and may be hoisted above it (DESIGN.md 4.1)
+    int L0, L1;
+    asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L0) : "l"(a.piece_start + blockIdx.x) : "memory");
+    asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L1) : "l"(a.piece_start + blockIdx.x + 1) : "memory");
 
     if (warp >= kConsumerWarps) {
         // =============================== producers ===============================
@@ -668,14 +614,14 @@ roi_align_stream_fwd(const StreamArgs a) {
             const bool isx = lane < nn * SR;                   // one predicated load: the two tables differ in base and index only
             const uint4* base = isx ? a.xtab : a.ytab;
             const int idx = isx ? rn * a.nx + pwn * SR + lane : rn * a.ny + phn * SR + (lane - 16);
-            if (isx || (lane >= 16 && lane < 16 + SR)) v = __ldg(base + idx);
+            if (isx || (lane >= 16 && lane < 16 + SR)) v = __ldcg(base + idx);
             return v;
         };
         int e = it.e0 + warp;
         uint2 ent0 = make_uint2(0u, 0u), ent1 = make_uint2(0u, 0u);
         uint4 tab = make_uint4(0u, 0u, 0u, 0u);
-        if (e < it.e1) { ent0 = __ldg(&a.entries[e]); tab = load_tab(ent0); }
-        if (e + kConsumerWarps < it.e1) ent1 = __ldg(&a.entries[e + kConsumerWarps]);
+        if (e < it.e1) { ent0 = __ldcg(&a.entries[e]); tab = load_tab(ent0); }
+        if (e + kConsumerWarps < it.e1) ent1 = __ldcg(&a.entries[e + kConsumerWarps]);
         while (e < it.e1) {
             const uint2 cur = ent0;
             const int e_next = e + kConsumerWarps;
@@ -684,7 +630,7 @@ roi_align_stream_fwd(const StreamArgs a) {
             __syncwarp();
             ent0 = ent1;
             if (e_next < it.e1) tab = load_tab(ent0);                               // in flight while this fragment computes
-            if (e_next + kConsumerWarps < it.e1) ent1 = __ldg(&a.entries[e_next + kConsumerWarps]);
+            if (e_next + kConsumerWarps < it.e1) ent1 = __ldcg(&a.entries[e_next + kConsumerWarps]);
             const int r = cur.x & 0xffffu, ph = (cur.x >> 16) & 31u, pw0 = (cur.x >> 21) & 31u;
             const int npw = (int)((cur.x >> 26) & 7u) + 1;
             const bool red = (cur.x >> 29) & 1u;
@@ -788,7 +734,8 @@ roi_align_stream_fwd(const StreamArgs a) {
 size_t align_up_sz(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 struct StreamLayout {
-    size_t ytab_off, xtab_off, zero_off, zero_bytes, rowptr_off, cpre_off, piece_off, entries_off, ws_bytes;
+    size_t ytab_off, xtab_off, zero_off, zero_bytes, rowptr_off, piece_off, entries_off, tmp_off, tmpcnt_off, ws_bytes;
+    size_t prep_smem;           // dynamic shared memory of stream_prep
 };
 
 // One launch serves `levels` feature maps (FPN: the pyramid levels of one head; a plain call: one map).  All levels share the
@@ -854,15 +801,20 @@ bool stream_geometry(int levels, const float* const* bottoms, const int* heights
     if (g->G < 1) g->G = 1;
     if (keys * g->G >= (1LL << 30)) return false;
     g->pieces = sm_count > 0 ? sm_count : kNumSMs;
-    g->max_entries = R * PH * PW * sr * sr;                    // worst case: every sample its own fragment
+    g->cap_r = PH * PW * sr * sr;                              // worst case: every sample its own fragment
+    g->max_entries = R * g->cap_r;
+    // the prepass scans the keys in shared memory
+    lay->prep_smem = (size_t)2 * (g->keys + 1) * 4 + (size_t)g->cap_r * 12;
+    if (lay->prep_smem > kPrepSmemMax) return false;
     size_t off = 0;
     lay->ytab_off = off; off = align_up_sz(off + (size_t)R * g->ny * 16, 256);
     lay->xtab_off = off; off = align_up_sz(off + (size_t)R * g->nx * 16, 256);
-    lay->zero_off = off; lay->zero_bytes = align_up_sz(((size_t)4 * g->keys + 4) * 4, 256); off += lay->zero_bytes;
+    lay->zero_off = off; lay->zero_bytes = align_up_sz(((size_t)3 * g->keys + 4) * 4, 256); off += lay->zero_bytes;
     lay->rowptr_off = off; off = align_up_sz(off + ((size_t)g->keys + 1) * 4, 256);
-    lay->cpre_off = off; off = align_up_sz(off + ((size_t)g->keys + 1) * 4, 256);
     lay->piece_off = off; off = align_up_sz(off + ((size_t)g->pieces + 1) * 4, 256);
     lay->entries_off = off; off = align_up_sz(off + (size_t)g->max_entries * 8, 256);
+    lay->tmp_off = off; off = align_up_sz(off + (size_t)g->max_entries * 16, 256);
+    lay->tmpcnt_off = off; off = align_up_sz(off + (size_t)R * 4, 256);
     lay->ws_bytes = off;
     *smem_bytes = (unsigned)(g->K + 1) * (unsigned)g->row_bytes + fixed;
     return true;
@@ -888,6 +840,8 @@ bool stream_device_info(int* sm_count) {
         B200_STREAM_ATTR(1, 1); B200_STREAM_ATTR(1, 2); B200_STREAM_ATTR(1, 3);
         B200_STREAM_ATTR(2, 1); B200_STREAM_ATTR(2, 2); B200_STREAM_ATTR(2, 3);
 #undef B200_STREAM_ATTR
+        ok = ok && cudaFuncSetAttribute(stream_prep<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmemMax) == cudaSuccess;
+        ok = ok && cudaFuncSetAttribute(stream_prep<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmemMax) == cudaSuccess;
         if (!ok) {
             (void)cudaGetLastError();
             return false;
@@ -925,35 +879,58 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
     ws.ytab = (uint4*)(wsb + lay.ytab_off);
     ws.xtab = (uint4*)(wsb + lay.xtab_off);
     int* zero = (int*)(wsb + lay.zero_off);
-    ws.hist = zero; ws.cost = zero + g.keys; ws.cursor = zero + 2 * (size_t)g.keys; ws.maxend = zero + 3 * (size_t)g.keys;
-    ws.ticket = zero + 4 * (size_t)g.keys;
+    ws.hist = zero; ws.cost = zero + g.keys; ws.maxend = zero + 2 * (size_t)g.keys;
+    ws.ticket = zero + 3 * (size_t)g.keys;
     ws.rowptr = (int*)(wsb + lay.rowptr_off);
-    ws.cpre = (unsigned*)(wsb + lay.cpre_off);
     ws.piece_start = (int*)(wsb + lay.piece_off);
     ws.entries = (uint2*)(wsb + lay.entries_off);
+    ws.tmp = (uint4*)(wsb + lay.tmp_off);
+    ws.tmpcnt = (int*)(wsb + lay.tmpcnt_off);
 
-    cudaError_t err = cudaMemsetAsync(zero, 0, lay.zero_bytes, stream);
-    if (err != cudaSuccess) return (int)err;
+    // prepass grid: one CTA per RoI when they are all resident at once (the kernel has a grid barrier), else a resident grid
+    int per_sm = 0;
+    cudaError_t err = sr == 1 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, stream_prep<1>, kPrepThreads, lay.prep_smem)
+                              : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, stream_prep<2>, kPrepThreads, lay.prep_smem);
+    if (err != cudaSuccess || per_sm < 1) { (void)cudaGetLastError(); return kPathDeclined; }
+    const long long cap = (long long)per_sm * sm_count;
+    const int prep_grid = (int)(R < cap ? R : cap);
+    const int n16 = (int)(lay.zero_bytes / 16);
+
     StreamArgs a;
     a.ytab = ws.ytab; a.xtab = ws.xtab; a.entries = ws.entries; a.rowptr = ws.rowptr; a.maxend = ws.maxend;
     a.piece_start = ws.piece_start; a.out = top; a.row_map = row_map;
     a.C = C; a.G = g.G; a.K = g.K; a.WX = g.WX; a.PH = PH; a.PW = PW; a.ny = g.ny; a.nx = g.nx; a.L = g.L; a.Q = g.Q;
     for (int l = 0; l < kMaxLevels; ++l) a.lv[l] = g.lv[l];
     for (int c = 0; c <= kMaxCols; ++c) a.colstart[c] = g.colstart[c];
+
+    // clear -> prep -> main, each launched as the programmatic dependent of the one before (it starts once every CTA of the
+    // previous kernel has signalled launch_dependents, and waits for that kernel's results with griddepcontrol.wait)
+    stream_clear<<<(n16 + kPrepThreads - 1) / kPrepThreads, kPrepThreads, 0, stream>>>((int4*)zero, n16);
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg;
+    memset(&cfg, 0, sizeof(cfg));
+    cfg.gridDim = dim3((unsigned)prep_grid);
+    cfg.blockDim = dim3(kPrepThreads);
+    cfg.dynamicSmemBytes = lay.prep_smem;
+    cfg.stream = stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    err = sr == 1 ? cudaLaunchKernelEx(&cfg, stream_prep<1>, rois, g, ws, top, row_map)
+                  : cudaLaunchKernelEx(&cfg, stream_prep<2>, rois, g, ws, top, row_map);
+    if (err != cudaSuccess) return (int)err;
+    cfg.gridDim = dim3((unsigned)g.pieces);
+    cfg.blockDim = dim3(kStreamThreads);
+    cfg.dynamicSmemBytes = smem;
     const int m = (g.SX - 1) / 32;
-    if (sr == 1) {
-        stream_count<1><<<R, kPrepThreads, 0, stream>>>(rois, g, ws);
-        stream_fill<1><<<R, kPrepThreads, 0, stream>>>(rois, g, ws, top, row_map);
-    } else {
-        stream_count<2><<<R, kPrepThreads, 0, stream>>>(rois, g, ws);
-        stream_fill<2><<<R, kPrepThreads, 0, stream>>>(rois, g, ws, top, row_map);
-    }
-#define B200_STREAM_LAUNCH(SRV, MV) roi_align_stream_fwd<SRV, MV><<<g.pieces, kStreamThreads, smem, stream>>>(a)
-#define B200_STREAM_LAUNCH_M(SRV) (m == 1 ? B200_STREAM_LAUNCH(SRV, 1) : m == 2 ? B200_STREAM_LAUNCH(SRV, 2) : B200_STREAM_LAUNCH(SRV, 3))
-    if (sr == 1) B200_STREAM_LAUNCH_M(1);
-    else         B200_STREAM_LAUNCH_M(2);
+#define B200_STREAM_LAUNCH(SRV, MV) err = cudaLaunchKernelEx(&cfg, roi_align_stream_fwd<SRV, MV>, a)
+#define B200_STREAM_LAUNCH_M(SRV) if (m == 1) B200_STREAM_LAUNCH(SRV, 1); else if (m == 2) B200_STREAM_LAUNCH(SRV, 2); else B200_STREAM_LAUNCH(SRV, 3)
+    if (sr == 1) { B200_STREAM_LAUNCH_M(1); }
+    else         { B200_STREAM_LAUNCH_M(2); }
 #undef B200_STREAM_LAUNCH_M
 #undef B200_STREAM_LAUNCH
+    if (err != cudaSuccess) return (int)err;
     return finish_launch(3);
 }
 

@@ -42,6 +42,7 @@
 //
 // Semantics: lib/modeling/roi_xfrom/roi_align/src/roi_align_kernel.cu (reference) :16-63, :65-121.
 #include "common.cuh"
+#include "strip_prep.cuh"
 #include <cuda.h>                                              // CUtensorMap types only: the encoder is fetched with cudaGetDriverEntryPoint
 #include <mutex>
 #include <string.h>
@@ -183,12 +184,6 @@ __device__ __forceinline__ void enum_row(const int* yl, const int* xl, int ph, c
     }
 }
 
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-
 // ------------------------------------------------------------------------------------------------
 // prepass (one launch): tables + histogram | grid barrier | CSR scan (every CTA) | records, zero-fill, pieces
 // ------------------------------------------------------------------------------------------------
@@ -268,93 +263,16 @@ strip_prep(const float* __restrict__ rois, StripGeom g, StripWs ws, float* __res
         if (t == 0) ws.tmpcnt[r] = batch_ok ? n : -1;
     }
     // ---- grid barrier (the grid is sized to be resident: see the launcher)
-    __syncthreads();
-    if (t == 0) {
-        __threadfence();
-        atomicAdd(&ws.ticket[0], 1);
-        unsigned spins = 0;
-        while (ld_acquire_gpu(&ws.ticket[0]) < (int)gridDim.x) {
-            __nanosleep(64);
-            if (++spins > (1u << 24)) __trap();               // seconds: a non-resident grid, not a slow one
-        }
-    }
-    __syncthreads();
+    prepass::grid_barrier(ws.ticket);
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");      // the main kernel may start its prologue
     // ---- phase 2: exclusive prefix of the fragment histogram and of the cost, in every CTA's shared memory
-    for (int k = t; k < keys; k += kPrepThreads) {
-        s_pre[k] = (unsigned)__ldcg(&ws.hist[k]);
-        s_cpre[k] = (unsigned)__ldcg(&ws.cost[k]) + kRowCost;
-    }
-    __syncthreads();
-    const int chunk = ((keys + kPrepThreads - 1) / kPrepThreads) | 1;     // odd: thread-strided chunks do not collide on banks
-    const int k0 = min(keys, t * chunk), k1 = min(keys, k0 + chunk);
-    {
-        unsigned sh = 0, sc = 0;
-        for (int k = k0; k < k1; ++k) { sh += s_pre[k]; sc += s_cpre[k]; }
-        s_ph[t] = sh; s_pc[t] = sc;
-    }
-    __syncthreads();
-    if (t < 32) {                                             // exclusive scan of the 128 chunk sums by one warp (4 per lane)
-        unsigned vh[4], vc[4], th = 0, tc = 0;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { vh[j] = s_ph[t * 4 + j]; vc[j] = s_pc[t * 4 + j]; th += vh[j]; tc += vc[j]; }
-        unsigned ih = th, ic = tc;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const unsigned uh = __shfl_up_sync(0xffffffffu, ih, d), uc = __shfl_up_sync(0xffffffffu, ic, d);
-            if (t >= d) { ih += uh; ic += uc; }
-        }
-        unsigned rh = ih - th, rc = ic - tc;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { s_ph[t * 4 + j] = rh; s_pc[t * 4 + j] = rc; rh += vh[j]; rc += vc[j]; }
-        if (t == 31) { s_pre[keys] = rh; s_cpre[keys] = rc; }
-    }
-    __syncthreads();
-    {
-        unsigned rh = s_ph[t], rc = s_pc[t];
-        for (int k = k0; k < k1; ++k) {
-            const unsigned h = s_pre[k], c = s_cpre[k];
-            s_pre[k] = rh; s_cpre[k] = rc;
-            rh += h; rc += c;
-        }
-    }
-    __syncthreads();
+    prepass::scan_keys<kPrepThreads>(ws.hist, ws.cost, kRowCost, keys, s_pre, s_cpre, s_ph, s_pc);
     // row pointers for the main kernel: every CTA writes a slice
     for (int k = blockIdx.x * kPrepThreads + t; k <= keys; k += gridDim.x * kPrepThreads) ws.rowptr[k] = (int)s_pre[k];
-    // piece boundaries: piece p starts where the cumulative cost over the linear order (column, group, row) reaches p / pieces.
-    // Every CTA holds the whole prefix, so the boundaries are spread over the grid (one per CTA, thread 0) instead of queueing in one
-    if (t == 0) {
-        const unsigned total = s_cpre[keys];
-        const u64 grand = (u64)total * (u64)g.G;
-        for (int p = blockIdx.x; p <= g.pieces; p += gridDim.x) {
-            int L;
-            if (p == 0) L = 0;
-            else if (p == g.pieces) L = g.G * g.keys;
-            else {
-                const u64 target = grand / (u64)g.pieces * (u64)p + (grand % (u64)g.pieces) * (u64)p / (u64)g.pieces;
-                int lo = 0, hi = g.Q - 1;
-                while (lo < hi) {
-                    const int mid = (lo + hi + 1) >> 1;
-                    if ((u64)g.G * (u64)s_cpre[g.colstart[mid]] <= target) lo = mid; else hi = mid - 1;
-                }
-                const int q = lo;
-                const int kb = g.colstart[q], Hq = g.colstart[q + 1] - kb;
-                const unsigned c0 = s_cpre[kb];
-                const unsigned colsum = s_cpre[kb + Hq] - c0;                 // >= kRowCost * Hq > 0
-                u64 rem = target - (u64)g.G * (u64)c0;
-                int gg = (int)(rem / colsum);
-                if (gg > g.G - 1) gg = g.G - 1;
-                rem -= (u64)gg * colsum;
-                int ylo = 0, yhi = Hq - 1;
-                while (ylo < yhi) {
-                    const int mid = (ylo + yhi + 1) >> 1;
-                    if ((u64)(s_cpre[kb + mid] - c0) <= rem) ylo = mid; else yhi = mid - 1;
-                }
-                L = g.G * kb + gg * Hq + ylo;
-            }
-            ws.piece_start[p] = L;
-        }
-    }
+    // piece boundaries: every CTA holds the whole prefix, so they are spread over the grid (one per CTA, thread 0)
+    if (t == 0)
+        for (int p = blockIdx.x; p <= g.pieces; p += gridDim.x)
+            ws.piece_start[p] = prepass::piece_start(p, g.pieces, g.G, keys, g.Q, g.colstart, s_cpre);
     // ---- phase 3: fragment records into the CSR (position = row pointer + rank); zero-fill of the elements that are
     // accumulated with red.add (the bins of the fragments that hold a split bin's first sample)
     const int bins = g.PH * g.PW;
