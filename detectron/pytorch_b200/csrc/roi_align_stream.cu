@@ -490,6 +490,20 @@ __device__ __forceinline__ void stage_row(const float* __restrict__ src_row, siz
     }
 }
 
+// Prefetch into L2 the output runs fragment `en` will store (lane = channel: the first and the last bin of its run, at most
+// two sectors).  A run is npw <= 8 consecutive floats of one channel plane, so every flush store covers only part of a
+// 32-byte sector, and such a store that misses L2 stalls the memory pipeline the bin loop's shared-memory loads share (at
+// cfg2 the main kernel spans 115 us with the stores and 57 us without them; 95 us with this prefetch: DESIGN.md 4.1a).
+__device__ __forceinline__ void prefetch_out(const uint2& en, const StreamArgs& a, int c0, int bins, int lane) {
+    const int r = en.x & 0xffffu, ph = (en.x >> 16) & 31u, pw0 = (en.x >> 21) & 31u, npw = (int)((en.x >> 26) & 7u) + 1;
+    if (c0 + lane < a.C) {
+        const int orow = a.row_map ? __ldg(&a.row_map[r]) : r;
+        const float* p = a.out + ((size_t)orow * a.C + c0 + lane) * bins + ph * a.PW + pw0;
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+        asm volatile("prefetch.global.L2 [%0];" ::"l"(p + npw - 1));
+    }
+}
+
 template <int SR, int M>
 __global__ void __launch_bounds__(kStreamThreads, 1)
 roi_align_stream_fwd(const StreamArgs a) {
@@ -644,6 +658,7 @@ roi_align_stream_fwd(const StreamArgs a) {
                 acquire_to(acq + 1, 0x2000u);
                 release_to(acq);
             }
+            prefetch_out(cur, a, c0, bins, lane);               // lands while this warp waits for its rows and computes
             acquire_to(end, 0x2800u);                           // rows [key, end) must be resident
             const uint4 yA = lds128(tbuf + 16 * 16);
             uint4 yB = yA;
