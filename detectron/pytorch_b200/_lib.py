@@ -133,6 +133,29 @@ _SIGNATURES = {
     # (src, descs, N, mean_table, blob_h, blob_w, out, stream)
     "b200_image_blob": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                        _c_float_p, _stream_t]),
+    # (P, pair_det_begin, pair_entry_begin, det_score, entry_det, entry_rank, entry_score, stream)
+    "b200_coco_rank": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 6 + [_stream_t]),
+    # (P, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_box, gt_box, gt_flags, ious, stream)
+    "b200_coco_bbox_iou": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 8 + [_stream_t]),
+    # (P, vars_host, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_kp, gt_kp, gt_box, gt_area, ious, stream)
+    "b200_coco_oks": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 10 + [_stream_t]),
+    # (words, num_words, S, slot_word, slot_hw, n_str, str_slot, str_begin, bytes, n_cnt, cnt_slot, cnt_begin, counts, n_poly, n_vtx,
+    #  poly_slot, vtx_begin, xy, n_masks, mask_slot_begin, mask_area, mask_range, stream)
+    "b200_coco_masks": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_longlong, ctypes.c_int] + [ctypes.c_void_p] * 2 + [ctypes.c_int] +
+                        [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 3 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 3 +
+                        [ctypes.c_int] + [ctypes.c_void_p] * 3 + [_stream_t]),
+    # (pair_begin, P, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det0, gt0, gt_mask0, mask_slot_begin, slot_word,
+    #  slot_hw, words, mask_area, mask_range, gt_flags, ious, stream)
+    "b200_coco_segm_iou": (ctypes.c_int, [ctypes.c_int] * 2 + [ctypes.c_void_p] * 4 + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 8 +
+                           [_stream_t]),
+    # (P, T, iou_thrs_host, A, area_rng_host, max_gt, pair_gt_begin, pair_entry_begin, pair_iou_begin, pair_cat, entry_det, det_area,
+    #  gt_area, gt_flags, ious, E, entry_flags, npig, stream)
+    "b200_coco_match": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int] +
+                        [ctypes.c_void_p] * 9 + [ctypes.c_int] + [ctypes.c_void_p] * 2 + [_stream_t]),
+    # (K, A, M, T, R, max_dets_host, cat_entry_begin, cat_pairs, order, entry_rank, entry_score, entry_flags, E, max_cat_entries, npig,
+    #  rec_thrs, workspace, workspace_bytes, precision, recall, scores, stream)
+    "b200_coco_accumulate": (ctypes.c_int, [ctypes.c_int] * 5 + [ctypes.c_void_p] * 7 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 3 +
+                             [ctypes.c_size_t] + [ctypes.c_void_p] * 3 + [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

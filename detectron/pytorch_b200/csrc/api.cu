@@ -84,6 +84,19 @@ int rpn_labels(int, const int*, const int*, const double*, const double*, int, c
 int rpn_emit(int, const int*, const int*, const double*, const double*, int, const double*, const int*, const float*, double, const int*,
              const int*, const int*, const int*, const int*, void*, size_t, int* const*, float* const*, float* const*, float* const*,
              cudaStream_t);
+int coco_rank(int, const int*, const int*, const double*, int*, int*, double*, cudaStream_t);
+int coco_bbox_iou(int, const int*, const int*, const long long*, const int*, const double*, const double*, const int*, double*, cudaStream_t);
+int coco_oks(int, const double*, const int*, const int*, const long long*, const int*, const double*, const double*, const double*,
+             const double*, double*, cudaStream_t);
+int coco_masks(unsigned*, long long, int, const long long*, const int*, int, const int*, const long long*, const unsigned char*, int,
+               const int*, const long long*, const unsigned*, int, int, const int*, const int*, const double*, int, const int*, long long*,
+               int*, cudaStream_t);
+int coco_segm_iou(int, int, const int*, const int*, const long long*, const int*, int, int, int, const int*, const long long*, const int*,
+                  const unsigned*, const long long*, const int*, const int*, double*, cudaStream_t);
+int coco_match(int, int, const double*, int, const double*, int, const int*, const int*, const long long*, const int*, const int*,
+               const double*, const double*, const int*, const double*, int, unsigned*, int*, cudaStream_t);
+int coco_accumulate(int, int, int, int, int, const int*, const int*, const int*, const int*, const int*, const double*, const unsigned*, int,
+                    int, const int*, const double*, void*, size_t, double*, double*, double*, cudaStream_t);
 int mask_targets(const float*, const int*, const int*, int, int, const int*, int, const int*, int, const int*, const float*, int, int,
                  float*, int*, cudaStream_t);
 int keypoint_candidates(const float*, const float*, const int*, int, const int*, const int*, const int*, const int*, const int*, int, float,
@@ -695,6 +708,67 @@ int b200_keypoint_targets(const float* boxes_dev, const int* box_to_gt_dev, int 
 int b200_image_blob(const unsigned char* src_dev, const b200_image_blob_desc* descs_dev, int num_images, const float* mean_table_dev,
                     int blob_h, int blob_w, float* out_dev, b200_stream_t stream) {
     return image_blob(src_dev, descs_dev, num_images, mean_table_dev, blob_h, blob_w, out_dev, (cudaStream_t)stream);
+}
+
+int b200_coco_rank(int num_pairs, const int* pair_det_begin_dev, const int* pair_entry_begin_dev, const double* det_score_dev,
+                   int* entry_det_out_dev, int* entry_rank_out_dev, double* entry_score_out_dev, b200_stream_t stream) {
+    return coco_rank(num_pairs, pair_det_begin_dev, pair_entry_begin_dev, det_score_dev, entry_det_out_dev, entry_rank_out_dev,
+                     entry_score_out_dev, (cudaStream_t)stream);
+}
+
+int b200_coco_bbox_iou(int num_pairs, const int* pair_gt_begin_dev, const int* pair_entry_begin_dev, const long long* pair_iou_begin_dev,
+                       const int* entry_det_dev, const double* det_box_dev, const double* gt_box_dev, const int* gt_flags_dev,
+                       double* ious_out_dev, b200_stream_t stream) {
+    return coco_bbox_iou(num_pairs, pair_gt_begin_dev, pair_entry_begin_dev, pair_iou_begin_dev, entry_det_dev, det_box_dev, gt_box_dev,
+                         gt_flags_dev, ious_out_dev, (cudaStream_t)stream);
+}
+
+int b200_coco_oks(int num_pairs, const double* vars_host, const int* pair_gt_begin_dev, const int* pair_entry_begin_dev,
+                  const long long* pair_iou_begin_dev, const int* entry_det_dev, const double* det_kp_dev, const double* gt_kp_dev,
+                  const double* gt_box_dev, const double* gt_area_dev, double* ious_out_dev, b200_stream_t stream) {
+    return coco_oks(num_pairs, vars_host, pair_gt_begin_dev, pair_entry_begin_dev, pair_iou_begin_dev, entry_det_dev, det_kp_dev, gt_kp_dev,
+                    gt_box_dev, gt_area_dev, ious_out_dev, (cudaStream_t)stream);
+}
+
+int b200_coco_masks(unsigned* words_dev, long long num_words, int num_slots, const long long* slot_word_dev, const int* slot_hw_dev,
+                    int num_strings, const int* str_slot_dev, const long long* str_begin_dev, const unsigned char* str_bytes_dev,
+                    int num_counts, const int* cnt_slot_dev, const long long* cnt_begin_dev, const unsigned* counts_dev,
+                    int num_polys, int num_vertices, const int* poly_slot_dev, const int* vtx_begin_dev, const double* xy_dev,
+                    int num_masks, const int* mask_slot_begin_dev, long long* mask_area_out_dev, int* mask_range_out_dev,
+                    b200_stream_t stream) {
+    return coco_masks(words_dev, num_words, num_slots, slot_word_dev, slot_hw_dev, num_strings, str_slot_dev, str_begin_dev, str_bytes_dev,
+                      num_counts, cnt_slot_dev, cnt_begin_dev, counts_dev, num_polys, num_vertices, poly_slot_dev, vtx_begin_dev, xy_dev,
+                      num_masks, mask_slot_begin_dev, mask_area_out_dev, mask_range_out_dev, (cudaStream_t)stream);
+}
+
+int b200_coco_segm_iou(int pair_begin, int num_pairs, const int* pair_gt_begin_dev, const int* pair_entry_begin_dev,
+                       const long long* pair_iou_begin_dev, const int* entry_det_dev, int det0, int gt0, int gt_mask0,
+                       const int* mask_slot_begin_dev, const long long* slot_word_dev, const int* slot_hw_dev, const unsigned* words_dev,
+                       const long long* mask_area_dev, const int* mask_range_dev, const int* gt_flags_dev, double* ious_out_dev,
+                       b200_stream_t stream) {
+    return coco_segm_iou(pair_begin, num_pairs, pair_gt_begin_dev, pair_entry_begin_dev, pair_iou_begin_dev, entry_det_dev, det0, gt0,
+                         gt_mask0, mask_slot_begin_dev, slot_word_dev, slot_hw_dev, words_dev, mask_area_dev, mask_range_dev, gt_flags_dev,
+                         ious_out_dev, (cudaStream_t)stream);
+}
+
+int b200_coco_match(int num_pairs, int num_thresholds, const double* iou_thrs_host, int num_areas, const double* area_rng_host, int max_gt,
+                    const int* pair_gt_begin_dev, const int* pair_entry_begin_dev, const long long* pair_iou_begin_dev,
+                    const int* pair_cat_dev, const int* entry_det_dev, const double* det_area_dev, const double* gt_area_dev,
+                    const int* gt_flags_dev, const double* ious_dev, int num_entries, unsigned* entry_flags_dev, int* npig_dev,
+                    b200_stream_t stream) {
+    return coco_match(num_pairs, num_thresholds, iou_thrs_host, num_areas, area_rng_host, max_gt, pair_gt_begin_dev, pair_entry_begin_dev,
+                      pair_iou_begin_dev, pair_cat_dev, entry_det_dev, det_area_dev, gt_area_dev, gt_flags_dev, ious_dev, num_entries,
+                      entry_flags_dev, npig_dev, (cudaStream_t)stream);
+}
+
+int b200_coco_accumulate(int num_cats, int num_areas, int num_max_dets, int num_thresholds, int num_recall, const int* max_dets_host,
+                         const int* cat_entry_begin_dev, const int* cat_pairs_dev, const int* order_dev, const int* entry_rank_dev,
+                         const double* entry_score_dev, const unsigned* entry_flags_dev, int num_entries, int max_cat_entries,
+                         const int* npig_dev, const double* rec_thrs_dev, void* workspace, size_t workspace_bytes, double* precision_out_dev,
+                         double* recall_out_dev, double* scores_out_dev, b200_stream_t stream) {
+    return coco_accumulate(num_cats, num_areas, num_max_dets, num_thresholds, num_recall, max_dets_host, cat_entry_begin_dev, cat_pairs_dev,
+                           order_dev, entry_rank_dev, entry_score_dev, entry_flags_dev, num_entries, max_cat_entries, npig_dev, rec_thrs_dev, workspace,
+                           workspace_bytes, precision_out_dev, recall_out_dev, scores_out_dev, (cudaStream_t)stream);
 }
 
 }  // extern "C"

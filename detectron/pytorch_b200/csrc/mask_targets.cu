@@ -15,9 +15,7 @@
 // monotone, so the single walk step that crosses column c (u from 5c + 2 to 5c + 3 or back) is found by bisection with the
 // reference's own rounding.  Crossings toggle one bit of a per-column 64-bit word (XOR, so duplicates cancel); a prefix
 // parity over the column-major order, carried across columns, gives the filled polygon.
-#include <climits>
-
-#include "common.cuh"
+#include "poly_walk.cuh"
 
 namespace b200 {
 
@@ -28,7 +26,6 @@ namespace {
 
 constexpr int kMaskThreads = 256;
 constexpr int kPolyBatch = 16;       // polygons rasterised side by side in one CTA (an object with more takes several rounds)
-constexpr int kUpsample = 5;         // rleFrPoly's `scale`
 
 struct MaskImages {
     int num_images;
@@ -55,81 +52,23 @@ mask_boxes_kernel(int num_objects, int num_polys, int num_coords, const int* __r
     if (lane == 0) boxes[o] = make_float4(x0, y0, x1, y1);
 }
 
-// One edge of the upsampled walk, after rleFrPoly's swap.  Walk point d (0..n) is t = flip ? n - d : d.
-struct Edge {
-    int xs, ys, n;
-    bool shallow, flip, degenerate;
-    double s;
-};
+using poly::Edge;
+using poly::edge_u;
+using poly::edge_v;
+using poly::make_edge;
+using poly::kUpsample;
 
-__device__ __forceinline__ Edge make_edge(int xs, int ys, int xe, int ye) {
-    Edge e;
-    const int dx = abs(xe - xs), dy = abs(ys - ye);
-    e.shallow = dx >= dy;
-    e.flip = (e.shallow && xs > xe) || (!e.shallow && ys > ye);
-    if (e.flip) { int t = xs; xs = xe; xe = t; t = ys; ys = ye; ye = t; }
-    e.xs = xs; e.ys = ys;
-    e.n = e.shallow ? dx : dy;
-    e.degenerate = dx == 0 && dy == 0;                                  // 0 / 0: the point's v is never a kept crossing's
-    e.s = e.degenerate ? 0.0 : e.shallow ? __ddiv_rn((double)(ye - ys), (double)dx) : __ddiv_rn((double)(xe - xs), (double)dy);
-    return e;
-}
-
-// (int)(a + s * t + .5): separate double roundings, C truncation
-__device__ __forceinline__ int interp(int a, double s, int t) {
-    return __double2int_rz(__dadd_rn(__dadd_rn((double)a, __dmul_rn(s, (double)t)), 0.5));
-}
-
-__device__ __forceinline__ int edge_u(const Edge& e, int d) {
-    const int t = e.flip ? e.n - d : d;
-    return e.shallow ? e.xs + t : interp(e.xs, e.s, t);
-}
-
-__device__ __forceinline__ int edge_v(const Edge& e, int d) {
-    const int t = e.flip ? e.n - d : d;
-    return e.shallow ? (e.degenerate ? INT_MIN : interp(e.ys, e.s, t)) : e.ys + t;   // INT_MIN: x86 cvttsd2si of NaN
-}
-
-// the crossing between consecutive walk points (pu, pv) -> (qu, qv), exactly rleFrPoly's downsampling: a toggle in column
-// xd at row yd, stored as bit yd of word xd (yd == h is the top of the next column; past the last column it is the sentinel)
+// a kept crossing toggles bit yd of column word xd (yd == h is the top of the next column; past the last column it is the
+// sentinel)
 __device__ __forceinline__ void crossing(int pu, int pv, int qu, int qv, int h, int w, unsigned long long* tog) {
-    if (qu == pu) return;
-    double xd = (double)(qu < pu ? qu : qu - 1);
-    xd = __dsub_rn(__ddiv_rn(__dadd_rn(xd, 0.5), (double)kUpsample), 0.5);
-    if (floor(xd) != xd || xd < 0.0 || xd > (double)(w - 1)) return;
-    double yd = (double)min(pv, qv);
-    yd = __dsub_rn(__ddiv_rn(__dadd_rn(yd, 0.5), (double)kUpsample), 0.5);
-    yd = yd < 0.0 ? 0.0 : yd > (double)h ? (double)h : yd;
-    int c = (int)xd, y = (int)ceil(yd);
+    int c, y;
+    if (!poly::crossing(pu, pv, qu, qv, h, w, c, y)) return;
     if (y == h) { ++c; y = 0; }
     if (c < w) atomicXor(tog + c, 1ull << y);
 }
 
-// floor(a / 5) for any sign
-__device__ __forceinline__ int floordiv5(long long a) { return (int)(a >= 0 ? a / kUpsample : -((-a + kUpsample - 1) / kUpsample)); }
-
-// every crossing inside one edge: u is monotone along the walk, so the step that crosses column c is the first walk point
-// past it, found by bisection; it is a crossing iff it lands exactly on 5c + 3 (rising) or 5c + 2 (falling)
-__device__ void edge_crossings(const Edge& e, int h, int w, unsigned long long* tog) {
-    if (e.n == 0) return;
-    const int u0 = edge_u(e, 0), un = edge_u(e, e.n);
-    if (u0 == un) return;
-    const bool rising = un > u0;
-    // rising: columns with 5c + 3 in (u0, un]; falling: 5c + 2 in [un, u0)
-    const int clo = max(rising ? floordiv5((long long)u0 - 3) + 1 : floordiv5((long long)un - 2 + kUpsample - 1), 0);
-    const int chi = min(rising ? floordiv5((long long)un - 3) : floordiv5((long long)u0 - 3), w - 1);
-    for (int c = clo; c <= chi; ++c) {
-        const int target = rising ? kUpsample * c + 3 : kUpsample * c + 2;
-        int lo = 1, hi = e.n;                                             // point 0 is on the near side of the column
-        while (lo < hi) {
-            const int mid = lo + ((hi - lo) >> 1);
-            const int u = edge_u(e, mid);
-            if (rising ? u >= target : u <= target) hi = mid; else lo = mid + 1;
-        }
-        const int q = edge_u(e, lo);
-        if (q != target) continue;                                        // the walk jumped over it: no crossing here
-        crossing(edge_u(e, lo - 1), edge_v(e, lo - 1), q, edge_v(e, lo), h, w, tog);
-    }
+__device__ __forceinline__ void edge_crossings(const Edge& e, int h, int w, unsigned long long* tog) {
+    poly::edge_crossings(e, w, [&](int pu, int pv, int qu, int qv) { crossing(pu, pv, qu, qv, h, w, tog); });
 }
 
 // float32 normalisation to the RoI (segms.py:104-110), then rleFrPoly's (int)(5 * x + .5)

@@ -1,0 +1,219 @@
+"""The reference's COCO evaluators (lib/datasets/json_dataset_evaluator.py:38-233, 320-430) with COCOeval on the device.
+
+evaluate_boxes / evaluate_masks / evaluate_keypoints take the reference's arguments and return an object shaped like
+pycocotools' COCOeval after accumulate() and summarize() (datasets/coco_eval.py): `.params`, `.eval`, `.stats`,
+`.summarize()`.  They log the reference's per-category AP lines and pickle the result to its file names in output_dir.
+
+The results are not written to JSON and read back: the evaluator works on the float64 values the reference's writers put in
+that file (json round-trips float64 exactly).  The conversion is the writers', step for step:
+  * boxes: float64 of the float32 all_boxes, xyxy_to_xywh with the + 1, score = the box's last column;
+  * masks: the compressed COCO strings of all_segms, the box score;
+  * keypoints: float64 of x and y of cls_keyps (v = 1), score = the box score (KEYPOINT_CONFIDENCE 'bbox') or the mean of
+    row 2 ('logit') / row 3 ('prob') over the keypoints, summed in order in float64 -- the reference's `kps_score = 0;
+    kps_score += ...` under numpy 1's promotion of a Python int plus a float32 scalar.
+`use_salt` / `cleanup` are accepted for the reference's signature; there is no results file to salt or remove.
+"""
+import json
+import logging
+import os
+import pickle
+
+import numpy as np
+
+from . import coco_eval
+
+logger = logging.getLogger(__name__)
+
+
+class JsonDataset:
+    """The parts of the reference's JsonDataset the evaluators read: name, classes, category_to_id_map and COCO, whose
+    `dataset` is the annotation-file dict and getImgIds() its image ids."""
+
+    class _Coco:
+        def __init__(self, dataset):
+            self.dataset = dataset
+
+        def getImgIds(self):
+            return [img["id"] for img in self.dataset.get("images", [])]
+
+        def getCatIds(self):
+            return [c["id"] for c in self.dataset.get("categories", [])]
+
+    def __init__(self, name, dataset):
+        self.name = name
+        self.COCO = JsonDataset._Coco(dataset)
+        category_ids = sorted(self.COCO.getCatIds())
+        names = {c["id"]: c["name"] for c in dataset.get("categories", [])}
+        categories = [names[i] for i in category_ids]
+        self.category_to_id_map = dict(zip(categories, category_ids))     # json_dataset.py:69-80
+        self.classes = ["__background__"] + categories
+        self.num_classes = len(self.classes)
+        self.json_category_id_to_contiguous_id = {v: i + 1 for i, v in enumerate(category_ids)}
+        self.contiguous_category_id_to_json_id = {v: k for k, v in self.json_category_id_to_contiguous_id.items()}
+
+
+def load_json_dataset(name, annotation_file_or_dict):
+    """A JsonDataset from a COCO annotation file (path) or its already-loaded dict, without pycocotools."""
+    if isinstance(annotation_file_or_dict, dict):
+        return JsonDataset(name, annotation_file_or_dict)
+    with open(annotation_file_or_dict) as f:
+        return JsonDataset(name, json.load(f))
+
+
+def _image_ids(json_dataset):
+    ids = json_dataset.COCO.getImgIds()
+    ids.sort()
+    return ids
+
+
+def _classes(json_dataset, n):
+    """(cls_ind, cat_id) in the writers' order: classes after __background__, stopping at the length of the per-class list."""
+    for cls_ind, cls in enumerate(json_dataset.classes):
+        if cls == "__background__":
+            continue
+        if cls_ind >= n:
+            break
+        yield cls_ind, json_dataset.category_to_id_map[cls]
+
+
+def _empty(dets):
+    return isinstance(dets, list) and len(dets) == 0
+
+
+def _box_results(json_dataset, all_boxes):
+    image_ids = _image_ids(json_dataset)
+    img, cat, score, box = [], [], [], []
+    for cls_ind, cat_id in _classes(json_dataset, len(all_boxes)):
+        assert len(all_boxes[cls_ind]) == len(image_ids)
+        for i, image_id in enumerate(image_ids):
+            dets = all_boxes[cls_ind][i]
+            if _empty(dets):
+                continue
+            dets = np.asarray(dets).astype(np.float64)
+            xy = dets[:, 0:4]
+            box.append(np.hstack((xy[:, 0:2], xy[:, 2:4] - xy[:, 0:2] + 1)))      # utils/boxes.py xyxy_to_xywh
+            score.append(dets[:, -1]); img.append(np.full(len(dets), image_id)); cat.append(np.full(len(dets), cat_id))
+    cat_ = lambda xs, w: np.concatenate(xs) if xs else np.zeros((0,) + w)  # noqa: E731
+    return coco_eval.Detections(cat_(img, ()), cat_(cat, ()), cat_(score, ()), box=cat_(box, (4,)))
+
+
+def _segm_results(json_dataset, all_boxes, all_segms):
+    image_ids = _image_ids(json_dataset)
+    img, cat, score, strings = [], [], [], []
+    for cls_ind, cat_id in _classes(json_dataset, len(all_boxes)):
+        assert len(all_boxes[cls_ind]) == len(image_ids) and len(all_segms[cls_ind]) == len(image_ids)
+        for i, image_id in enumerate(image_ids):
+            dets = all_boxes[cls_ind][i]
+            if _empty(dets):
+                continue
+            rles = all_segms[cls_ind][i]
+            dets = np.asarray(dets).astype(np.float64)
+            for k in range(dets.shape[0]):
+                c = rles[k]["counts"]
+                if isinstance(c, list):
+                    raise ValueError("all_segms holds compressed COCO RLEs (strings), got uncompressed counts")
+                strings.append((c.encode("ascii") if isinstance(c, str) else bytes(c), tuple(int(v) for v in rles[k]["size"])))
+            score.append(dets[:, -1]); img.append(np.full(len(dets), image_id)); cat.append(np.full(len(dets), cat_id))
+    cat_ = lambda xs: np.concatenate(xs) if xs else np.zeros(0)  # noqa: E731
+    return coco_eval.Detections(cat_(img), cat_(cat), cat_(score), strings=strings)
+
+
+def _keypoint_confidence(cfg, keypoint_confidence):
+    if keypoint_confidence is None:
+        keypoint_confidence = cfg.KRCNN.KEYPOINT_CONFIDENCE if cfg is not None else "bbox"
+    if keypoint_confidence not in ("logit", "prob", "bbox"):
+        raise ValueError('KRCNN.KEYPOINT_CONFIDENCE must be "logit", "prob", or "bbox"')
+    return keypoint_confidence
+
+
+def _keypoint_results(json_dataset, all_boxes, all_keyps, confidence):
+    image_ids = _image_ids(json_dataset)
+    img, cat, score, kps = [], [], [], []
+    for cls_ind, cat_id in _classes(json_dataset, len(all_keyps)):
+        assert len(all_keyps[cls_ind]) == len(image_ids) and len(all_boxes[cls_ind]) == len(image_ids)
+        for i, image_id in enumerate(image_ids):
+            if len(all_boxes[cls_ind][i]) == 0:
+                continue
+            kps_dets = all_keyps[cls_ind][i]
+            if len(kps_dets) == 0:
+                continue
+            scores = np.asarray(all_boxes[cls_ind][i])[:, -1].astype(np.float64)
+            for j in range(len(kps_dets)):
+                kd = np.asarray(kps_dets[j])
+                if kd.shape[1] != 17:
+                    raise ValueError("COCO keypoints are 17 per person, got %d" % kd.shape[1])
+                xyv = np.stack([kd[0].astype(np.float64), kd[1].astype(np.float64), np.ones(17)], axis=1)
+                if confidence == "bbox":
+                    s = scores[j]
+                else:
+                    row = kd[2 if confidence == "logit" else 3].astype(np.float64)
+                    s = 0.0
+                    for v in row:                                          # in order, in float64
+                        s += v
+                    s /= kd.shape[1]
+                kps.append(xyv); score.append(s); img.append(image_id); cat.append(cat_id)
+    return coco_eval.Detections(img, cat, score, keypoints=np.asarray(kps, np.float64).reshape(-1, 17, 3))
+
+
+def _save(result, output_dir, file_name):
+    eval_file = os.path.join(output_dir, file_name)
+    with open(eval_file, "wb") as f:
+        pickle.dump(result, f, pickle.HIGHEST_PROTOCOL)
+    logger.info("Wrote json eval results to: {}".format(eval_file))
+
+
+def _log_detection_eval_metrics(json_dataset, coco_eval_result):
+    """The reference's mean and per-category AP at IoU 0.50:0.95 (area all, 100 detections), then summarize()."""
+    def _get_thr_ind(thr):
+        ind = np.where((coco_eval_result.params.iouThrs > thr - 1e-5) & (coco_eval_result.params.iouThrs < thr + 1e-5))[0][0]
+        assert np.isclose(coco_eval_result.params.iouThrs[ind], thr)
+        return ind
+
+    ind_lo, ind_hi = _get_thr_ind(0.5), _get_thr_ind(0.95)
+    precision = coco_eval_result.eval["precision"][ind_lo:(ind_hi + 1), :, :, 0, 2]
+    ap_default = np.mean(precision[precision > -1])
+    logger.info("~~~~ Mean and per-category AP @ IoU=[{:.2f},{:.2f}] ~~~~".format(0.5, 0.95))
+    logger.info("{:.1f}".format(100 * ap_default))
+    for cls_ind, cls in enumerate(json_dataset.classes):
+        if cls == "__background__":
+            continue
+        precision = coco_eval_result.eval["precision"][ind_lo:(ind_hi + 1), :, cls_ind - 1, 0, 2]
+        ap = np.mean(precision[precision > -1])
+        logger.info("{:.1f}".format(100 * ap))
+    logger.info("~~~~ Summary metrics ~~~~")
+    coco_eval_result.summarize()
+
+
+def _evaluates(json_dataset):
+    return json_dataset.name.find("test") == -1                          # annotations of test sets are undisclosed
+
+
+def evaluate_boxes(json_dataset, all_boxes, output_dir, use_salt=True, cleanup=False, device=None):
+    if not _evaluates(json_dataset):
+        return None
+    res = coco_eval.evaluate(json_dataset.COCO.dataset, _box_results(json_dataset, all_boxes), "bbox", device)
+    _log_detection_eval_metrics(json_dataset, res)
+    _save(res, output_dir, "detection_results.pkl")
+    return res
+
+
+def evaluate_masks(json_dataset, all_boxes, all_segms, output_dir, use_salt=True, cleanup=False, device=None):
+    if not _evaluates(json_dataset):
+        return None
+    res = coco_eval.evaluate(json_dataset.COCO.dataset, _segm_results(json_dataset, all_boxes, all_segms), "segm", device)
+    _log_detection_eval_metrics(json_dataset, res)
+    _save(res, output_dir, "segmentation_results.pkl")
+    return res
+
+
+def evaluate_keypoints(json_dataset, all_boxes, all_keypoints, output_dir, use_salt=True, cleanup=False, cfg=None,
+                       keypoint_confidence=None, device=None):
+    """KRCNN.KEYPOINT_CONFIDENCE comes from `keypoint_confidence`, else from cfg.KRCNN.KEYPOINT_CONFIDENCE, else 'bbox'."""
+    confidence = _keypoint_confidence(cfg, keypoint_confidence)
+    if not _evaluates(json_dataset):
+        return None
+    res = coco_eval.evaluate(json_dataset.COCO.dataset, _keypoint_results(json_dataset, all_boxes, all_keypoints, confidence),
+                             "keypoints", device)
+    _save(res, output_dir, "keypoint_results.pkl")
+    res.summarize()
+    return res

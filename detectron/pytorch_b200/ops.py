@@ -1028,3 +1028,116 @@ def image_blob_raw(images, scales, flipped, pixel_means, stride, out=None):
         _lib.check(_lib.load().b200_image_blob(base, base, N, base + descs.nbytes, Hp, Wp, out.data_ptr(), _stream()),
                    "b200_image_blob")
     return out, sizes
+
+
+# ------------------------------------------------------------------------------------------------
+# COCO evaluation stages (pycocotools COCOeval.evaluate / accumulate; datasets/coco_eval.py drives them)
+# ------------------------------------------------------------------------------------------------
+def _ptr(t):
+    return 0 if t is None else t.data_ptr()
+
+
+def coco_rank_raw(pair_det_begin, pair_entry_begin, det_score, num_entries):
+    """Stable descending-score rank per (image, category) pair, cut to each pair's entry count (COCOeval.computeIoU /
+    evaluateImg's mergesort on -score and [0:maxDets[-1]]).  Returns (entry_det int32, entry_rank int32, entry_score f64)."""
+    dev = det_score.device
+    P = pair_det_begin.numel() - 1
+    entry_det = torch.empty((max(num_entries, 1),), dtype=torch.int32, device=dev)
+    entry_rank = torch.empty_like(entry_det)
+    entry_score = torch.empty((max(num_entries, 1),), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().b200_coco_rank(P, pair_det_begin.data_ptr(), pair_entry_begin.data_ptr(), det_score.data_ptr(),
+                                              entry_det.data_ptr(), entry_rank.data_ptr(), entry_score.data_ptr(), _stream()),
+                   "b200_coco_rank")
+    return entry_det, entry_rank, entry_score
+
+
+def coco_bbox_iou_raw(pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_box, gt_box, gt_flags, ious):
+    """computeIoU for iouType 'bbox' (maskApi bbIou) of every pair into `ious` (float64, rows = entries)."""
+    with torch.cuda.device(ious.device):
+        _lib.check(_lib.load().b200_coco_bbox_iou(pair_gt_begin.numel() - 1, pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(),
+                                                  pair_iou_begin.data_ptr(), entry_det.data_ptr(), det_box.data_ptr(), gt_box.data_ptr(),
+                                                  gt_flags.data_ptr(), ious.data_ptr(), _stream()), "b200_coco_bbox_iou")
+
+
+def coco_oks_raw(vars, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_kp, gt_kp, gt_box, gt_area, ious):
+    """computeOks of every pair into `ious`; vars = (sigmas * 2) ** 2 as a host float64 array of 17."""
+    import ctypes
+    import numpy as np
+    v = np.ascontiguousarray(vars, np.float64)
+    if v.size != 17:
+        raise ValueError("OKS needs 17 keypoint variances, got %d" % v.size)
+    with torch.cuda.device(ious.device):
+        _lib.check(_lib.load().b200_coco_oks(pair_gt_begin.numel() - 1, v.ctypes.data_as(ctypes.c_void_p), pair_gt_begin.data_ptr(),
+                                             pair_entry_begin.data_ptr(), pair_iou_begin.data_ptr(), entry_det.data_ptr(), det_kp.data_ptr(),
+                                             gt_kp.data_ptr(), gt_box.data_ptr(), gt_area.data_ptr(), ious.data_ptr(), _stream()),
+                   "b200_coco_oks")
+
+
+def coco_masks_raw(words, slot_word, slot_hw, strings, counts, polys, mask_slot_begin, mask_area, mask_range):
+    """Mask bitmaps (annToRLE: rleFrString, uncompressed counts, rleFrPoly + merge) into `words`.  strings / counts / polys are
+    (slot, begin, data) triples of device tensors, or None; polys' begin is per-polygon vertex offsets and data float64 x, y."""
+    def parts(x):
+        return (0, None, None, None) if x is None else (x[0].numel(), x[0], x[1], x[2])
+    ns, ss, sb, sd = parts(strings)
+    nc, cs, cb, cd = parts(counts)
+    npl, ps, pb, pd = parts(polys)
+    with torch.cuda.device(words.device):
+        _lib.check(_lib.load().b200_coco_masks(words.data_ptr(), words.numel(), slot_hw.size(0), slot_word.data_ptr(), slot_hw.data_ptr(),
+                                               ns, _ptr(ss), _ptr(sb), _ptr(sd), nc, _ptr(cs), _ptr(cb), _ptr(cd),
+                                               npl, 0 if pd is None else pd.numel() // 2, _ptr(ps), _ptr(pb), _ptr(pd),
+                                               mask_slot_begin.numel() - 1, mask_slot_begin.data_ptr(), mask_area.data_ptr(),
+                                               mask_range.data_ptr(), _stream()), "b200_coco_masks")
+
+
+def coco_segm_iou_raw(pair_begin, num_pairs, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det0, gt0, gt_mask0,
+                      mask_slot_begin, slot_word, slot_hw, words, mask_area, mask_range, gt_flags, ious):
+    """computeIoU for iouType 'segm' (rleIou) of pairs pair_begin .. + num_pairs - 1 on the bitmaps of one coco_masks_raw call."""
+    with torch.cuda.device(ious.device):
+        _lib.check(_lib.load().b200_coco_segm_iou(pair_begin, num_pairs, pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(),
+                                                  pair_iou_begin.data_ptr(), entry_det.data_ptr(), det0, gt0, gt_mask0,
+                                                  mask_slot_begin.data_ptr(), slot_word.data_ptr(), slot_hw.data_ptr(), words.data_ptr(),
+                                                  mask_area.data_ptr(), mask_range.data_ptr(), gt_flags.data_ptr(), ious.data_ptr(),
+                                                  _stream()), "b200_coco_segm_iou")
+
+
+def coco_match_raw(iou_thrs, area_rng, max_gt, num_cats, pair_gt_begin, pair_entry_begin, pair_iou_begin, pair_cat, entry_det, det_area,
+                   gt_area, gt_flags, ious, num_entries):
+    """evaluateImg at maxDets[-1] for every pair and area range.  Returns (entry_flags (A, E) uint32 as int32 bits, npig (K, A))."""
+    import ctypes
+    import numpy as np
+    thr = np.ascontiguousarray(iou_thrs, np.float64)
+    rng = np.ascontiguousarray(area_rng, np.float64).reshape(-1)
+    A, dev = rng.size // 2, ious.device
+    flags = torch.zeros((A, max(num_entries, 1)), dtype=torch.int32, device=dev)
+    npig = torch.zeros((num_cats, A), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().b200_coco_match(pair_gt_begin.numel() - 1, thr.size, thr.ctypes.data_as(ctypes.c_void_p), A,
+                                               rng.ctypes.data_as(ctypes.c_void_p), int(max_gt), pair_gt_begin.data_ptr(),
+                                               pair_entry_begin.data_ptr(), pair_iou_begin.data_ptr(), pair_cat.data_ptr(), entry_det.data_ptr(),
+                                               det_area.data_ptr(), gt_area.data_ptr(), gt_flags.data_ptr(), ious.data_ptr(), num_entries,
+                                               flags.data_ptr(), npig.data_ptr(), _stream()), "b200_coco_match")
+    return flags, npig
+
+
+def coco_accumulate_raw(max_dets, cat_entry_begin, cat_pairs, order, entry_rank, entry_score, entry_flags, npig, rec_thrs, T, num_entries,
+                        max_cat_entries):
+    """accumulate(): precision / scores (T, R, K, A, M) and recall (T, K, A, M) float64 on the device, -1 where COCOeval skips.
+    max_cat_entries: the largest category's entry count (host int, < 2^21)."""
+    import ctypes
+    import numpy as np
+    md = np.ascontiguousarray(max_dets, np.int32)
+    K, A = npig.shape
+    M, R, dev = md.size, rec_thrs.numel(), npig.device
+    precision = torch.full((T, R, K, A, M), -1.0, dtype=torch.float64, device=dev)
+    scores = torch.full((T, R, K, A, M), -1.0, dtype=torch.float64, device=dev)
+    recall = torch.full((T, K, A, M), -1.0, dtype=torch.float64, device=dev)
+    ws_bytes = A * M * num_entries * 20
+    ws = torch.empty((max(ws_bytes // 8, 1),), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().b200_coco_accumulate(K, A, M, T, R, md.ctypes.data_as(ctypes.c_void_p), cat_entry_begin.data_ptr(),
+                                                    cat_pairs.data_ptr(), order.data_ptr(), entry_rank.data_ptr(), entry_score.data_ptr(),
+                                                    entry_flags.data_ptr(), num_entries, int(max_cat_entries), npig.data_ptr(), rec_thrs.data_ptr(), ws.data_ptr(),
+                                                    ws_bytes, precision.data_ptr(), recall.data_ptr(), scores.data_ptr(), _stream()),
+                   "b200_coco_accumulate")
+    return precision, recall, scores

@@ -460,6 +460,70 @@ typedef struct b200_image_blob_desc {
 B200_API int b200_image_blob(const unsigned char* src_dev, const b200_image_blob_desc* descs_dev, int num_images, const float* mean_table_dev,
                              int blob_h, int blob_w, float* out_dev, b200_stream_t stream);
 
+/* ---- COCO evaluation (lib/datasets/json_dataset_evaluator.py:38-233, 320-430 -> pycocotools COCOeval) --------------------
+ * The device stages of COCOeval.evaluate() and accumulate() for one iouType.  Work is grouped per (image, category) pair; pairs
+ * are ordered image-major.  Pair p owns detections pair_det_begin[p] .. [p + 1] - 1 (results order), ground truth
+ * pair_gt_begin[p] .. [p + 1] - 1 (annotation order), entries pair_entry_begin[p] .. [p + 1] - 1 (min(D, maxDets[-1]) each)
+ * and IoU rows pair_iou_begin[p] (int64, entries x ground truth, float64, row = entry).  All tables are DEVICE int32 unless
+ * stated.  gt_flags: bit 0 iscrowd, bit 1 ignore (iscrowd, or num_keypoints == 0 for keypoints), bit 2 annotation id != 0.
+ * b200_coco_rank        (computeIoU's / evaluateImg's mergesort on -score, cut to maxDets[-1]) writes entry r of pair p:
+ *                       entry_det (detection index), entry_rank (r), entry_score (float64).
+ * b200_coco_bbox_iou    (computeIoU, iouType 'bbox': maskApi bbIou) det_box / gt_box float64 (x, y, w, h), 16-byte aligned.
+ * b200_coco_oks         (computeOks) det_kp / gt_kp float64 (n, 17, 3) (x, y, v), gt_box float64 (x, y, w, h), gt_area float64,
+ *                       vars_host = (sigmas * 2) ** 2 (17 float64, HOST).  exp() is CUDA's, not numpy's: within a few ulp.
+ * b200_coco_masks       (annToRLE, rleFrString, rleFrPoly, rleMerge) column-major bitmaps: slot s is words[slot_word[s] ..
+ *                       slot_word[s + 1]) (int64 word offsets) of an image of slot_hw[s] = (h, w) int32 pairs.  Strings (compressed
+ *                       COCO counts, str_bytes[str_begin[i] .. [i + 1]), int64 offsets), uncompressed counts (uint32,
+ *                       cnt_begin int64) and polygons (float64 x, y; polygon i is vertices vtx_begin[i] .. [i + 1] - 1, at least 3,
+ *                       |coordinate| <= 2^20) each toggle into their slot; mask m is the union of slots mask_slot_begin[m] ..
+ *                       [m + 1] - 1 (same image size), left in its first slot.  words is zeroed here (num_words words).  Writes
+ *                       mask_area (int64) and mask_range (int32 pairs: first and last non-zero word, (1, 0) when empty).
+ *                       Counts must add up to h * w, as pycocotools assumes.
+ * b200_coco_segm_iou    (computeIoU, iouType 'segm': rleIou) pairs pair_begin .. + num_pairs - 1; detection d is mask d - det0,
+ *                       ground truth g is mask gt_mask0 + g - gt0 of the b200_coco_masks call.
+ * b200_coco_match       (evaluateImg at maxDets[-1]) 1 <= T <= 16 thresholds and 1 <= A <= 8 area ranges (HOST float64, [lo, hi]
+ *                       pairs), A * T <= 64, max_gt = the largest ground truth count of a pair (A * T * max_gt <= 200 KiB).
+ *                       entry_flags (A, num_entries) uint32, zeroed by the caller: bit t = matched to a ground truth with a non-zero
+ *                       id at threshold t, bit 16 + t = ignored.  npig (K, A), zeroed by the caller: += non-ignored ground truth;
+ *                       pair_cat = the pair's category index.
+ * b200_coco_accumulate  (accumulate) order = all entries sorted stably by category index, then descending score, so that ties keep
+ *                       (image, rank) order; category k's are order[cat_entry_begin[k] .. [k + 1]), cat_pairs[k] = its number of
+ *                       pairs.  max_dets_host (M ints, HOST), rec_thrs float64 (R).  precision / scores (T, R, K, A, M) and recall
+ *                       (T, K, A, M) float64 must hold -1 on entry; the skipped (category, area) cells keep it.
+ *                       max_cat_entries = the largest category's entry count, < 2^21 (HOST value: the scans pack three counts);
+ *                       workspace: A * M * num_entries * 20 bytes, 8-byte aligned, else B200_ROI_EWORKSPACE.
+ * Bad sizes or null pointers: B200_ROI_EINVAL before any launch. */
+B200_API int b200_coco_rank(int num_pairs, const int* pair_det_begin_dev, const int* pair_entry_begin_dev, const double* det_score_dev,
+                            int* entry_det_out_dev, int* entry_rank_out_dev, double* entry_score_out_dev, b200_stream_t stream);
+B200_API int b200_coco_bbox_iou(int num_pairs, const int* pair_gt_begin_dev, const int* pair_entry_begin_dev, const long long* pair_iou_begin_dev,
+                                const int* entry_det_dev, const double* det_box_dev, const double* gt_box_dev, const int* gt_flags_dev,
+                                double* ious_out_dev, b200_stream_t stream);
+B200_API int b200_coco_oks(int num_pairs, const double* vars_host, const int* pair_gt_begin_dev, const int* pair_entry_begin_dev,
+                           const long long* pair_iou_begin_dev, const int* entry_det_dev, const double* det_kp_dev, const double* gt_kp_dev,
+                           const double* gt_box_dev, const double* gt_area_dev, double* ious_out_dev, b200_stream_t stream);
+B200_API int b200_coco_masks(unsigned* words_dev, long long num_words, int num_slots, const long long* slot_word_dev, const int* slot_hw_dev,
+                             int num_strings, const int* str_slot_dev, const long long* str_begin_dev, const unsigned char* str_bytes_dev,
+                             int num_counts, const int* cnt_slot_dev, const long long* cnt_begin_dev, const unsigned* counts_dev,
+                             int num_polys, int num_vertices, const int* poly_slot_dev, const int* vtx_begin_dev, const double* xy_dev,
+                             int num_masks, const int* mask_slot_begin_dev, long long* mask_area_out_dev, int* mask_range_out_dev,
+                             b200_stream_t stream);
+B200_API int b200_coco_segm_iou(int pair_begin, int num_pairs, const int* pair_gt_begin_dev, const int* pair_entry_begin_dev,
+                                const long long* pair_iou_begin_dev, const int* entry_det_dev, int det0, int gt0, int gt_mask0,
+                                const int* mask_slot_begin_dev, const long long* slot_word_dev, const int* slot_hw_dev,
+                                const unsigned* words_dev, const long long* mask_area_dev, const int* mask_range_dev, const int* gt_flags_dev,
+                                double* ious_out_dev, b200_stream_t stream);
+B200_API int b200_coco_match(int num_pairs, int num_thresholds, const double* iou_thrs_host, int num_areas, const double* area_rng_host,
+                             int max_gt, const int* pair_gt_begin_dev, const int* pair_entry_begin_dev, const long long* pair_iou_begin_dev,
+                             const int* pair_cat_dev, const int* entry_det_dev, const double* det_area_dev, const double* gt_area_dev,
+                             const int* gt_flags_dev, const double* ious_dev, int num_entries, unsigned* entry_flags_dev, int* npig_dev,
+                             b200_stream_t stream);
+B200_API int b200_coco_accumulate(int num_cats, int num_areas, int num_max_dets, int num_thresholds, int num_recall, const int* max_dets_host,
+                                  const int* cat_entry_begin_dev, const int* cat_pairs_dev, const int* order_dev, const int* entry_rank_dev,
+                                  const double* entry_score_dev, const unsigned* entry_flags_dev, int num_entries, int max_cat_entries,
+                                  const int* npig_dev,
+                                  const double* rec_thrs_dev, void* workspace, size_t workspace_bytes, double* precision_out_dev,
+                                  double* recall_out_dev, double* scores_out_dev, b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
