@@ -13,7 +13,7 @@ or, to make an unmodified checkout of the reference pick these up under ITS impo
 __version__ = "0.1.0"
 
 
-def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False):
+def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False, voc=False):
     """Register this package's op modules in sys.modules under the reference's import paths.
 
     After this, `from modeling.roi_xfrom.roi_align.functions.roi_align import RoIAlignFunction`
@@ -33,6 +33,9 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
     `keypoints=True` re-points the reference's `core.test.keypoint_results` (lib/core/test.py:850-866, called from
     im_detect_all) at the device keypoint extraction and OKS NMS (`core/test.py` here), reading the reference's `cfg`
     at call time; the reference's `core.test` must be importable for that.
+    `voc=True` re-points the reference's `datasets.voc_eval.voc_eval` (lib/datasets/voc_eval.py:86-223) and the copy of that name
+    bound in `datasets.voc_dataset_evaluator` at the device evaluation (`datasets/voc_eval.py` here), which reads and writes the
+    annotation cache in binary mode, so the reference's VOC evaluator runs on Python 3; both reference modules must be importable.
     """
     import importlib
     import sys
@@ -84,4 +87,9 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
         ref_test.keypoint_results = lambda cls_boxes, pred_heatmaps, ref_boxes: ours_kp(cls_boxes, pred_heatmaps, ref_boxes,
                                                                                          cfg=ref_test.cfg)
         installed.append("core.test.keypoint_results")
+    if voc:
+        ours_voc = importlib.import_module(__name__ + ".datasets.voc_eval").voc_eval
+        for name in ("datasets.voc_eval", "datasets.voc_dataset_evaluator"):      # the reference's modules
+            importlib.import_module(name).voc_eval = ours_voc
+            installed.append(name + ".voc_eval")
     return installed

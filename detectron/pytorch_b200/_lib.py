@@ -156,6 +156,8 @@ _SIGNATURES = {
     #  rec_thrs, workspace, workspace_bytes, precision, recall, scores, stream)
     "b200_coco_accumulate": (ctypes.c_int, [ctypes.c_int] * 5 + [ctypes.c_void_p] * 7 + [ctypes.c_int] * 2 + [ctypes.c_void_p] * 3 +
                              [ctypes.c_size_t] + [ctypes.c_void_p] * 3 + [_stream_t]),
+    # (num_dets, num_pairs, num_gt, ovthresh, pair_gt_begin, gt_box, gt_difficult, det_pair, det_box, workspace, outcome, stream)
+    "b200_voc_match": (ctypes.c_int, [ctypes.c_int] * 3 + [ctypes.c_double] + [ctypes.c_void_p] * 7 + [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

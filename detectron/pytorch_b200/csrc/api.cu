@@ -97,6 +97,8 @@ int coco_match(int, int, const double*, int, const double*, int, const int*, con
                const double*, const double*, const int*, const double*, int, unsigned*, int*, cudaStream_t);
 int coco_accumulate(int, int, int, int, int, const int*, const int*, const int*, const int*, const int*, const double*, const unsigned*, int,
                     int, const int*, const double*, void*, size_t, double*, double*, double*, cudaStream_t);
+int voc_match(int, int, int, double, const int*, const double*, const unsigned char*, const int*, const double*, int*, unsigned char*,
+              cudaStream_t);
 int mask_targets(const float*, const int*, const int*, int, int, const int*, int, const int*, int, const int*, const float*, int, int,
                  float*, int*, cudaStream_t);
 int keypoint_candidates(const float*, const float*, const int*, int, const int*, const int*, const int*, const int*, const int*, int, float,
@@ -769,6 +771,13 @@ int b200_coco_accumulate(int num_cats, int num_areas, int num_max_dets, int num_
     return coco_accumulate(num_cats, num_areas, num_max_dets, num_thresholds, num_recall, max_dets_host, cat_entry_begin_dev, cat_pairs_dev,
                            order_dev, entry_rank_dev, entry_score_dev, entry_flags_dev, num_entries, max_cat_entries, npig_dev, rec_thrs_dev, workspace,
                            workspace_bytes, precision_out_dev, recall_out_dev, scores_out_dev, (cudaStream_t)stream);
+}
+
+int b200_voc_match(int num_dets, int num_pairs, int num_gt, double ovthresh, const int* pair_gt_begin_dev, const double* gt_box_dev,
+                   const unsigned char* gt_difficult_dev, const int* det_pair_dev, const double* det_box_dev, int* workspace_dev,
+                   unsigned char* outcome_out_dev, b200_stream_t stream) {
+    return voc_match(num_dets, num_pairs, num_gt, ovthresh, pair_gt_begin_dev, gt_box_dev, gt_difficult_dev, det_pair_dev, det_box_dev,
+                     workspace_dev, outcome_out_dev, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -27,7 +27,8 @@ logger = logging.getLogger(__name__)
 
 class JsonDataset:
     """The parts of the reference's JsonDataset the evaluators read: name, classes, category_to_id_map and COCO, whose
-    `dataset` is the annotation-file dict and getImgIds() its image ids."""
+    `dataset` is the annotation-file dict and getImgIds() its image ids; devkit_path is a PASCAL VOC dataset's devkit directory
+    (the reference's catalog entry DEVKIT_DIR)."""
 
     class _Coco:
         def __init__(self, dataset):
@@ -39,8 +40,9 @@ class JsonDataset:
         def getCatIds(self):
             return [c["id"] for c in self.dataset.get("categories", [])]
 
-    def __init__(self, name, dataset):
+    def __init__(self, name, dataset, devkit_path=None):
         self.name = name
+        self.devkit_path = devkit_path
         self.COCO = JsonDataset._Coco(dataset)
         category_ids = sorted(self.COCO.getCatIds())
         names = {c["id"]: c["name"] for c in dataset.get("categories", [])}
@@ -52,12 +54,13 @@ class JsonDataset:
         self.contiguous_category_id_to_json_id = {v: k for k, v in self.json_category_id_to_contiguous_id.items()}
 
 
-def load_json_dataset(name, annotation_file_or_dict):
-    """A JsonDataset from a COCO annotation file (path) or its already-loaded dict, without pycocotools."""
+def load_json_dataset(name, annotation_file_or_dict, devkit_path=None):
+    """A JsonDataset from a COCO annotation file (path) or its already-loaded dict, without pycocotools.  devkit_path: the
+    VOCdevkit directory that voc_dataset_evaluator reads a `voc_*` dataset's image set and annotations from."""
     if isinstance(annotation_file_or_dict, dict):
-        return JsonDataset(name, annotation_file_or_dict)
+        return JsonDataset(name, annotation_file_or_dict, devkit_path)
     with open(annotation_file_or_dict) as f:
-        return JsonDataset(name, json.load(f))
+        return JsonDataset(name, json.load(f), devkit_path)
 
 
 def _image_ids(json_dataset):

@@ -1141,3 +1141,19 @@ def coco_accumulate_raw(max_dets, cat_entry_begin, cat_pairs, order, entry_rank,
                                                     ws_bytes, precision.data_ptr(), recall.data_ptr(), scores.data_ptr(), _stream()),
                    "b200_coco_accumulate")
     return precision, recall, scores
+
+
+# ------------------------------------------------------------------------------------------------
+# PASCAL VOC evaluation (the reference's voc_eval loop; datasets/voc_eval.py drives it)
+# ------------------------------------------------------------------------------------------------
+def voc_match_raw(pair_gt_begin, gt_box, gt_difficult, det_pair, det_box, ovthresh):
+    """tp / fp / neither of every detection (uint8 1 / 0 / 2), detections in rank order within each class.  pair_gt_begin
+    (P + 1) int32, gt_box (G, 4) float64, gt_difficult (G,) uint8, det_pair (D,) int32, det_box (D, 4) float64, all on one device."""
+    D, G, dev = det_pair.numel(), gt_difficult.numel(), det_pair.device
+    outcome = torch.empty((max(D, 1),), dtype=torch.uint8, device=dev)
+    ws = torch.empty((max(G, 1),), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().b200_voc_match(D, pair_gt_begin.numel() - 1, G, float(ovthresh), pair_gt_begin.data_ptr(), gt_box.data_ptr(),
+                                              gt_difficult.data_ptr(), det_pair.data_ptr(), det_box.data_ptr(), ws.data_ptr(),
+                                              outcome.data_ptr(), _stream()), "b200_voc_match")
+    return outcome[:D]

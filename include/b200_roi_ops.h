@@ -524,6 +524,22 @@ B200_API int b200_coco_accumulate(int num_cats, int num_areas, int num_max_dets,
                                   const double* rec_thrs_dev, void* workspace, size_t workspace_bytes, double* precision_out_dev,
                                   double* recall_out_dev, double* scores_out_dev, b200_stream_t stream);
 
+/* ---- PASCAL VOC evaluation (lib/datasets/voc_eval.py:86-223, the per-detection loop) ------------------------------------------
+ * b200_voc_match marks each detection a true positive, a false positive or neither, as the reference's loop does.
+ * Detections: num_dets rows of det_box_dev (float64 x1, y1, x2, y2, 16-byte aligned) and det_pair_dev (int32, in 0 .. num_pairs - 1,
+ *   the detection's (class, image) pair).  Within one class the rows are in rank order (the caller's sort), so a row's index is its rank.
+ * Ground truth: pair p owns rows pair_gt_begin_dev[p] .. [p + 1] - 1 (num_pairs + 1 non-decreasing int32, last = num_gt) of gt_box_dev
+ *   (float64 x1, y1, x2, y2, 16-byte aligned) and gt_difficult_dev (uint8, non-zero = difficult).
+ * Overlap in float64 without contraction: iw = max(min(x2) - max(x1) + 1, 0), ih likewise, inters = iw * ih,
+ *   uni = (bw * bh + gw * gh) - inters, ov = inters / uni; jmax = numpy's argmax (first maximum; a NaN wins and fails the test).
+ * outcome_out_dev (num_dets uint8): 1 = tp (ov > ovthresh, jmax not difficult, the lowest-ranked such detection of jmax), 2 = neither
+ *   (ov > ovthresh and jmax difficult), 0 = fp (every other case, no ground truth of the pair included).
+ * workspace_dev: num_gt ints (overwritten).
+ * Bad sizes or null pointers: B200_ROI_EINVAL before any launch. */
+B200_API int b200_voc_match(int num_dets, int num_pairs, int num_gt, double ovthresh, const int* pair_gt_begin_dev, const double* gt_box_dev,
+                            const unsigned char* gt_difficult_dev, const int* det_pair_dev, const double* det_box_dev, int* workspace_dev,
+                            unsigned char* outcome_out_dev, b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
