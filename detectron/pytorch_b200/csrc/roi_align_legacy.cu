@@ -6,6 +6,15 @@
 // ROIAlignBackward :94-143.  The mixed fp32/fp64 rounding recipe below is the one nvcc emits for
 // the reference (see oracle/roi_ops_oracle.c, "RoIAlign, legacy variant").
 //
+// One departure from the reference: maps with a single row or column.  The reference takes the first tap at
+// hstart = min(floor(h), H - 2) and the second at hstart + 1, so on H = 1 every in-map sample reads (forward) and
+// atomically adds to (backward) row -1 -- before the tensor, or in the previous channel plane -- and likewise column -1
+// on W = 1.  Small images give such maps at the top pyramid levels, so here the first tap is clamped to
+// max(min(floor(h), H - 2), 0) and the second to min(hstart + 1, H - 1) (same for w): on a one-row map both taps are
+// row 0, the convention of the Caffe2-style RoIAlign on its clamped last row.  The weights are left as computed, so
+// the forward gives the row's value and the backward puts the whole gradient on row 0.  For H, W >= 2 the clamps
+// change nothing and the results stay bit-identical to the reference.
+//
 // Layout choice: one CTA per (RoI, channel slab); the P x P lattice geometry (cell index + the two
 // ratios) is computed once per CTA into shared memory instead of once per output element.
 #include "common.cuh"
@@ -18,7 +27,7 @@ constexpr int kLegTabMax = 1024;   // lattice points cached per CTA (P*P); large
 struct __align__(16) LegPoint {
     int   off;       // hstart * W + wstart, or -1 if the point is outside the map
     float hr, wr;    // h_ratio, w_ratio
-    int   pad;
+    int   taps;      // bit 0: the right taps are column wstart + 1 (else wstart); bit 1: the lower taps are row hstart + 1
 };
 
 __device__ __forceinline__ LegPoint legacy_point(const float* __restrict__ roi, float scale, int PH, int PW,
@@ -31,14 +40,14 @@ __device__ __forceinline__ LegPoint legacy_point(const float* __restrict__ roi, 
     const float h = __fmaf_rn((float)ph, bh, sh);
     const float w = __fmaf_rn((float)pw, bw, sw);
     LegPoint p;
-    p.pad = 0;
     if (h < 0 || h >= (float)H || w < 0 || w >= (float)W) {
-        p.off = -1; p.hr = 0.f; p.wr = 0.f;
+        p.off = -1; p.hr = 0.f; p.wr = 0.f; p.taps = 0;
         return p;
     }
-    const int hs = (int)fminf(floorf(h), (float)(H - 2));
-    const int ws = (int)fminf(floorf(w), (float)(W - 2));
+    const int hs = (int)fmaxf(fminf(floorf(h), (float)(H - 2)), 0.f);   // 0 on a one-row map (the reference: -1)
+    const int ws = (int)fmaxf(fminf(floorf(w), (float)(W - 2)), 0.f);
     p.off = hs * W + ws;
+    p.taps = (ws + 1 <= W - 1 ? 1 : 0) | (hs + 1 <= H - 1 ? 2 : 0);
     p.hr = __fsub_rn(h, (float)hs);
     p.wr = __fsub_rn(w, (float)ws);
     return p;
@@ -72,8 +81,9 @@ roi_align_legacy_kernel(const float* __restrict__ in, const float* __restrict__ 
             continue;
         }
         const size_t ul = (size_t)(img_start + (long long)c * H * W + p.off);
+        const size_t ur = ul + (p.taps & 1), dl = ul + (p.taps & 2 ? W : 0), dr = dl + (p.taps & 1);
         if (!BACKWARD) {
-            const float vul = __ldg(in + ul), vur = __ldg(in + ul + 1), vdl = __ldg(in + ul + W), vdr = __ldg(in + ul + W + 1);
+            const float vul = __ldg(in + ul), vur = __ldg(in + ur), vdl = __ldg(in + dl), vdr = __ldg(in + dr);
             const double omh = __dsub_rn(1.0, (double)p.hr), omw = __dsub_rn(1.0, (double)p.wr);
             const double t_ur = __dmul_rn((double)p.wr, __dmul_rn(omh, (double)vur));
             double acc = __fma_rn(__dmul_rn((double)vul, omh), omw, t_ur);
@@ -86,9 +96,9 @@ roi_align_legacy_kernel(const float* __restrict__ in, const float* __restrict__ 
             const float omw = __fsub_rn(1.f, p.wr);
             const float ghr = __fmul_rn(p.hr, g);
             atomicAdd(out + ul, (float)__dmul_rn(gomh, (double)omw));
-            atomicAdd(out + ul + 1, (float)__dmul_rn(gomh, (double)p.wr));
-            atomicAdd(out + ul + W, __fmul_rn(omw, ghr));
-            atomicAdd(out + ul + W + 1, __fmul_rn(p.wr, ghr));
+            atomicAdd(out + ur, (float)__dmul_rn(gomh, (double)p.wr));
+            atomicAdd(out + dl, __fmul_rn(omw, ghr));
+            atomicAdd(out + dr, __fmul_rn(p.wr, ghr));
         }
     }
 }

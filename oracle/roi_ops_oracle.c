@@ -246,6 +246,11 @@ ORACLE_API long oracle_roi_align_touched_cells(const float* rois, int N, int H, 
  *   bin     = (float)((double)roi_w / (double)(P - 1))
  *   h       = FFMA((float)ph, bin_h, start_h)
  *   hstart  = (int)fminf(floorf(h), H-2);   h_ratio = FADD(h, -(float)hstart)   (float)
+ *             taps at rows hstart, hstart + 1 and columns wstart, wstart + 1
+ * DEPARTURE from the reference (the only one): on a one-row map (H = 1) the reference's hstart is -1, so it reads
+ *   and scatters into row -1, outside the channel plane (W = 1: column -1).  Here, as in roi_align_legacy.cu,
+ *   hstart = max(min(floor(h), H-2), 0) and the second tap row is min(hstart + 1, H - 1) (same for columns), so on a
+ *   one-row map both taps are row 0; the weights are unchanged.  For H, W >= 2 this is the reference's arithmetic.
  *   fwd     = (float)( DADD( DFMA(omw, (double)FMUL(hr, dl),
  *                               DFMA(DMUL((double)ul, omh), omw, DMUL((double)wr, DMUL(omh,(double)ur)))),
  *                            (double)FMUL(wr, FMUL(hr, dr)) ) )
@@ -254,7 +259,7 @@ ORACLE_API long oracle_roi_align_touched_cells(const float* rois, int N, int H, 
  *             dl += (1.f - wr) * (hr * g),  dr += wr * (hr * g)
  * ------------------------------------------------------------------------------------------ */
 static inline int legacy_geometry(const float* roi, float scale, int PH, int PW, int H, int W, int ph, int pw,
-                                  float* h_ratio, float* w_ratio, int* hstart, int* wstart) {
+                                  float* h_ratio, float* w_ratio, int* hstart, int* wstart, int* dh, int* dw) {
     float sw = roi[1] * scale, sh = roi[2] * scale;
     float rw = fmaxf(fmaf(roi[3], scale, -sw) + 1.f, 0.f);
     float rh = fmaxf(fmaf(roi[4], scale, -sh) + 1.f, 0.f);
@@ -262,8 +267,10 @@ static inline int legacy_geometry(const float* roi, float scale, int PH, int PW,
     float bw = (float)((double)rw / ((double)PW - 1.));
     float h = fmaf((float)ph, bh, sh);
     float w = fmaf((float)pw, bw, sw);
-    *hstart = (int)fminf(floorf(h), (float)(H - 2));
-    *wstart = (int)fminf(floorf(w), (float)(W - 2));
+    *hstart = (int)fmaxf(fminf(floorf(h), (float)(H - 2)), 0.f);
+    *wstart = (int)fmaxf(fminf(floorf(w), (float)(W - 2)), 0.f);
+    *dh = (*hstart + 1 <= H - 1) ? W : 0;     /* offset of the lower taps from the upper ones */
+    *dw = (*wstart + 1 <= W - 1) ? 1 : 0;
     if (h < 0 || h >= (float)H || w < 0 || w >= (float)W) return 0;
     *h_ratio = h - (float)(*hstart);
     *w_ratio = w - (float)(*wstart);
@@ -280,11 +287,11 @@ ORACLE_API void oracle_roi_align_legacy_forward(const float* bottom, const float
         for (int c = 0; c < C; ++c)
             for (int ph = 0; ph < PH; ++ph)
                 for (int pw = 0; pw < PW; ++pw) {
-                    float hr, wr; int hs, ws;
+                    float hr, wr; int hs, ws, dh, dw;
                     float* o = top + (((size_t)n * C + c) * PH + ph) * PW + pw;
-                    if (!legacy_geometry(rois + 5 * n, scale, PH, PW, H, W, ph, pw, &hr, &wr, &hs, &ws)) { *o = 0.f; continue; }
+                    if (!legacy_geometry(rois + 5 * n, scale, PH, PW, H, W, ph, pw, &hr, &wr, &hs, &ws, &dh, &dw)) { *o = 0.f; continue; }
                     const float* p = bottom + img_start + ((size_t)c * H + hs) * W + ws;
-                    float ul = p[0], ur = p[1], dl = p[W], dr = p[W + 1];
+                    float ul = p[0], ur = p[dw], dl = p[dh], dr = p[dh + dw];
                     double omh = 1.0 - (double)hr, omw = 1.0 - (double)wr;
                     double t_ur = (double)wr * (omh * (double)ur);
                     double acc = fma((double)ul * omh, omw, t_ur);
@@ -306,8 +313,8 @@ ORACLE_API void oracle_roi_align_legacy_backward(const float* top_diff, const fl
             int img_start = (int)(rois[5 * n] * (float)C * (float)H * (float)W);
             for (int ph = 0; ph < PH; ++ph)
                 for (int pw = 0; pw < PW; ++pw) {
-                    float hr, wr; int hs, ws;
-                    if (!legacy_geometry(rois + 5 * n, scale, PH, PW, H, W, ph, pw, &hr, &wr, &hs, &ws)) continue;
+                    float hr, wr; int hs, ws, dh, dw;
+                    if (!legacy_geometry(rois + 5 * n, scale, PH, PW, H, W, ph, pw, &hr, &wr, &hs, &ws, &dh, &dw)) continue;
                     float g = top_diff[(((size_t)n * C + c) * PH + ph) * PW + pw];
                     size_t ul = (size_t)img_start + ((size_t)c * H + hs) * W + ws;
                     double gomh = (double)g * (1.0 - (double)hr);
@@ -317,8 +324,8 @@ ORACLE_API void oracle_roi_align_legacy_backward(const float* top_diff, const fl
                     float ghr = hr * g;
                     float g_dl = omw * ghr;
                     float g_dr = wr * ghr;
-                    if (acc64) { dacc[ul] += g_ul; dacc[ul + 1] += g_ur; dacc[ul + W] += g_dl; dacc[ul + W + 1] += g_dr; }
-                    else { bottom_diff[ul] += g_ul; bottom_diff[ul + 1] += g_ur; bottom_diff[ul + W] += g_dl; bottom_diff[ul + W + 1] += g_dr; }
+                    if (acc64) { dacc[ul] += g_ul; dacc[ul + dw] += g_ur; dacc[ul + dh] += g_dl; dacc[ul + dh + dw] += g_dr; }
+                    else { bottom_diff[ul] += g_ul; bottom_diff[ul + dw] += g_ur; bottom_diff[ul + dh] += g_dl; bottom_diff[ul + dh + dw] += g_dr; }
                 }
         }
     if (acc64) { for (size_t i = 0; i < total; ++i) bottom_diff[i] = (float)dacc[i]; free(dacc); }
