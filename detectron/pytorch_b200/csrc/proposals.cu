@@ -43,19 +43,23 @@ proposal_decode_kernel(const float* __restrict__ deltas,        // (4A, H, W) of
     const float ctr_x = __fadd_rn(x1, __fmul_rn(.5f, widths)), ctr_y = __fadd_rn(y1, __fmul_rn(.5f, heights));
     const float pcx = __fadd_rn(__fmul_rn(dx, widths), ctr_x), pcy = __fadd_rn(__fmul_rn(dy, heights), ctr_y);
     const double kClip = 4.135166556742356;                      // log(1000 / 16)
-    const double pw = __dmul_rn(exp(fmin((double)dw, kClip)), (double)widths);
-    const double ph = __dmul_rn(exp(fmin((double)dh, kClip)), (double)heights);
+    // np.minimum(d, clip): a NaN delta stays NaN (fmin would return the clip)
+    const double dwc = (double)dw > kClip ? kClip : (double)dw, dhc = (double)dh > kClip ? kClip : (double)dh;
+    const double pw = __dmul_rn(exp(dwc), (double)widths);
+    const double ph = __dmul_rn(exp(dhc), (double)heights);
     const double hw = __dmul_rn(.5, pw), hh = __dmul_rn(.5, ph);
     float bx1 = (float)__dsub_rn((double)pcx, hw), by1 = (float)__dsub_rn((double)pcy, hh);
     float bx2 = (float)__dsub_rn(__dadd_rn((double)pcx, hw), 1.0), by2 = (float)__dsub_rn(__dadd_rn((double)pcy, hh), 1.0);
 
+    // NaN survives the reference's np.minimum / np.maximum clip and fails _filter_boxes; fminf / fmaxf would clip it, so test it first
+    const bool finite_box = !(bx1 != bx1 || by1 != by1 || bx2 != bx2 || by2 != by2);
     const float wmax = __fsub_rn(im_w, 1.f), hmax = __fsub_rn(im_h, 1.f);
     bx1 = fmaxf(fminf(bx1, wmax), 0.f); by1 = fmaxf(fminf(by1, hmax), 0.f);
     bx2 = fmaxf(fminf(bx2, wmax), 0.f); by2 = fmaxf(fminf(by2, hmax), 0.f);
 
     const float ws = __fadd_rn(__fsub_rn(bx2, bx1), 1.f), hs = __fadd_rn(__fsub_rn(by2, by1), 1.f);
     const float xc = __fadd_rn(bx1, __fmul_rn(ws, .5f)), yc = __fadd_rn(by1, __fmul_rn(hs, .5f));
-    const bool ok = ws >= min_size && hs >= min_size && xc < im_w && yc < im_h;
+    const bool ok = finite_box && ws >= min_size && hs >= min_size && xc < im_w && yc < im_h;
     float* d = dets + (size_t)t * 5;
     d[0] = ok ? bx1 : 0.f; d[1] = ok ? by1 : 0.f; d[2] = ok ? bx2 : -1.f; d[3] = ok ? by2 : -1.f; d[4] = scores[t];
     valid[t] = ok ? 1 : 0;

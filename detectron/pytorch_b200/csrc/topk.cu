@@ -7,9 +7,11 @@
 //     problem-parallel AND chunk-parallel: a CTA per 16 K scores, shared-memory histogram, one global atomic per non-empty bin;
 //     from the second pass on every CTA re-derives the digits selected so far from the global histograms -- no host read, no
 //     grid barrier, the stream order of the four launches is the only synchronisation),
-//   1 collect + sort launch (a CTA per problem): scores above the k-th key and the first ties in memory order are compacted
-//     into shared memory as (key << 32 | ~index) words and sorted there (bitonic, descending): equal scores come out in
-//     ascending (h, w, a) index, deterministically (the reference's tie order is unspecified).
+//   1 collect + sort launch (a CTA per problem): the map is walked in (H, W, A) order; scores above the k-th key and the
+//     first ties in that order are compacted into shared memory as (key << 32 | ~index) words and sorted there (bitonic,
+//     descending).  The result is exactly np.argsort(-x_hwa, kind="stable")[:k]: equal scores -- also those that straddle
+//     the cut -- are taken and returned in ascending (h, w, a) index.  NaN ranks below every number (numpy sorts it last),
+//     NaNs among themselves by index, and -0.0 ties with +0.0 (one key each, shared by every pass).
 // The maps are read where they lie, in (A, H, W) layout; the returned indices enumerate (H, W, A) like the reference's
 // `scores.transpose((1, 2, 0)).reshape((-1, 1))`, so no permuted copy of the scores is made.
 #include "common.cuh"
@@ -25,6 +27,7 @@ constexpr int kHistThreads = 256;
 constexpr int kChunk = 16384;                 // scores per histogram CTA
 constexpr int kBins = 2048;
 constexpr int kSortThreads = 1024;
+constexpr int kCollectUnroll = 4;              // chunks of kSortThreads scores per collect round
 
 typedef unsigned long long u64;
 
@@ -36,8 +39,10 @@ struct TopkBatch {
     int chunk_off[kTopkMaxProblems + 1];      // first histogram CTA
 };
 
+// order-preserving key; every NaN gets 0 (below -inf's 0x007fffff: the stable-argsort rank of NaN), -0.0 the key of +0.0
 __device__ __forceinline__ unsigned ordered_key(float x) {
-    const unsigned b = __float_as_uint(x);
+    if (x != x) return 0u;
+    const unsigned b = __float_as_uint(x == 0.f ? 0.f : x);
     return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 __device__ __forceinline__ float key_to_float(unsigned k) {
@@ -143,29 +148,39 @@ topk_collect_sort_kernel(const __grid_constant__ TopkBatch tb, const int* __rest
     if (t == 0) { s_count = 0; s_ties = 0; }
     __syncthreads();
     const float* src = tb.src[p];
-    for (int base = 0; base < n; base += kSortThreads) {
-        const int m = base + t;
-        unsigned key = 0u;
-        bool gt = false, eq = false;
-        if (m < n) { key = ordered_key(__ldg(src + m)); gt = key > T; eq = key == T; }
-        // ties are admitted in memory order (deterministic): rank of this tie among all ties seen so far.  Ties are rare: the
-        // block-wide rank is only worked out for a chunk that holds one
-        bool take = gt;
-        if (__syncthreads_or(eq ? 1 : 0)) {
-            const unsigned em = __ballot_sync(0xffffffffu, eq);
-            if (lane == 0) s_warp[warp] = __popc(em);
-            __syncthreads();
-            int rank = s_ties + __popc(em & ((1u << lane) - 1u));
-            for (int w = 0; w < warp; ++w) rank += s_warp[w];
-            take = gt || (eq && rank < ties_wanted);
-            __syncthreads();
-            if (t == 0) { int tot = 0; for (int w = 0; w < 32; ++w) tot += s_warp[w]; s_ties += tot; }
+    for (int base = 0; base < n; base += kSortThreads * kCollectUnroll) {
+        unsigned keys[kCollectUnroll];
+#pragma unroll
+        for (int j = 0; j < kCollectUnroll; ++j) {             // every load of the round first: several in flight per thread
+            const int e = base + j * kSortThreads + t;         // index in (H, W, A) enumeration
+            keys[j] = 0u;
+            if (e < n) {
+                const int cell = e / A, a = e - cell * A;
+                keys[j] = ordered_key(__ldg(src + (size_t)a * HW + cell));
+            }
         }
-        if (take) {
-            const int a = m / HW, cell = m - a * HW;
-            const unsigned e = (unsigned)cell * (unsigned)A + (unsigned)a;                // index in (H, W, A) enumeration
-            const int pos = atomicAdd(&s_count, 1);
-            if (pos < m2) s_items[pos] = ((u64)key << 32) | (u64)(0xffffffffu - e);
+#pragma unroll
+        for (int j = 0; j < kCollectUnroll; ++j) {
+            const int e = base + j * kSortThreads + t;
+            const unsigned key = keys[j];
+            const bool gt = e < n && key > T, eq = e < n && key == T;
+            // ties are admitted in (H, W, A) order: rank of this tie among all ties seen so far.  The block-wide rank is only
+            // worked out for a chunk that holds one
+            bool take = gt;
+            if (__syncthreads_or(eq ? 1 : 0)) {
+                const unsigned em = __ballot_sync(0xffffffffu, eq);
+                if (lane == 0) s_warp[warp] = __popc(em);
+                __syncthreads();
+                int rank = s_ties + __popc(em & ((1u << lane) - 1u));
+                for (int w = 0; w < warp; ++w) rank += s_warp[w];
+                take = gt || (eq && rank < ties_wanted);
+                __syncthreads();
+                if (t == 0) { int tot = 0; for (int w = 0; w < 32; ++w) tot += s_warp[w]; s_ties += tot; }
+            }
+            if (take) {
+                const int pos = atomicAdd(&s_count, 1);
+                if (pos < m2) s_items[pos] = ((u64)key << 32) | (u64)(0xffffffffu - (unsigned)e);
+            }
         }
     }
     __syncthreads();

@@ -9,16 +9,20 @@ thread, and the caller copies the RoIs back.  Here everything up to the final re
     b200_topk_batched (radix select + in-CTA sort over every (level, image) score map of the step, read in place)  ->
     b200_proposal_decode (anchor rebuild + bbox_transform + clip + filter, one kernel)  ->  b200_nms_batched (bitmask +
     on-device scan)  ->  ONE D2H of the kept rows per image
-(torch.topk / torch.sort remain only as the fallback for k > 16384 candidates per map.)
+(torch.sort remains only as the fallback for k > 16384 candidates per map.)
 
 Configuration: the reference reads `cfg[TRAIN|TEST].RPN_{PRE,POST}_NMS_TOP_N, RPN_NMS_THRESH, RPN_MIN_SIZE` from its
 global config at call time; pass that object as `cfg=` to do the same, or give the four values per mode as keyword
 arguments (`train=dict(...)`, `test=dict(...)`); defaults are the reference's (lib/core/config.py:127-141, 200-214).
 
 Documented differences (see oracle/proposals.py): the reference leaves the order of EQUAL scores unspecified (its
-argpartition/argsort); here they come out in ascending (h, w, a) index (which of several scores equal to the k-th survive the
-cut is decided in memory order), and NMS suppresses at IoU > thresh with the CUDA kernel's rounding (the reference's
-host NMS uses >=); results on the golden vectors are identical.  All images of a call -- and, through
+argpartition/argsort); here the pre-NMS candidates are exactly np.argsort(-scores, kind="stable")[:pre_nms_topN] of the
+(H, W, A)-flattened map, on the device top-k and on the torch.sort fallback alike: equal scores -- also those that straddle the
+cut -- are taken in ascending (h, w, a) index, NaN scores rank below every number (as numpy sorts them) and -0.0 ties with
++0.0.  A candidate whose decoded box has a NaN coordinate is dropped, as the reference's _filter_boxes drops it.  NaN scores
+that do reach NMS (only when pre_nms_topN exceeds the number of finite scores) stay where the sort put them, last; the
+reference's Cython NMS re-sorts and puts them first.  NMS suppresses at IoU > thresh with the CUDA kernel's rounding (the
+reference's host NMS uses >=); results on the golden vectors are identical.  All images of a call -- and, through
 generate_proposals_batched, all FPN levels of a step -- share ONE batched NMS launch pair and ONE host read.
 """
 import numpy as np
@@ -95,10 +99,10 @@ class GenerateProposalsOp(nn.Module):
             order, top_scores = ranked
         else:                                                                       # library fallback: k beyond the device top-k's 16384
             flat = scores.permute(1, 2, 0).reshape(-1)                              # (H, W, A) order, as the reference enumerates anchors
-            if pre_nms_topN <= 0 or pre_nms_topN >= total:
-                top_scores, order = torch.sort(flat, descending=True, stable=True)
-            else:
-                top_scores, order = torch.topk(flat, int(pre_nms_topN), largest=True, sorted=True)
+            order = _stable_descending_order(flat)
+            if 0 < pre_nms_topN < total:
+                order = order[:int(pre_nms_topN)]
+            top_scores = flat[order]
         k = int(order.numel())
         dets = torch.empty((k, 5), dtype=torch.float32, device=dev)
         valid = torch.empty((k,), dtype=torch.int32, device=dev)
@@ -114,6 +118,15 @@ class GenerateProposalsOp(nn.Module):
             keep, num = ops.nms_raw(dets, float(nms_thresh))
             return dets, valid, keep, num
         return dets, valid, None, None
+
+
+def _stable_descending_order(flat):
+    """np.argsort(-flat, kind="stable") on the device: NaN after every number (torch.sort puts it first), NaNs and equal
+    scores in ascending index, -0.0 equal to +0.0 -- the rule b200_topk_batched follows."""
+    nan = torch.isnan(flat)
+    key = torch.where(nan, torch.full_like(flat, float("-inf")), flat) + 0.0    # + 0.0 turns -0.0 into +0.0
+    order = torch.sort(key, descending=True, stable=True).indices
+    return order[torch.sort(nan[order].to(torch.uint8), stable=True).indices]  # NaNs to the end, keeping their index order
 
 
 def generate_proposals_batched(op_list, cls_probs, bbox_preds, im_info):

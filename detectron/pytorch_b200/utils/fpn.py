@@ -14,5 +14,10 @@ def map_rois_to_fpn_levels(rois, k_min, k_max, canonical_scale=224, canonical_le
     areas = w * h
     areas = torch.where(areas < 0, torch.zeros_like(areas), areas)
     s = torch.sqrt(areas)
-    lvls = torch.floor(canonical_level + torch.log2(s / canonical_scale + 1e-6))
+    # At a level boundary floor() turns a last-bit difference into a level, so both roundings are pinned to numpy's: a true
+    # float32 division by a tensor (a Python-number divisor may be applied as a multiplication by its rounded reciprocal on
+    # CUDA) and log2 rounded once from float64 (CUDA's float32 log2 is not correctly rounded).  Without this, 161 of 182 232
+    # boxes within 64 ulps of a boundary got another level than the reference's numpy on an H100.
+    y = torch.div(s, torch.full((), float(canonical_scale), dtype=s.dtype, device=s.device)) + 1e-6
+    lvls = torch.floor(canonical_level + torch.log2(y.double()).to(s.dtype))
     return torch.clamp(lvls, k_min, k_max)

@@ -11,7 +11,7 @@ Follows, step for step and in float32 like the reference (whose arrays come from
 Two places where the reference is not a function of its inputs are made deterministic here and documented as such:
   * top-k: the reference orders the pre-NMS candidates with np.argpartition + np.argsort (unstable: equal scores come
     out in an unspecified order); this restatement uses a stable descending sort, i.e. ties keep ascending anchor
-    index in (H, W, A) order -- the order torch.topk / torch.sort(stable=True) can reproduce;
+    index in (H, W, A) order and NaN scores come last -- the rule b200_topk_batched and the torch.sort fallback follow;
   * NMS: the reference calls utils.boxes.nms -> cython_nms.nms on the host (suppress when IoU >= thresh).  The device
     path uses the CUDA kernel's semantics (IoU > thresh, the SASS rounding recipe); `nms="cuda"` (default) selects
     oracle_nms_cuda, `nms="cython"` the restatement of the Cython routine, so both can be compared.

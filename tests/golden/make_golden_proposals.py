@@ -22,6 +22,7 @@ import tempfile
 import types
 
 import numpy as np
+import numpy.ma  # noqa: F401  (imported before import_reference aliases np.bool, which numpy.ma's own import trips over)
 import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -104,6 +105,26 @@ def main():
         out[name + "/params"] = np.asarray([stride, pre, post, thresh, min_size], dtype=np.float64)
         out[name + "/rois"] = rois.astype(np.float32); out[name + "/probs"] = probs.astype(np.float32)
         print(name, "A =", A, "rois", rois.shape)
+    # cases from tests/proposal_cases.py on which the reference is deterministic: NaN / inf deltas and NaN scores kept out of the
+    # top k, dw / dh at the float32 neighbours of BBOX_XFORM_CLIP, and an FPN P2 level with unique sigmoid-shaped scores (the
+    # tests regenerate their inputs from the case seed: only a sha256 of them is stored)
+    from tests import proposal_cases as PC
+    for name in PC.GOLDEN:
+        scores, deltas, im_info, anchors, stride, pre, post, thresh, min_size, training = PC.golden_inputs(name)
+        key = "TRAIN" if training else "TEST"
+        cfg[key].RPN_PRE_NMS_TOP_N = pre; cfg[key].RPN_POST_NMS_TOP_N = post
+        cfg[key].RPN_NMS_THRESH = thresh; cfg[key].RPN_MIN_SIZE = min_size
+        op = gp.GenerateProposalsOp(anchors, 1.0 / stride)
+        op.train(training)
+        import warnings
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")                                          # NaN / inf arithmetic
+            rois, probs = op(torch.from_numpy(scores.copy()), torch.from_numpy(deltas.copy()), torch.from_numpy(im_info.copy()))
+        out[name + "/input_sha256"] = np.array(PC.sha256(scores, deltas))
+        out[name + "/im_info"] = im_info; out[name + "/anchors"] = anchors
+        out[name + "/params"] = np.asarray([stride, pre, post, thresh, min_size], dtype=np.float64)
+        out[name + "/rois"] = rois.astype(np.float32); out[name + "/probs"] = probs.astype(np.float32)
+        print(name, "A =", anchors.shape[0], "rois", rois.shape)
     # the live CPU NMS of the reference on the NMS oracle's own cases (pins oracle_nms_cython)
     sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
     from detectron.pytorch_b200 import synthetic as S

@@ -8,6 +8,7 @@ import pytest
 from detectron.pytorch_b200 import synthetic as S
 from oracle import cpu as O
 from oracle import proposals as P
+from tests import proposal_cases as PC
 
 GOLD = np.load(os.path.join(os.path.dirname(__file__), "golden", "proposals.npz"))
 CASES = sorted({k.split("/")[0] for k in GOLD.files if k.endswith("/params")})
@@ -15,6 +16,9 @@ CASES = sorted({k.split("/")[0] for k in GOLD.files if k.endswith("/params")})
 
 def case(name):
     g = {k.split("/", 1)[1]: GOLD[k] for k in GOLD.files if k.startswith(name + "/")}
+    if "scores" not in g:                                        # inputs regenerated from the case seed, pinned by their digest
+        g["scores"], g["deltas"] = PC.golden_inputs(name)[:2]
+        assert PC.sha256(g["scores"], g["deltas"]) == str(g["input_sha256"])
     stride, pre, post, thresh, min_size = g["params"]
     return g, float(stride), int(pre), int(post), float(thresh), float(min_size)
 
@@ -36,6 +40,26 @@ def test_cuda_nms_semantics_give_the_same_proposals_on_these_inputs(name):
     rois, probs = P.generate_proposals(g["scores"], g["deltas"], g["im_info"], g["anchors"], stride, pre, post, thresh,
                                        min_size, nms="cuda")
     assert np.array_equal(rois, g["rois"]) and np.array_equal(probs, g["probs"])
+
+
+def test_new_golden_cases_reach_the_edges_they_are_for():
+    """nonfinite: NaN scores exist but none is selected, NaN- and inf-delta candidates are among the pre-NMS top k, and the
+    reference dropped every NaN box; clip_edges: dw / dh at all three float32 neighbours of the clip reach the decode."""
+    g, stride, pre, post, thresh, min_size = case("nonfinite")
+    for i in range(2):
+        s = g["scores"][i].transpose(1, 2, 0).reshape(-1)
+        d = g["deltas"][i].reshape(-1, 4, s.size // 3).transpose(2, 0, 1).reshape(-1, 4)
+        top = PC.stable_topk(g["scores"][i], pre)
+        assert np.isnan(s).any() and not np.isnan(s[top]).any()
+        for c in range(4):
+            assert np.isnan(d[top, c]).any()
+        assert np.isinf(d[top]).any()
+    assert not np.isnan(g["rois"]).any() and not np.isnan(g["probs"]).any()
+    g, stride, pre, post, thresh, min_size = case("clip_edges")
+    d = g["deltas"][0].reshape(-1, 4, g["scores"][0][0].size).transpose(2, 0, 1).reshape(-1, 4)
+    top = PC.stable_topk(g["scores"][0], pre)
+    for v in PC.CLIP_NEIGHBOURS:
+        assert (d[top, 2] == v).any() and (d[top, 3] == v).any()
 
 
 @pytest.mark.parametrize("n", [1, 65, 1000, 3000])
