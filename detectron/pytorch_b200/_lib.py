@@ -158,6 +158,11 @@ _SIGNATURES = {
                              [ctypes.c_size_t] + [ctypes.c_void_p] * 3 + [_stream_t]),
     # (num_dets, num_pairs, num_gt, ovthresh, pair_gt_begin, gt_box, gt_difficult, det_pair, det_box, workspace, outcome, stream)
     "b200_voc_match": (ctypes.c_int, [ctypes.c_int] * 3 + [ctypes.c_double] + [ctypes.c_void_p] * 7 + [_stream_t]),
+    "b200_box_proposal_match_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int] * 4),
+    # (num_images, num_props, num_gt, num_areas, num_limits, num_thresholds, prop_box, prop_begin, gt_box, gt_area, gt_begin, prop_count,
+    #  area_range (host), thresholds, workspace, workspace_bytes, overlap, excluded, error, counts, stream)
+    "b200_box_proposal_match": (ctypes.c_int, [ctypes.c_int] * 6 + [ctypes.c_void_p] * 9 + [ctypes.c_size_t] + [ctypes.c_void_p] * 4 +
+                                [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

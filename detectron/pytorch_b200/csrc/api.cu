@@ -99,6 +99,9 @@ int coco_accumulate(int, int, int, int, int, const int*, const int*, const int*,
                     int, const int*, const double*, void*, size_t, double*, double*, double*, cudaStream_t);
 int voc_match(int, int, int, double, const int*, const double*, const unsigned char*, const int*, const double*, int*, unsigned char*,
               cudaStream_t);
+size_t box_proposal_match_workspace_bytes(int, int, int, int);
+int box_proposal_match(int, int, int, int, int, int, const float*, const int*, const float*, const double*, const int*, const int*,
+                       const double*, const double*, void*, size_t, float*, unsigned char*, unsigned char*, long long*, cudaStream_t);
 int mask_targets(const float*, const int*, const int*, int, int, const int*, int, const int*, int, const int*, const float*, int, int,
                  float*, int*, cudaStream_t);
 int keypoint_candidates(const float*, const float*, const int*, int, const int*, const int*, const int*, const int*, const int*, int, float,
@@ -778,6 +781,20 @@ int b200_voc_match(int num_dets, int num_pairs, int num_gt, double ovthresh, con
                    unsigned char* outcome_out_dev, b200_stream_t stream) {
     return voc_match(num_dets, num_pairs, num_gt, ovthresh, pair_gt_begin_dev, gt_box_dev, gt_difficult_dev, det_pair_dev, det_box_dev,
                      workspace_dev, outcome_out_dev, (cudaStream_t)stream);
+}
+
+size_t b200_box_proposal_match_workspace_bytes(int num_props, int num_gt, int num_areas, int num_limits) {
+    return box_proposal_match_workspace_bytes(num_props, num_gt, num_areas, num_limits);
+}
+
+int b200_box_proposal_match(int num_images, int num_props, int num_gt, int num_areas, int num_limits, int num_thresholds,
+                            const float* prop_box_dev, const int* prop_begin_dev, const float* gt_box_dev, const double* gt_area_dev,
+                            const int* gt_begin_dev, const int* prop_count_dev, const double* area_range_host, const double* thresholds_dev,
+                            void* workspace, size_t workspace_bytes, float* overlap_out_dev, unsigned char* excluded_out_dev,
+                            unsigned char* error_out_dev, long long* count_out_dev, b200_stream_t stream) {
+    return box_proposal_match(num_images, num_props, num_gt, num_areas, num_limits, num_thresholds, prop_box_dev, prop_begin_dev, gt_box_dev,
+                              gt_area_dev, gt_begin_dev, prop_count_dev, area_range_host, thresholds_dev, workspace, workspace_bytes,
+                              overlap_out_dev, excluded_out_dev, error_out_dev, count_out_dev, (cudaStream_t)stream);
 }
 
 }  // extern "C"

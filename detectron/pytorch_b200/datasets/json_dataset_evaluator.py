@@ -1,4 +1,5 @@
-"""The reference's COCO evaluators (lib/datasets/json_dataset_evaluator.py:38-233, 320-430) with COCOeval on the device.
+"""The reference's COCO evaluators (lib/datasets/json_dataset_evaluator.py:38-233, 320-430) with COCOeval on the device, and its
+proposal recall (:236-317, evaluate_box_proposals) with the greedy matching on the device (csrc/box_proposals.cu).
 
 evaluate_boxes / evaluate_masks / evaluate_keypoints take the reference's arguments and return an object shaped like
 pycocotools' COCOeval after accumulate() and summarize() (datasets/coco_eval.py): `.params`, `.eval`, `.stats`,
@@ -15,8 +16,10 @@ that file (json round-trips float64 exactly).  The conversion is the writers', s
 """
 import json
 import logging
+import operator
 import os
 import pickle
+from collections import OrderedDict
 
 import numpy as np
 
@@ -220,3 +223,116 @@ def evaluate_keypoints(json_dataset, all_boxes, all_keypoints, output_dir, use_s
     _save(res, output_dir, "keypoint_results.pkl")
     res.summarize()
     return res
+
+
+# ---- proposal recall (lib/datasets/json_dataset_evaluator.py:236-317) ------------------------------------------------------
+# Area ranges by name, in the reference's order: [side_lo², side_hi²], both ends inclusive; "unbounded" is a side of 1e5.
+BOX_PROPOSAL_AREA_RANGES = OrderedDict(
+    (name, (float(lo) ** 2, float(hi) ** 2))
+    for name, lo, hi in (("all", 0, 1e5), ("small", 0, 32), ("medium", 32, 96), ("large", 96, 1e5), ("96-128", 96, 128),
+                         ("128-256", 128, 256), ("256-512", 256, 512), ("512-inf", 512, 1e5)))
+# Images packed per launch: bounds the device memory of a train-set-sized roidb.  The results do not depend on it.
+BOX_PROPOSAL_CHUNK_IMAGES = 1024
+
+
+def default_recall_thresholds():
+    return np.arange(0.5, 0.95 + 1e-5, 0.05)
+
+
+def effective_proposal_counts(num_props, limits):
+    """(len(limits), N) int32: how many of each image's num_props proposals a limit keeps, len(boxes[:limit]) (None keeps all; a
+    negative limit drops that many from the end, as the reference's slice does)."""
+    n = np.asarray(num_props, np.int64).reshape(-1)
+    out = np.empty((len(limits), n.size), np.int32)
+    for k, limit in enumerate(limits):
+        if limit is None:
+            out[k] = n
+        else:
+            limit = operator.index(limit)
+            out[k] = np.minimum(n, limit) if limit >= 0 else np.maximum(n + limit, 0)
+    return out
+
+
+def pack_roidb(roidb):
+    """The reference's per-entry selection, concatenated: proposals (gt_classes == 0 rows of `boxes`, float32) and ground truth
+    (gt_classes > 0 and not is_crowd: float32 boxes and float64 seg_areas), each with its (N + 1) row offsets."""
+    props, gts, areas = [], [], []
+    for entry in roidb:
+        cls = np.asarray(entry["gt_classes"])
+        rows = np.asarray(entry["boxes"])
+        positive = (cls > 0) & (np.asarray(entry["is_crowd"]) == 0)
+        gts.append(rows[positive].astype(np.float32).reshape(-1, 4))
+        areas.append(np.asarray(entry["seg_areas"])[positive].astype(np.float64))
+        props.append(rows[cls == 0].astype(np.float32).reshape(-1, 4))
+    begin = lambda xs: np.concatenate([[0], np.cumsum([len(x) for x in xs])]).astype(np.int32)  # noqa: E731
+    cat = lambda xs, w: np.ascontiguousarray(np.concatenate(xs)) if xs else np.zeros((0,) + w)  # noqa: E731
+    return (cat(props, (4,)).astype(np.float32), begin(props), cat(gts, (4,)).astype(np.float32), cat(areas, ()).astype(np.float64),
+            begin(gts))
+
+
+def _box_proposal_recall(roidb, area_names, limits, thresholds, device, want_overlaps):
+    """counts (L, A, T) int64, num_pos per area, and per (limit, area) the float64 gt_overlaps (unsorted) when want_overlaps, over
+    the whole roidb in chunks of BOX_PROPOSAL_CHUNK_IMAGES images, one launch per chunk.  A NaN IoU raises AssertionError naming
+    the first image of the first (limit, area) that has one, where the reference's `assert gt_ovr >= 0` fails."""
+    import torch
+    from .. import ops
+    for area in area_names:
+        _check_area(area)
+    ranges = np.asarray([BOX_PROPOSAL_AREA_RANGES[a] for a in area_names], np.float64)
+    thr = np.asarray(thresholds, np.float64).reshape(-1)
+    L, A = len(limits), len(area_names)
+    device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    counts = np.zeros((L, A, thr.size), np.int64)
+    num_pos = [0] * A
+    overlaps = [[[] for _ in range(A)] for _ in range(L)]
+    first_error = {}
+    thr_dev = torch.from_numpy(thr).to(device)
+    for c0 in range(0, len(roidb), BOX_PROPOSAL_CHUNK_IMAGES):
+        prop_box, prop_begin, gt_box, gt_area, gt_begin = pack_roidb(roidb[c0:c0 + BOX_PROPOSAL_CHUNK_IMAGES])
+        for a in range(A):
+            num_pos[a] += int(np.count_nonzero((gt_area >= ranges[a, 0]) & (gt_area <= ranges[a, 1])))
+        prop_count = effective_proposal_counts(np.diff(prop_begin), limits)
+        up = lambda x: torch.from_numpy(x).to(device)  # noqa: E731
+        overlap, excluded, error, cnt = ops.box_proposal_match_raw(up(prop_box), up(prop_begin), up(gt_box), up(gt_area), up(gt_begin),
+                                                                   up(prop_count), ranges, thr_dev)
+        counts += cnt.cpu().numpy()
+        error = error.cpu().numpy()
+        for l, a, i in zip(*np.nonzero(error)):                 # row-major: the first image of each (l, a) comes first
+            first_error.setdefault((int(l), int(a)), c0 + int(i))
+        if want_overlaps:
+            overlap, excluded = overlap.cpu().numpy(), excluded.cpu().numpy()
+            for l in range(L):
+                for a in range(A):
+                    overlaps[l][a].append(overlap[l, a][~excluded[l, a]].astype(np.float64))
+    if first_error:
+        (l, a), i = min(first_error.items())
+        raise AssertionError("roidb entry {}: a NaN IoU between its proposals and ground truth (limit {}, area '{}'); the "
+                             "reference's `assert gt_ovr >= 0` fails there".format(i, limits[l], area_names[a]))
+    return counts, num_pos, overlaps
+
+
+def _check_area(area):
+    if area not in BOX_PROPOSAL_AREA_RANGES:              # the reference's assert and message
+        raise AssertionError("Unknown area range: {}".format(area))
+
+
+def _recall_result(count, num_pos, thresholds, gt_overlaps):
+    """The dict the reference returns.  Each recall is the int64 count over float(num_pos) as a numpy scalar division (NaN, with
+    numpy's warning, when num_pos is 0), stored into an array shaped and typed like `thresholds`; ar is that array's mean."""
+    denom = float(num_pos)
+    recalls = np.zeros_like(thresholds)
+    for k, hits in enumerate(count):
+        recalls[k] = hits / denom
+    return {"ar": recalls.mean(), "recalls": recalls, "thresholds": thresholds, "gt_overlaps": gt_overlaps, "num_pos": num_pos}
+
+
+def evaluate_box_proposals(json_dataset, roidb, thresholds=None, area="all", limit=None, device=None):
+    """Proposal recall as the reference computes it (json_dataset_evaluator.py:236-317): the reference's dict `ar`, `recalls`,
+    `thresholds`, `gt_overlaps` (sorted float64) and `num_pos`, with the greedy matching and the per-threshold counts on the device.
+    roidb entries need `boxes` (proposals are the gt_classes == 0 rows, in order), `gt_classes`, `is_crowd` and `seg_areas`."""
+    _check_area(area)
+    if thresholds is None:
+        thresholds = default_recall_thresholds()
+    counts, num_pos, overlaps = _box_proposal_recall(roidb, [area], [limit], thresholds, device, want_overlaps=True)
+    gt_overlaps = np.sort(np.concatenate([np.zeros(0)] + overlaps[0][0]))
+    return _recall_result(counts[0, 0], num_pos[0], thresholds, gt_overlaps)

@@ -1,5 +1,5 @@
-"""The COCO branch of the reference's task_evaluation.evaluate_all (lib/datasets/task_evaluation.py:52-70), with the
-reference's OrderedDict result layout, so check_expected_results-style comparisons read it as they read the reference's."""
+"""The COCO branch of the reference's task_evaluation.evaluate_all (lib/datasets/task_evaluation.py:52-70) and its box-proposal
+task (evaluate_box_proposals, log_box_proposal_results), with the reference's OrderedDict result layout, so check_expected_results-style comparisons read it as they read the reference's."""
 import logging
 from collections import OrderedDict
 
@@ -77,3 +77,39 @@ def evaluate_all(dataset, all_boxes, all_segms, all_keyps, output_dir, cfg=None,
         all_results[dataset.name].update(_coco_eval_to_keypoint_results(coco_eval))
         logger.info("Evaluating keypoints is done!")
     return all_results
+
+
+# ---- box proposals (lib/datasets/task_evaluation.py:151-163, 371-386) ------------------------------------------------------
+_BOX_PROPOSAL_LIMITS = [100, 1000]
+_BOX_PROPOSAL_AREAS = OrderedDict([("all", ""), ("small", "s"), ("medium", "m"), ("large", "l")])
+
+
+def _empty_box_proposal_results():
+    return OrderedDict({"box_proposal": OrderedDict([("AR{}@{:d}".format(s, limit), -1)
+                                                     for limit in _BOX_PROPOSAL_LIMITS for s in _BOX_PROPOSAL_AREAS.values()])})
+
+
+def evaluate_box_proposals(dataset, roidb, device=None):
+    """The reference's eight keys (AR@100, ARs@100, ..., ARl@1000), each what json_dataset_evaluator.evaluate_box_proposals
+    returns as `ar` for that area and limit, all eight from one launch per chunk of the roidb."""
+    res = _empty_box_proposal_results()
+    areas = list(_BOX_PROPOSAL_AREAS)
+    thresholds = json_dataset_evaluator.default_recall_thresholds()
+    counts, num_pos, _ = json_dataset_evaluator._box_proposal_recall(roidb, areas, _BOX_PROPOSAL_LIMITS, thresholds, device,
+                                                                     want_overlaps=False)
+    for l, limit in enumerate(_BOX_PROPOSAL_LIMITS):
+        for a, (area, suffix) in enumerate(_BOX_PROPOSAL_AREAS.items()):
+            stats = json_dataset_evaluator._recall_result(counts[l, a], num_pos[a], thresholds, None)
+            res["box_proposal"]["AR{}@{:d}".format(suffix, limit)] = stats["ar"]
+    return OrderedDict([(dataset.name, res)])
+
+
+def log_box_proposal_results(results):
+    """Logs each dataset's name, then one `<metric>: <value>` line per box-proposal metric, the names padded to the longest and the
+    values with three decimals."""
+    for name, tasks in results.items():
+        metrics = tasks["box_proposal"]
+        width = max(len(key) for key in metrics)
+        logger.info(name)
+        for key, value in metrics.items():
+            logger.info("%s: %.3f", key.ljust(width), value)

@@ -7,6 +7,7 @@ These are what the reference-shaped shims in `model/` and `modeling/` delegate t
   * allocates outputs with torch.empty (the kernels define every output element; the reference
     needed `.zero_()` passes, functions/roi_align.py:23,39-40).
 """
+import numpy as np
 import torch
 from torch.autograd import Function
 from torch.autograd.function import once_differentiable
@@ -1157,3 +1158,64 @@ def voc_match_raw(pair_gt_begin, gt_box, gt_difficult, det_pair, det_box, ovthre
                                               gt_difficult.data_ptr(), det_pair.data_ptr(), det_box.data_ptr(), ws.data_ptr(),
                                               outcome.data_ptr(), _stream()), "b200_voc_match")
     return outcome[:D]
+
+
+# ------------------------------------------------------------------------------------------------
+# Proposal recall (the reference's evaluate_box_proposals; datasets/json_dataset_evaluator.py drives it)
+# ------------------------------------------------------------------------------------------------
+def _offsets_ok(begin, rows):
+    b = begin.cpu()
+    return b.numel() >= 1 and int(b[0]) == 0 and int(b[-1]) == rows and bool((b[1:] >= b[:-1]).all())
+
+
+def box_proposal_match_raw(prop_box, prop_begin, gt_box, gt_area, gt_begin, prop_count, area_ranges, thresholds):
+    """The greedy proposal-to-gt assignment of every (limit, area range, image) in one launch.
+    prop_box (P, 4) and prop_begin (N + 1): each image's proposals in the reference's order (e.g. GenerateProposalsOp's
+    rois[:, 1:] / im_scale); gt_box (G, 4), gt_area (G,) and gt_begin (N + 1): each image's non-crowd foreground gt boxes and
+    seg_areas; prop_count (L, N): the proposals each limit keeps (json_dataset_evaluator.effective_proposal_counts).  All are CUDA
+    tensors on one device; boxes are evaluated as float32, gt_area as float64 and the offsets and counts as int32 (other dtypes are
+    converted, as the reference casts its boxes with astype(np.float32)).  The offsets must start at 0, not decrease and end at P / G.
+    area_ranges: A <= 8 host pairs [lo, hi]; thresholds: T float64 values (host sequence or device tensor).
+    Returns overlap (L, A, G) float32 (the recorded IoU, 0 if unmatched), excluded (L, A, G) bool (not part of gt_overlaps: out of range
+    or image without proposals), error (L, A, N) bool (a NaN IoU fails the reference's assert) and counts (L, A, T) int64 (counted gts
+    whose float64 overlap is >= each threshold, over the images without error)."""
+    named = (("prop_box", prop_box), ("prop_begin", prop_begin), ("gt_box", gt_box), ("gt_area", gt_area), ("gt_begin", gt_begin),
+             ("prop_count", prop_count))
+    for name, t in named:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise ValueError("box_proposal_match_raw: %s must be a CUDA tensor" % name)
+    dev = prop_begin.device
+    if any(t.device != dev for _, t in named):
+        raise ValueError("box_proposal_match_raw: all tensors must be on one device, got %s" % ([str(t.device) for _, t in named],))
+    prop_box = prop_box.to(torch.float32).contiguous()
+    gt_box = gt_box.to(torch.float32).contiguous()
+    gt_area = gt_area.to(torch.float64).contiguous()
+    prop_begin, gt_begin, prop_count = (t.to(torch.int32).contiguous() for t in (prop_begin, gt_begin, prop_count))
+    if prop_box.dim() != 2 or prop_box.shape[1] != 4 or gt_box.dim() != 2 or gt_box.shape[1] != 4:
+        raise ValueError("box_proposal_match_raw: prop_box and gt_box must be (rows, 4), got %s and %s"
+                         % (tuple(prop_box.shape), tuple(gt_box.shape)))
+    N, P, G = prop_begin.numel() - 1, prop_box.shape[0], gt_box.shape[0]
+    if prop_begin.dim() != 1 or gt_begin.shape != prop_begin.shape or gt_area.shape != (G,):
+        raise ValueError("box_proposal_match_raw: prop_begin and gt_begin must both be (N + 1,) and gt_area (G,)")
+    if prop_count.dim() != 2 or prop_count.shape[1] != N:
+        raise ValueError("box_proposal_match_raw: prop_count must be (L, %d), got %s" % (N, tuple(prop_count.shape)))
+    if not _offsets_ok(prop_begin, P) or not _offsets_ok(gt_begin, G):
+        raise ValueError("box_proposal_match_raw: row offsets must start at 0, not decrease and end at the row count")
+    L = prop_count.shape[0]
+    ranges = np.ascontiguousarray(np.asarray(area_ranges, np.float64).reshape(-1, 2))
+    A = ranges.shape[0]
+    thr = torch.as_tensor(thresholds, dtype=torch.float64, device=dev).reshape(-1).contiguous()
+    T = thr.numel()
+    overlap = torch.empty((L, A, G), dtype=torch.float32, device=dev)
+    excluded = torch.empty((L, A, G), dtype=torch.uint8, device=dev)
+    error = torch.empty((L, A, N), dtype=torch.uint8, device=dev)
+    counts = torch.zeros((L, A, T), dtype=torch.int64, device=dev)
+    lib = _lib.load()
+    ws = torch.empty((lib.b200_box_proposal_match_workspace_bytes(P, G, A, L),), dtype=torch.uint8, device=dev)
+    ptr = lambda t: t.data_ptr() if t.numel() else None  # noqa: E731
+    with torch.cuda.device(dev):
+        _lib.check(lib.b200_box_proposal_match(N, P, G, A, L, T, ptr(prop_box), prop_begin.data_ptr(), ptr(gt_box), ptr(gt_area),
+                                               gt_begin.data_ptr(), prop_count.data_ptr(), ranges.ctypes.data, ptr(thr), ws.data_ptr(),
+                                               ws.numel(), ptr(overlap), ptr(excluded), error.data_ptr(), ptr(counts), _stream()),
+                   "b200_box_proposal_match")
+    return overlap, excluded.bool(), error.bool(), counts

@@ -540,6 +540,34 @@ B200_API int b200_voc_match(int num_dets, int num_pairs, int num_gt, double ovth
                             const unsigned char* gt_difficult_dev, const int* det_pair_dev, const double* det_box_dev, int* workspace_dev,
                             unsigned char* outcome_out_dev, b200_stream_t stream);
 
+/* ---- Proposal recall (lib/datasets/json_dataset_evaluator.py:236-317, evaluate_box_proposals' greedy assignment) ---------------
+ * b200_box_proposal_match runs the reference's per-image assignment for every (limit l, area range a, image i) in one launch.
+ * Proposals: image i owns rows prop_begin_dev[i] .. [i + 1] - 1 (num_images + 1 non-decreasing int32, last = num_props) of prop_box_dev
+ *   (float32 x1, y1, x2, y2, 16-byte aligned).  prop_count_dev (num_limits x num_images int32): how many of them limit l keeps, clamped
+ *   to [0, P_i] (the caller's len(boxes[:limit])).  An image with P_i == 0 is skipped, as the reference skips it.
+ * Ground truth: image i owns rows gt_begin_dev[i] .. [i + 1] - 1 (last = num_gt) of gt_box_dev (float32, 16-byte aligned) and
+ *   gt_area_dev (float64 seg_areas); only non-crowd foreground boxes belong here.  area_range_host: num_areas (1 .. 8) float64 pairs
+ *   [lo, hi]; a gt is in range when lo <= area <= hi (a NaN area never is).
+ * Matching, per item, over the kept proposals x the in-range gts, IoU by the reference's cython bbox_overlaps (float32 with double
+ *   area sums): min(P, G) times, the gt whose best IoU over the unused proposals is largest (lowest gt row on ties) is matched to the
+ *   first proposal reaching it; that IoU is recorded and both are used.
+ * Outputs, per (l, a, gt row) at [(l * num_areas + a) * num_gt + row]: overlap_out_dev (float32) the recorded IoU, 0 if unmatched;
+ *   excluded_out_dev (uint8) 1 when the gt is out of range or its image is skipped (not part of gt_overlaps), else 0.
+ *   error_out_dev (num_limits x num_areas x num_images uint8): 1 when a NaN IoU lies in the item's matrix and the reference's
+ *   `assert gt_ovr >= 0` would fail (only items with at least one iteration); the item's outputs are then unspecified.
+ *   count_out_dev (num_limits x num_areas x num_thresholds int64, 8-byte aligned): the counted gts with float64(overlap) >=
+ *   thresholds_dev[t] (float64), summed over the images without error.
+ * workspace: b200_box_proposal_match_workspace_bytes(...) bytes, overwritten (small or missing: B200_ROI_EWORKSPACE).
+ * Bad sizes or null pointers: B200_ROI_EINVAL before any launch.  Zero items (no images, areas or limits): 0, outputs untouched. */
+#define B200_BOX_PROPOSAL_MAX_AREAS 8
+B200_API size_t b200_box_proposal_match_workspace_bytes(int num_props, int num_gt, int num_areas, int num_limits);
+B200_API int b200_box_proposal_match(int num_images, int num_props, int num_gt, int num_areas, int num_limits, int num_thresholds,
+                                     const float* prop_box_dev, const int* prop_begin_dev, const float* gt_box_dev, const double* gt_area_dev,
+                                     const int* gt_begin_dev, const int* prop_count_dev, const double* area_range_host,
+                                     const double* thresholds_dev, void* workspace, size_t workspace_bytes, float* overlap_out_dev,
+                                     unsigned char* excluded_out_dev, unsigned char* error_out_dev, long long* count_out_dev,
+                                     b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
