@@ -16,11 +16,17 @@
 //
 // Work = "fragments": up to 8 consecutive bins of one bin row of one RoI, keyed by the first feature row
 // they read.  A fragment is processed by ONE warp when the rows [key, end) it needs are resident, so every
-// output element is computed by one lane in the reference's own operation order and written exactly once
-// with a plain store: bit-identical to the reference kernel, deterministic, no zero-fill of the output.
-// Only bins whose samples cannot be resident together (x-span beyond the strip halo, y-span beyond the
-// ring) are cut into per-sample fragments that accumulate with red.global.add onto elements the
-// prepass zeroed (at most two partial sums per element -> still deterministic).
+// output element is computed by one lane in the reference's own operation order: bit-identical to the
+// reference kernel, deterministic, no zero-fill of the output.  Only bins whose samples cannot be resident
+// together (x-span beyond the strip halo, y-span beyond the ring) are cut into per-sample fragments that
+// accumulate with red.global.add onto elements the prepass zeroed (at most two partial sums per element ->
+// still deterministic).
+//
+// Output: staged once, transposed once.  The bin loop stores each bin's result for lane = channel into its own
+// output row laid out (bin, channel): one aligned 128-byte line per bin and 32-channel group.  (The (channel, bin)
+// layout would give every store a run of at most 8 floats inside one channel plane -- part of a 32-byte sector,
+// and such a store that misses L2 stalls the memory pipeline the bin loop's shared-memory loads share.)  After
+// a grid barrier every CTA transposes whole rows in place to (channel, bin) through shared memory.
 //
 // Prepass (channel independent): `clear` zeroes the counters; `prep`, ONE kernel launched as its programmatic
 // dependent, builds the per-RoI axis tables (all IEEE divisions; ring-slot byte offsets precomputed), lists the
@@ -33,6 +39,7 @@
 #include "common.cuh"
 #include "strip_prep.cuh"
 #include <mutex>
+#include <type_traits>
 #include <string.h>
 #include <stdlib.h>
 
@@ -43,11 +50,10 @@ namespace {
 constexpr int kConsumerWarps = 16;
 constexpr int kProducerWarps = 4;
 constexpr int kStreamThreads = 32 * (kConsumerWarps + kProducerWarps);
-constexpr int kFragBins = 8;                                  // bins per fragment (one flush)
-constexpr int kStageStride = 36;                              // words per staged bin: conflict-free both ways
+constexpr int kFragBins = 8;                                  // bins per fragment
 constexpr int kTabWords = 18 * 4;                              // per-warp axis-table buffer: 16 x entries + 2 y entries
-constexpr int kStageWordsPerWarp = kFragBins * kStageStride + kTabWords;
 constexpr int kMaxSlots = 32;                                 // ring depth K <= 32 (phase bits live in one register)
+constexpr unsigned kBarBytes = 2 * kMaxSlots * 8;             // full[] and empty[] mbarriers, at the start of dynamic shared memory
 constexpr int kAxisMaxS = 32;                                 // P * sampling_ratio per axis
 constexpr int kPrepThreads = 128;
 constexpr unsigned kRowCost = 8u;                             // cost of streaming one row (16 acquires + staging), in bins
@@ -78,6 +84,7 @@ struct StreamGeom {
     int G;                      // 32-channel groups
     int pieces;                 // persistent CTAs
     int max_entries, cap_r;     // cap_r: fragments one RoI can have at most
+    int tail_rows;              // output rows the main kernel's tail holds in shared memory at once
     StreamLevel lv[kMaxLevels];
     int colstart[kMaxCols + 1]; // first key of every column (its rows are consecutive keys); colstart[Q] = keys
 };
@@ -95,7 +102,7 @@ struct StreamWs {
     int* hist;                  // [keys] fragments per key                           (zero block)
     int* cost;                  // [keys] estimated cost per key                      (zero block)
     int* maxend;                // [keys] max over the key's fragments of `end`       (zero block)
-    int* ticket;                // [4] grid barrier of the prepass                    (zero block)
+    int* ticket;                // [4] grid barriers: [0] the prepass's, [1] the main kernel's (zero block)
     int* rowptr;                // [keys + 1] CSR offsets into entries
     int* piece_start;           // [pieces + 1] linear start index of every piece
     uint2* entries;             // fragment records
@@ -304,11 +311,11 @@ stream_prep(const float* __restrict__ rois, StreamGeom g, StreamWs ws, float* __
         }
         __syncthreads();
         const int nz = s_nzero;
-        if (nz > 0) {
+        if (nz > 0) {                                         // the output row is in the main kernel's staging layout (bin, channel)
             float* out_r = out + (size_t)(row_map ? row_map[r] : r) * g.C * bins;
             for (int idx = t; idx < g.C * nz; idx += kPrepThreads) {
-                const int c = idx / nz, k = idx - c * nz;
-                out_r[(size_t)c * bins + s_zero[k]] = 0.f;
+                const int k = idx / g.C, c = idx - k * g.C;
+                out_r[(size_t)s_zero[k] * g.C + c] = 0.f;
             }
         }
     }
@@ -353,13 +360,25 @@ __device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity, unsigne
         if (spins > (1 << 20)) __trap();
     }
 }
+// L2 eviction priorities.  Each feature row is read once (evict_first); the staged output rows are read back by the tail, so
+// they are kept (evict_last) until the tail rewrites them (evict_normal, which also leaves no evict_last lines behind).
+// At cfg2 the staged rows are 26 MB of the 50 MB L2 while 56 MB of features stream through it.
+__device__ __forceinline__ u64 l2_evict_first() { u64 p; asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p)); return p; }
+__device__ __forceinline__ u64 l2_evict_last() { u64 p; asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p)); return p; }
+__device__ __forceinline__ u64 l2_evict_normal() { u64 p; asm("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p)); return p; }
+__device__ __forceinline__ void st_hint(float* p, float v, u64 pol) {
+    asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(p), "f"(v), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void st_hint(float* p, float4 v, u64 pol) {
+    asm volatile("st.global.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w), "l"(pol) : "memory");
+}
 // 4-byte cp.async (LDGSTS): global -> shared without registers.
-__device__ __forceinline__ void cp_async4(unsigned dst, const float* src) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+__device__ __forceinline__ void cp_async4(unsigned dst, const float* src, u64 pol) {
+    asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "l"(pol) : "memory");
 }
 // ok == false copies nothing and zero-fills the word
-__device__ __forceinline__ void cp_async4_if(unsigned dst, const float* src, bool ok) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(ok ? 4 : 0) : "memory");
+__device__ __forceinline__ void cp_async4_if(unsigned dst, const float* src, bool ok, u64 pol) {
+    asm volatile("cp.async.ca.shared.global.L2::cache_hint [%0], [%1], 4, %2, %3;" ::"r"(dst), "l"(src), "r"(ok ? 4 : 0), "l"(pol) : "memory");
 }
 // the mbarrier receives one arrival from this thread once all its earlier cp.async have landed
 __device__ __forceinline__ void cp_async_arrive(unsigned bar) {
@@ -380,7 +399,9 @@ struct StreamArgs {
     const int* piece_start;
     float* out;
     const int* row_map;
-    int C, G, K, WX, PH, PW, ny, nx, L, Q;
+    int* ticket;                // grid barrier between the fragments and the transpose (zeroed by stream_clear)
+    int R, C, G, K, WX, PH, PW, ny, nx, L, Q;
+    int tail_rows;
     StreamLevel lv[kMaxLevels];
     int colstart[kMaxCols + 1];
 };
@@ -461,6 +482,7 @@ __device__ __forceinline__ float sample_val(const Taps& t, u64 hyhy, u64 lyly, u
 // with 4-byte cp.async.
 template <int M>
 __device__ __forceinline__ void stage_row(const float* __restrict__ src_row, size_t plane, unsigned dst, int xw, int cvalid, int lane) {
+    const u64 pol = l2_evict_first();
     // src_row: (channel 0, row y, column x0); xw = number of valid columns from x0; cvalid = number of real channels
     constexpr int SX = 32 * M + 1;
     if (cvalid == 32 && xw >= SX) {                           // interior: no predicates, constant offsets
@@ -469,10 +491,10 @@ __device__ __forceinline__ void stage_row(const float* __restrict__ src_row, siz
 #pragma unroll 8
         for (int c = 0; c < 32; ++c) {
 #pragma unroll
-            for (int m = 0; m < M; ++m) cp_async4(d + (unsigned)(c * SX + 32 * m) * 4u, sc + 32 * m);
+            for (int m = 0; m < M; ++m) cp_async4(d + (unsigned)(c * SX + 32 * m) * 4u, sc + 32 * m, pol);
             sc += plane;
         }
-        cp_async4(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (size_t)lane * plane + 32 * M);
+        cp_async4(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (size_t)lane * plane + 32 * M, pol);
     } else {
 #pragma unroll 4
         for (int c = 0; c < 32; ++c) {
@@ -482,59 +504,22 @@ __device__ __forceinline__ void stage_row(const float* __restrict__ src_row, siz
             for (int m = 0; m < M; ++m) {
                 const int x = lane + 32 * m;
                 const bool ok = cok && x < xw;
-                cp_async4_if(dst + (unsigned)(c * SX + x) * 4u, sc + (ok ? x : 0), ok);
+                cp_async4_if(dst + (unsigned)(c * SX + x) * 4u, sc + (ok ? x : 0), ok, pol);
             }
         }
         const bool ok = lane < cvalid && 32 * M < xw;
-        cp_async4_if(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (ok ? (size_t)lane * plane + 32 * M : 0), ok);
+        cp_async4_if(dst + (unsigned)(lane * SX + 32 * M) * 4u, src_row + (ok ? (size_t)lane * plane + 32 * M : 0), ok, pol);
     }
 }
 
-// Prefetch into L2 the output runs fragment `en` will store (lane = channel: the first and the last bin of its run, at most
-// two sectors).  A run is npw <= 8 consecutive floats of one channel plane, so every flush store covers only part of a
-// 32-byte sector, and such a store that misses L2 stalls the memory pipeline the bin loop's shared-memory loads share (at
-// cfg2 the main kernel spans 115 us with the stores and 57 us without them; 95 us with this prefetch: DESIGN.md 4.1a).
-__device__ __forceinline__ void prefetch_out(const uint2& en, const StreamArgs& a, int c0, int bins, int lane) {
-    const int r = en.x & 0xffffu, ph = (en.x >> 16) & 31u, pw0 = (en.x >> 21) & 31u, npw = (int)((en.x >> 26) & 7u) + 1;
-    if (c0 + lane < a.C) {
-        const int orow = a.row_map ? __ldg(&a.row_map[r]) : r;
-        const float* p = a.out + ((size_t)orow * a.C + c0 + lane) * bins + ph * a.PW + pw0;
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-        asm volatile("prefetch.global.L2 [%0];" ::"l"(p + npw - 1));
-    }
-}
-
+// The CTA's piece [L0, L1) of the linear space: producers stream its rows through the ring, consumers compute its fragments
+// and store every bin's result into the output row's staging layout (bin, channel).  ring: K + 1 slots of RB bytes, then
+// kConsumerWarps per-warp axis-table buffers of kTabWords words.
 template <int SR, int M>
-__global__ void __launch_bounds__(kStreamThreads, 1)
-roi_align_stream_fwd(const StreamArgs a) {
+__device__ __forceinline__ void stream_fragments(const StreamArgs& a, unsigned ring, unsigned bars, int L0, int L1) {
     constexpr int SX = 32 * M + 1;
     constexpr int RB = 128 * SX;                                  // bytes of one ring slot
-    extern __shared__ unsigned char smem_raw[];
-    const unsigned ring = (smem_addr(smem_raw) + 127u) & ~127u;
-    unsigned char* ring_ptr = smem_raw + (ring - smem_addr(smem_raw));
-    // ring: K logical slots + one mirror of slot 0 behind slot K - 1, so that row y + 1 is always the next physical slot
-    float* stage_all = reinterpret_cast<float*>(ring_ptr + (size_t)(a.K + 1) * RB);
-    const unsigned bars = ring + (unsigned)(a.K + 1) * (unsigned)RB + kConsumerWarps * kStageWordsPerWarp * 4;
-    // full[k] at bars + 8k (32 arrivals: the lanes of the producer warp that staged the row),
-    // empty[k] at bars + 8 * (kMaxSlots + k) (one arrival per consumer warp)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-
-    {   // the ring starts zeroed: a tap with weight 0 may read a slot that was never written (clamped last row)
-        const int n16 = (a.K + 1) * (RB / 16);
-        float4* r4 = reinterpret_cast<float4*>(ring_ptr);
-        for (int k = tid; k < n16; k += kStreamThreads) r4[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-    if (tid == 0) {
-        for (int k = 0; k < a.K; ++k) { mbar_init(bars + 8u * k, 32u); mbar_init(bars + 8u * (kMaxSlots + k), kConsumerWarps); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    asm volatile("griddepcontrol.wait;" ::: "memory");             // the prepass's results are visible from here on
-    // Everything the prepass wrote is read with ld.volatile / ld.cg from here on, never __ldg: a read-only (.nc) load carries
-    // no dependence on the wait above and may be hoisted above it (DESIGN.md 4.1)
-    int L0, L1;
-    asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L0) : "l"(a.piece_start + blockIdx.x) : "memory");
-    asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L1) : "l"(a.piece_start + blockIdx.x + 1) : "memory");
 
     if (warp >= kConsumerWarps) {
         // =============================== producers ===============================
@@ -579,13 +564,12 @@ roi_align_stream_fwd(const StreamArgs a) {
     }
 
     // =============================== consumers ===============================
-    float* stage = stage_all + warp * kStageWordsPerWarp;
-    const unsigned tbuf = smem_addr(stage + kFragBins * kStageStride);      // 16-byte aligned: 288 words precede it
+    const unsigned tbuf = ring + (unsigned)(a.K + 1) * (unsigned)RB + (unsigned)(warp * kTabWords) * 4u;   // 16-byte aligned
     const unsigned lane_base = ring + (unsigned)(lane * SX) * 4u;
     const int bins = a.PH * a.PW;
     unsigned fphase = 0u;
-    const int chsub = lane >> 3, fb = lane & 7;
     constexpr float kInvCount = 1.f / (float)(SR * SR);
+    const u64 keep = l2_evict_last();                             // the tail reads the staged rows back
 
     for (int L = L0; L < L1;) {
         const Item it = decode_item(L, L1, a, lane);
@@ -595,6 +579,7 @@ roi_align_stream_fwd(const StreamArgs a) {
         int acq = it.ya, rel = it.ya;
         int acq_slot = it.ya % a.K, rel_slot = acq_slot;
         const int c0 = it.g * 32;
+        const bool cok = c0 + lane < a.C;
         // every warp waits for every row of the item before it releases it, in stream order (keeps the per-slot
         // phase bits in step with the producers)
         auto acquire_to = [&](int row_end, unsigned tag) {
@@ -658,7 +643,7 @@ roi_align_stream_fwd(const StreamArgs a) {
                 acquire_to(acq + 1, 0x2000u);
                 release_to(acq);
             }
-            prefetch_out(cur, a, c0, bins, lane);               // lands while this warp waits for its rows and computes
+            const int orow = a.row_map ? __ldg(&a.row_map[r]) : r;       // lands while this warp waits for its rows
             acquire_to(end, 0x2800u);                           // rows [key, end) must be resident
             const uint4 yA = lds128(tbuf + 16 * 16);
             uint4 yB = yA;
@@ -668,7 +653,8 @@ roi_align_stream_fwd(const StreamArgs a) {
             const u64 hh0 = pack2f(__uint_as_float(yA.x), __uint_as_float(yA.x)), ll0 = pack2f(__uint_as_float(yA.y), __uint_as_float(yA.y));
             const u64 hh1 = pack2f(__uint_as_float(yB.x), __uint_as_float(yB.x)), ll1 = pack2f(__uint_as_float(yB.y), __uint_as_float(yB.y));
             unsigned tb = tbuf;                                   // this bin's x entries (broadcast reads)
-            unsigned sp = smem_addr(stage) + (unsigned)lane * 4u; // where this lane parks the bin's result
+            // this lane's result of the bin: output row orow in the staging layout (bin, channel)
+            float* op = a.out + ((size_t)orow * bins + ph * a.PW + pw0) * a.C + c0 + lane;
             const unsigned tb_end = tbuf + (unsigned)npw * (SR * 16u);
             if (SR == 2 && smask == 0xfu) {
                 // whole bins (the common case): all 16 taps are requested before the first one is used
@@ -684,8 +670,8 @@ roi_align_stream_fwd(const StreamArgs a) {
                     acc = __fadd_rn(acc, sample_val(t1, hh0, ll0, wxB));
                     acc = __fadd_rn(acc, sample_val(t2, hh1, ll1, wxA));
                     acc = __fadd_rn(acc, sample_val(t3, hh1, ll1, wxB));
-                    asm volatile("st.shared.f32 [%0], %1;" ::"r"(sp), "f"(__fmul_rn(acc, kInvCount)) : "memory");   // count 4: exact
-                    tb += 32u; sp += kStageStride * 4u;
+                    if (cok) st_hint(op, __fmul_rn(acc, kInvCount), keep);      // count 4: exact
+                    tb += 32u; op += a.C;
                 } while (tb != tb_end);
             } else {
                 do {
@@ -703,33 +689,15 @@ roi_align_stream_fwd(const StreamArgs a) {
                         if (smask & 4u) acc = __fadd_rn(acc, sample_val(load_taps<RB>(rt1 + cxA.z), hh1, ll1, wxA));
                         if (smask & 8u) acc = __fadd_rn(acc, sample_val(load_taps<RB>(rt1 + cxB.z), hh1, ll1, wxB));
                     }
-                    asm volatile("st.shared.f32 [%0], %1;" ::"r"(sp), "f"(__fmul_rn(acc, kInvCount)) : "memory");   // count 1 / 4: exact
-                    tb += SR * 16u; sp += kStageStride * 4u;
+                    const float v = __fmul_rn(acc, kInvCount);     // count 1 / 4: exact
+                    if (cok) {
+                        if (red) atomicAdd(op, v);
+                        else st_hint(op, v, keep);
+                    }
+                    tb += SR * 16u; op += a.C;
                 } while (tb != tb_end);
             }
-            __syncwarp();
-            // flush: lanes = (channel within a group of 4, bin) -> a store's lanes are consecutive bins of one channel
-            if (fb < npw) {
-                const int orow = a.row_map ? __ldg(&a.row_map[r]) : r;
-                float* dst = a.out + ((size_t)orow * a.C + c0) * bins + ph * a.PW + pw0 + fb;
-                const float* src = stage + fb * kStageStride + chsub;
-                const int cmax = a.C - c0 - chsub;               // channel 4*cb + chsub is real iff 4*cb < cmax
-                if (!red && cmax + chsub >= 32) {                        // a full channel group: no predicates, one pointer walk
-                    float* d = dst + (size_t)chsub * bins;
-                    const size_t step = (size_t)bins * 4;
-#pragma unroll
-                    for (int cb = 0; cb < 8; ++cb) { *d = src[4 * cb]; d += step; }
-                } else if (!red) {
-#pragma unroll
-                    for (int cb = 0; cb < 8; ++cb)
-                        if (4 * cb < cmax) dst[(size_t)(4 * cb + chsub) * bins] = src[4 * cb];
-                } else {
-#pragma unroll
-                    for (int cb = 0; cb < 8; ++cb)
-                        if (4 * cb < cmax) atomicAdd(dst + (size_t)(4 * cb + chsub) * bins, src[4 * cb]);
-                }
-            }
-            __syncwarp();
+            __syncwarp();                                       // the table buffer is rewritten for the next fragment
             e = e_next;
         }
         // item tail: nothing more to read -- give back what is held, then pass the remaining rows through one by one
@@ -741,6 +709,110 @@ roi_align_stream_fwd(const StreamArgs a) {
         }
         __syncwarp();
     }
+}
+
+// Words per bin of a row block in the tail's shared memory: odd, so that the lanes of a warp that read one channel at
+// consecutive bins hit distinct banks.
+__host__ __device__ __forceinline__ int tail_stride(int C) { return C | 1; }
+
+__device__ __forceinline__ void put_floats(float* d, float v) { d[0] = v; }
+__device__ __forceinline__ void put_floats(float* d, float4 v) { d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w; }
+
+// Transpose this CTA's output rows r = blockIdx.x + j * gridDim.x in place, from (bin, channel) to (channel, bin), through
+// shared memory s, a.tail_rows rows at a time: every element of a batch is read before any is written, and no other CTA
+// touches these rows.  V = 4: 16-byte loads and stores (C % 4 == 0 and a 16-byte aligned output); else V = 1.  The rows were
+// written by other CTAs of this grid: L2 loads (.cg), never .nc (DESIGN.md 4.1).
+template <int V>
+__device__ __forceinline__ void transpose_rows(const StreamArgs& a, float* s) {
+    using VT = typename std::conditional<V == 4, float4, float>::type;
+    constexpr int kUnroll = 4;                                    // loads in flight per thread
+    const int tid = threadIdx.x;
+    const int C = a.C, bins = a.PH * a.PW, cs = tail_stride(C);
+    const int nv = C * bins / V;                                  // V-wide items of one row
+    const int* row_map = a.row_map;
+    const u64 norm = l2_evict_normal();
+    for (int r0 = blockIdx.x; r0 < a.R; r0 += a.tail_rows * (int)gridDim.x) {
+        const int nrows = min(a.tail_rows, (a.R - r0 + (int)gridDim.x - 1) / (int)gridDim.x);
+        const int n = nrows * nv;
+        for (int i0 = tid; i0 < n; i0 += kUnroll * kStreamThreads) {
+            VT v[kUnroll];
+            int at[kUnroll];                                      // where item u goes in shared memory
+#pragma unroll
+            for (int u = 0; u < kUnroll; ++u) {
+                const int i = i0 + u * kStreamThreads;
+                if (i < n) {
+                    const int j = i / nv, f = (i - j * nv) * V;
+                    const int r = r0 + j * (int)gridDim.x;
+                    const int orow = row_map ? row_map[r] : r;
+                    v[u] = __ldcg(reinterpret_cast<const VT*>(a.out + (size_t)orow * C * bins + f));
+                    const int b = f / C;
+                    at[u] = (j * bins + b) * cs + (f - b * C);
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < kUnroll; ++u)
+                if (i0 + u * kStreamThreads < n) put_floats(s + at[u], v[u]);
+        }
+        __syncthreads();
+        for (int i = tid; i < n; i += kStreamThreads) {
+            const int j = i / nv, o = (i - j * nv) * V;
+            const int r = r0 + j * (int)gridDim.x;
+            const int orow = row_map ? row_map[r] : r;
+            const float* sj = s + (size_t)j * bins * cs;
+            int c = o / bins, b = o - c * bins;
+            float w[V];
+#pragma unroll
+            for (int e = 0; e < V; ++e) {
+                if (b == bins) { b = 0; ++c; }
+                w[e] = sj[b * cs + c];
+                ++b;
+            }
+            float* d = a.out + (size_t)orow * C * bins + o;
+            if constexpr (V == 4) st_hint(d, make_float4(w[0], w[1], w[2], w[3]), norm);
+            else st_hint(d, w[0], norm);
+        }
+        __syncthreads();
+    }
+}
+
+template <int SR, int M>
+__global__ void __launch_bounds__(kStreamThreads, 1)
+roi_align_stream_fwd(const StreamArgs a) {
+    constexpr int RB = 128 * (32 * M + 1);                        // bytes of one ring slot
+    extern __shared__ unsigned char smem_raw[];
+    // dynamic shared memory: the mbarriers -- full[k] at bars + 8k (32 arrivals: the lanes of the producer warp that staged the
+    // row), empty[k] at bars + 8 * (kMaxSlots + k) (one arrival per consumer warp) -- then the ring (K logical slots + one
+    // mirror of slot 0 behind slot K - 1, so that row y + 1 is always the next physical slot) and the per-warp table buffers,
+    // whose space the tail reuses for the row blocks it transposes
+    const unsigned bars = (smem_addr(smem_raw) + 127u) & ~127u;
+    const unsigned ring = bars + kBarBytes;
+    unsigned char* ring_ptr = smem_raw + (ring - smem_addr(smem_raw));
+    const int tid = threadIdx.x;
+
+    {   // the ring starts zeroed: a tap with weight 0 may read a slot that was never written (clamped last row)
+        const int n16 = (a.K + 1) * (RB / 16);
+        float4* r4 = reinterpret_cast<float4*>(ring_ptr);
+        for (int k = tid; k < n16; k += kStreamThreads) r4[k] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    if (tid == 0) {
+        for (int k = 0; k < a.K; ++k) { mbar_init(bars + 8u * k, 32u); mbar_init(bars + 8u * (kMaxSlots + k), kConsumerWarps); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    asm volatile("griddepcontrol.wait;" ::: "memory");             // the prepass's results are visible from here on
+    // Everything the prepass wrote is read with ld.volatile / ld.cg from here on, never __ldg: a read-only (.nc) load carries
+    // no dependence on the wait above and may be hoisted above it (DESIGN.md 4.1)
+    int L0, L1;
+    asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L0) : "l"(a.piece_start + blockIdx.x) : "memory");
+    asm volatile("ld.volatile.global.s32 %0, [%1];" : "=r"(L1) : "l"(a.piece_start + blockIdx.x + 1) : "memory");
+    stream_fragments<SR, M>(a, ring, bars, L0, L1);
+
+    // ---- tail: once every CTA has stored its fragments (the grid is resident: see the launcher), transpose the rows
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    prepass::grid_barrier(a.ticket);
+    float* blocks = reinterpret_cast<float*>(ring_ptr);
+    if ((a.C & 3) == 0 && (reinterpret_cast<uintptr_t>(a.out) & 15u) == 0) transpose_rows<4>(a, blocks);
+    else transpose_rows<1>(a, blocks);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -765,9 +837,9 @@ bool stream_geometry(int levels, const float* const* bottoms, const int* heights
     if ((long long)R * PH * PW * sr * sr >= (1LL << 28)) return false;
     for (int l = 0; l < levels; ++l)
         if (heights[l] < 2 || widths[l] < 2 || heights[l] > 65535) return false;
-    // ring budget: everything but the per-warp staging, the barriers and the alignment slack
-    const unsigned fixed = kConsumerWarps * kStageWordsPerWarp * 4 + 2 * kMaxSlots * 8 + 128;
-    const unsigned ring_budget = kSmemBudget - fixed;
+    // ring budget: everything but the per-warp table buffers, the barriers and the alignment slack
+    const unsigned tabs = kConsumerWarps * kTabWords * 4;
+    const unsigned ring_budget = kSmemBudget - tabs - kBarBytes - 128;
     int best_sx = 0, best_wx = 0, best_k = 0;
     long best_score = -1;
     for (int m = 1; m <= 3; ++m) {                            // SX = 32 m + 1: odd channel stride, m coalesced chunks + 1 column
@@ -786,6 +858,13 @@ bool stream_geometry(int levels, const float* const* bottoms, const int* heights
         if (best_score < 0 || score < best_score) { best_score = score; best_sx = sx; best_wx = wx; best_k = k; }
     }
     if (best_score < 0) return false;
+    // the main kernel's tail transposes whole output rows in shared memory: the ring's and the table buffers' space, or more
+    // when one row block needs it
+    const unsigned long long block = (unsigned long long)PH * PW * tail_stride(C) * 4u;
+    if (block > kSmemBudget - kBarBytes - 128) return false;
+    const unsigned ring_bytes = (unsigned)(best_k + 1) * 128u * (unsigned)best_sx + tabs;
+    const unsigned tail_bytes = ring_bytes > block ? ring_bytes : (unsigned)block;
+    g->tail_rows = (int)(tail_bytes / block);
     g->N = N; g->R = R; g->C = C; g->PH = PH; g->PW = PW; g->sr = sr;
     g->ny = PH * sr; g->nx = PW * sr;
     g->SX = best_sx; g->WX = best_wx; g->K = best_k;
@@ -831,7 +910,7 @@ bool stream_geometry(int levels, const float* const* bottoms, const int* heights
     lay->tmp_off = off; off = align_up_sz(off + (size_t)g->max_entries * 16, 256);
     lay->tmpcnt_off = off; off = align_up_sz(off + (size_t)R * 4, 256);
     lay->ws_bytes = off;
-    *smem_bytes = (unsigned)(g->K + 1) * (unsigned)g->row_bytes + fixed;
+    *smem_bytes = kBarBytes + tail_bytes + 128;
     return true;
 }
 
@@ -910,10 +989,20 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
     const long long cap = (long long)per_sm * sm_count;
     const int prep_grid = (int)(R < cap ? R : cap);
     const int n16 = (int)(lay.zero_bytes / 16);
+    // the main kernel has a grid barrier too: one CTA per SM must be resident at its shared-memory size
+    const int m = (g.SX - 1) / 32;
+#define B200_STREAM_OCC(SRV, MV) err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, roi_align_stream_fwd<SRV, MV>, kStreamThreads, smem)
+#define B200_STREAM_OCC_M(SRV) if (m == 1) B200_STREAM_OCC(SRV, 1); else if (m == 2) B200_STREAM_OCC(SRV, 2); else B200_STREAM_OCC(SRV, 3)
+    if (sr == 1) { B200_STREAM_OCC_M(1); }
+    else         { B200_STREAM_OCC_M(2); }
+#undef B200_STREAM_OCC_M
+#undef B200_STREAM_OCC
+    if (err != cudaSuccess || (long long)per_sm * sm_count < g.pieces) { (void)cudaGetLastError(); return kPathDeclined; }
 
     StreamArgs a;
     a.ytab = ws.ytab; a.xtab = ws.xtab; a.entries = ws.entries; a.rowptr = ws.rowptr; a.maxend = ws.maxend;
-    a.piece_start = ws.piece_start; a.out = top; a.row_map = row_map;
+    a.piece_start = ws.piece_start; a.out = top; a.row_map = row_map; a.ticket = ws.ticket + 1;
+    a.R = R; a.tail_rows = g.tail_rows;
     a.C = C; a.G = g.G; a.K = g.K; a.WX = g.WX; a.PH = PH; a.PW = PW; a.ny = g.ny; a.nx = g.nx; a.L = g.L; a.Q = g.Q;
     for (int l = 0; l < kMaxLevels; ++l) a.lv[l] = g.lv[l];
     for (int c = 0; c <= kMaxCols; ++c) a.colstart[c] = g.colstart[c];
@@ -938,7 +1027,6 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
     cfg.gridDim = dim3((unsigned)g.pieces);
     cfg.blockDim = dim3(kStreamThreads);
     cfg.dynamicSmemBytes = smem;
-    const int m = (g.SX - 1) / 32;
 #define B200_STREAM_LAUNCH(SRV, MV) err = cudaLaunchKernelEx(&cfg, roi_align_stream_fwd<SRV, MV>, a)
 #define B200_STREAM_LAUNCH_M(SRV) if (m == 1) B200_STREAM_LAUNCH(SRV, 1); else if (m == 2) B200_STREAM_LAUNCH(SRV, 2); else B200_STREAM_LAUNCH(SRV, 3)
     if (sr == 1) { B200_STREAM_LAUNCH_M(1); }

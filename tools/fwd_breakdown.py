@@ -7,8 +7,9 @@ calls alone captured into one CUDA graph, replayed once to warm up and once unde
 Every call is cut out of the trace as the device operations (kernels and memsets) up to and including the main kernel;
 reported per operation: mean device time and the mean gap to the previous operation of the same call (negative when
 the two overlap, e.g. under programmatic dependent launch); per call: the time from its first operation's start to the
-main kernel's start ("before_main_us") and to its end ("call_us").  The card's name and power limit are read in the
-same run.  Times taken under the profiler: use them for the split, not as a bench value.
+main kernel's start ("before_main_us") and to its end ("call_us").  On the stream path the main kernel includes its tail,
+the in-place transpose of the output rows after a grid barrier (tools/stream_probe.py splits the two).  The card's name and
+power limit are read in the same run.  Times taken under the profiler: use them for the split, not as a bench value.
 """
 import argparse
 import collections

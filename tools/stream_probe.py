@@ -8,14 +8,18 @@ small shared library with nvcc (same flags as the library) and runs clear -> pre
 CUDA graph with rotating input sets as bench.py and tools/fwd_breakdown.py run them.  Every warp of every CTA writes one record
 of the last call:
 
-  CTA      globaltimer after griddepcontrol.wait and at the warp's end (CTA time = latest warp end - start)
+  CTA      globaltimer after griddepcontrol.wait, at the warp's end of the fragment loop, after the grid barrier and at the
+           end of the tail (the in-place transpose of the output rows)
   producer clock64 cycles blocked in mbar_wait(empty) -- the ring full, consumers holding slots; rows of the stream
   consumer clock64 cycles blocked on rows it only passes through (acquire_to before a fragment's key and at an item's tail),
-           blocked on the rows of a fragment (acquire_to(end)), in the bin loop, in the flush; fragments and bins it computed
+           blocked on the rows of a fragment (acquire_to(end)), in the bin loop (its output stores included); fragments and
+           bins it computed
 
-Cycle shares are per warp (its own clock64 lifetime), averaged over the warps of a class; the per-CTA columns use globaltimer.
-The stamps cost a few instructions per row and per fragment: compare the probed kernel's span with the uninstrumented one
-(tools/fwd_breakdown.py) before reading absolute numbers from it.  The card's name and power limit are read in the same run.
+"main_loop" is the span from the first CTA's start to the last warp's end of the fragment loop; "tail" the span from there
+to the last warp's end of the transpose (grid barrier included).  Cycle shares are per warp (its own clock64 lifetime up to the
+end of the fragment loop), averaged over the warps of a class; the per-CTA columns use globaltimer.  The stamps cost a few
+instructions per row and per fragment: compare the probed kernel's span with the uninstrumented one (tools/fwd_breakdown.py)
+before reading absolute numbers from it.  The card's name and power limit are read in the same run.
 """
 import argparse
 import ctypes
@@ -31,48 +35,58 @@ sys.path.insert(0, ROOT)
 
 from detectron.pytorch_b200 import build as B  # noqa: E402
 
-NREC = 12                                                     # u64 per warp record
+NREC = 14                                                     # u64 per warp record
 WARPS = 20                                                    # 16 consumer + 4 producer warps per CTA
 
 # (anchor, replacement): the replacement keeps the anchor text and adds the stamps around it
 PATCHES = [
     ("__device__ u64* g_stream_dead = nullptr;\n",
      "__device__ u64* g_stream_dead = nullptr;\n"
-     "__device__ u64* g_probe = nullptr;                         // [CTA][20 warps][12] records of the last call\n"
+     "__device__ u64* g_probe = nullptr;                         // [CTA][20 warps][14] records of the last call\n"
      "__device__ __forceinline__ u64 probe_gtime() { u64 t; asm volatile(\"mov.u64 %0, %globaltimer;\" : \"=l\"(t)); return t; }\n"),
-    ("    asm volatile(\"ld.volatile.global.s32 %0, [%1];\" : \"=r\"(L1) : \"l\"(a.piece_start + blockIdx.x + 1) : \"memory\");\n",
-     "    asm volatile(\"ld.volatile.global.s32 %0, [%1];\" : \"=r\"(L1) : \"l\"(a.piece_start + blockIdx.x + 1) : \"memory\");\n"
+    ("    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;\n\n    if (warp >= kConsumerWarps) {\n",
+     "    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;\n"
      "    const u64 pr_g0 = probe_gtime();\n"
      "    const long long pr_c0 = clock64();\n"
-     "    long long pr_w0 = 0, pr_w1 = 0, pr_comp = 0, pr_bin = 0;\n"
+     "    long long pr_w0 = 0, pr_w1 = 0, pr_comp = 0;\n"
      "    unsigned pr_n0 = 0, pr_n1 = 0, pr_n2 = 0;\n"
      "    auto pr_write = [&]() {\n"
      "        if (g_probe == nullptr || lane != 0) return;\n"
-     "        u64* rec = g_probe + ((size_t)blockIdx.x * 20 + warp) * 12;\n"
+     "        u64* rec = g_probe + ((size_t)blockIdx.x * 20 + warp) * 14;\n"
      "        rec[0] = pr_g0; rec[1] = probe_gtime(); rec[2] = (u64)(clock64() - pr_c0);\n"
      "        rec[3] = (u64)pr_w0; rec[4] = (u64)pr_w1; rec[5] = (u64)pr_comp;\n"
-     "        rec[6] = pr_n0; rec[7] = pr_n1; rec[8] = pr_n2; rec[9] = (u64)(L1 - L0); rec[10] = (u64)pr_bin; rec[11] = 1;\n"
-     "    };\n"),
+     "        rec[6] = pr_n0; rec[7] = pr_n1; rec[8] = pr_n2; rec[9] = (u64)(L1 - L0); rec[11] = 1;\n"
+     "    };\n\n"
+     "    if (warp >= kConsumerWarps) {\n"),
     # producer: blocked on a free slot; rows staged / rows of the stream
     ("                mbar_wait(empty, (ephase >> slot) & 1u, 0x1000u + (unsigned)y);\n",
      "                { const long long pc = clock64(); mbar_wait(empty, (ephase >> slot) & 1u, 0x1000u + (unsigned)y); pr_w0 += clock64() - pc; }\n"
      "                ++pr_n1;\n"),
     ("        }\n        return;\n    }\n",
      "        }\n        pr_write();\n        return;\n    }\n"),
-    # consumer: pass-through waits, fragment waits, compute
+    # consumer: pass-through waits, fragment waits, bin loop (stores included)
     ("                acquire_to(acq + 1, 0x2000u);\n",
      "                { const long long pc = clock64(); acquire_to(acq + 1, 0x2000u); pr_w0 += clock64() - pc; }\n"),
     ("            acquire_to(end, 0x2800u);                           // rows [key, end) must be resident\n",
      "            { const long long pc = clock64(); acquire_to(end, 0x2800u); pr_w1 += clock64() - pc; }\n"
      "            const long long pr_cc = clock64(); ++pr_n0; pr_n1 += npw;\n"),
-    ("            __syncwarp();\n            // flush: lanes",
-     "            __syncwarp();\n            pr_bin += clock64() - pr_cc;\n            // flush: lanes"),
-    ("            __syncwarp();\n            e = e_next;\n",
-     "            __syncwarp();\n            pr_comp += clock64() - pr_cc;\n            e = e_next;\n"),
+    ("            __syncwarp();                                       // the table buffer is rewritten for the next fragment\n",
+     "            __syncwarp();                                       // the table buffer is rewritten for the next fragment\n"
+     "            pr_comp += clock64() - pr_cc;\n"),
     ("            acquire_to(acq + 1, 0x3000u);\n",
      "            { const long long pc = clock64(); acquire_to(acq + 1, 0x3000u); pr_w0 += clock64() - pc; }\n"),
     ("            release_to(acq);\n        }\n        __syncwarp();\n    }\n}\n",
      "            release_to(acq);\n        }\n        __syncwarp();\n        ++pr_n2;\n    }\n    pr_write();\n}\n"),
+    # tail: after the grid barrier, and at the end of the transpose
+    ("    prepass::grid_barrier(a.ticket);\n",
+     "    prepass::grid_barrier(a.ticket);\n"
+     "    const u64 pr_t1 = probe_gtime();\n"),
+    ("    else transpose_rows<1>(a, blocks);\n}\n",
+     "    else transpose_rows<1>(a, blocks);\n"
+     "    if (g_probe != nullptr && (threadIdx.x & 31) == 0) {\n"
+     "        u64* rec = g_probe + ((size_t)blockIdx.x * 20 + (threadIdx.x >> 5)) * 14;\n"
+     "        rec[12] = pr_t1; rec[13] = probe_gtime();\n"
+     "    }\n}\n"),
 ]
 
 ENTRY = r"""
@@ -128,11 +142,11 @@ def card_info():
 
 
 def summarize(rec, ctas):
-    """rec: [ctas][20][12] u64 of one call -> the breakdown table."""
+    """rec: [ctas][20][14] u64 of one call -> the breakdown table."""
     med = statistics.median
     t0 = min(int(rec[c][w][0]) for c in range(ctas) for w in range(WARPS))
     cta_start, cta_end, cta_rows, cta_frags, cta_bins = [], [], [], [], []
-    prod_wait, cons_pass, cons_frag, cons_comp, cons_bin = [], [], [], [], []
+    prod_wait, cons_pass, cons_frag, cons_comp = [], [], [], []
     for c in range(ctas):
         cta_start.append((int(rec[c][0][0]) - t0) / 1e3)
         cta_end.append((max(int(rec[c][w][1]) for w in range(WARPS)) - t0) / 1e3)
@@ -147,12 +161,17 @@ def summarize(rec, ctas):
                 cons_pass.append(int(rec[c][w][3]) / life)
                 cons_frag.append(int(rec[c][w][4]) / life)
                 cons_comp.append(int(rec[c][w][5]) / life)
-                cons_bin.append(int(rec[c][w][10]) / life)
     cta_time = [e - s for s, e in zip(cta_start, cta_end)]
+    main_end = max(cta_end)
+    barrier_out = (max(int(rec[c][w][12]) for c in range(ctas) for w in range(WARPS)) - t0) / 1e3
+    tail_end = (max(int(rec[c][w][13]) for c in range(ctas) for w in range(WARPS)) - t0) / 1e3
     mean = lambda v: sum(v) / len(v)
     order = sorted(range(ctas), key=lambda c: cta_time[c])
     return {
-        "span_us": max(cta_end) - min(cta_start),
+        "span_us": tail_end - min(cta_start),
+        "main_loop_span_us": main_end - min(cta_start),
+        "tail_span_us": tail_end - main_end,
+        "last_barrier_exit_after_main_loop_us": barrier_out - main_end,
         "cta_time_us": {"max": max(cta_time), "median": med(cta_time), "min": min(cta_time)},
         "cta_start_us": {"max": max(cta_start), "median": med(cta_start)},
         "rows_per_cta": {"max": max(cta_rows), "median": med(cta_rows), "min": min(cta_rows)},
@@ -162,7 +181,7 @@ def summarize(rec, ctas):
         "fastest_ctas": [{"cta": c, "us": cta_time[c], "rows": cta_rows[c], "frags": cta_frags[c], "bins": cta_bins[c]} for c in order[:4]],
         "producer_share_blocked_on_empty": mean(prod_wait),
         "consumer_share": {"blocked_pass_through": mean(cons_pass), "blocked_fragment_rows": mean(cons_frag),
-                           "bin_loop": mean(cons_bin), "flush": mean(cons_comp) - mean(cons_bin),
+                           "bin_loop_with_stores": mean(cons_comp),
                            "other": 1.0 - mean(cons_pass) - mean(cons_frag) - mean(cons_comp)},
     }
 
