@@ -13,7 +13,7 @@ or, to make an unmodified checkout of the reference pick these up under ITS impo
 __version__ = "0.1.0"
 
 
-def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False, voc=False):
+def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False, voc=False, losses=False):
     """Register this package's op modules in sys.modules under the reference's import paths.
 
     After this, `from modeling.roi_xfrom.roi_align.functions.roi_align import RoIAlignFunction`
@@ -36,6 +36,11 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
     `voc=True` re-points the reference's `datasets.voc_eval.voc_eval` (lib/datasets/voc_eval.py:86-223) and the copy of that name
     bound in `datasets.voc_dataset_evaluator` at the device evaluation (`datasets/voc_eval.py` here), which reads and writes the
     annotation cache in binary mode, so the reference's VOC evaluator runs on Python 3; both reference modules must be importable.
+    `losses=True` re-points the reference's training losses at the device ones that take the device target blobs:
+    `modeling.fast_rcnn_heads.fast_rcnn_losses`, `modeling.rpn_heads.single_scale_rpn_losses` (which the reference's
+    generic_rpn_losses calls), `modeling.FPN.fpn_rpn_losses`, `modeling.mask_rcnn_heads.mask_rcnn_losses` and
+    `modeling.keypoint_rcnn_heads.keypoint_losses` (`modeling/` here), each reading its reference module's `cfg` at call time;
+    those reference modules must be importable.
     """
     import importlib
     import sys
@@ -92,4 +97,23 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
         for name in ("datasets.voc_eval", "datasets.voc_dataset_evaluator"):      # the reference's modules
             importlib.import_module(name).voc_eval = ours_voc
             installed.append(name + ".voc_eval")
+    if losses:
+        ours = __name__ + ".modeling."
+        ref = importlib.import_module("modeling.fast_rcnn_heads")                  # the reference's modules
+        ref.fast_rcnn_losses = importlib.import_module(ours + "fast_rcnn_heads").fast_rcnn_losses
+        ref_rpn = importlib.import_module("modeling.rpn_heads")
+        ours_rpn = importlib.import_module(ours + "rpn_heads").single_scale_rpn_losses
+        ref_rpn.single_scale_rpn_losses = lambda *a, **k: ours_rpn(*a, cfg=ref_rpn.cfg, **k)
+        ref_fpn = importlib.import_module("modeling.FPN")
+        ours_fpn = importlib.import_module(ours + "FPN").fpn_rpn_losses
+        ref_fpn.fpn_rpn_losses = lambda **k: ours_fpn(cfg=ref_fpn.cfg, **k)
+        ref_mask = importlib.import_module("modeling.mask_rcnn_heads")
+        ours_mask = importlib.import_module(ours + "mask_rcnn_heads").mask_rcnn_losses
+        ref_mask.mask_rcnn_losses = lambda masks_pred, masks_int32: ours_mask(masks_pred, masks_int32, cfg=ref_mask.cfg)
+        ref_kp = importlib.import_module("modeling.keypoint_rcnn_heads")
+        ours_kp_loss = importlib.import_module(ours + "keypoint_rcnn_heads").keypoint_losses
+        ref_kp.keypoint_losses = lambda kps_pred, loc, w, norm=None: ours_kp_loss(kps_pred, loc, w, norm, cfg=ref_kp.cfg)
+        installed += ["modeling.fast_rcnn_heads.fast_rcnn_losses", "modeling.rpn_heads.single_scale_rpn_losses",
+                      "modeling.FPN.fpn_rpn_losses", "modeling.mask_rcnn_heads.mask_rcnn_losses",
+                      "modeling.keypoint_rcnn_heads.keypoint_losses"]
     return installed

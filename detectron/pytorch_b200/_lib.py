@@ -163,6 +163,19 @@ _SIGNATURES = {
     #  area_range (host), thresholds, workspace, workspace_bytes, overlap, excluded, error, counts, stream)
     "b200_box_proposal_match": (ctypes.c_int, [ctypes.c_int] * 6 + [ctypes.c_void_p] * 9 + [ctypes.c_size_t] + [ctypes.c_void_p] * 4 +
                                 [_stream_t]),
+    "b200_loss_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int]),
+    # (num_levels, levels_host, activation, fixed_divisor, workspace, workspace_bytes, losses_out, divisor_out, stream)
+    "b200_rpn_loss_forward": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_void_p, ctypes.c_size_t,
+                                             ctypes.c_void_p, ctypes.c_void_p, _stream_t]),
+    # (num_levels, levels_host, activation, grad_losses, divisor, stream)
+    "b200_rpn_loss_backward": (ctypes.c_int, [ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_void_p, _stream_t]),
+    # (R, C, B, cls_score, bbox_pred, labels, label_is_int64, targets, inside, outside, workspace, workspace_bytes, losses_out,
+    #  accuracy_out, stream)
+    "b200_fast_rcnn_loss_forward": (ctypes.c_int, [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 4 +
+                                    [ctypes.c_size_t] + [ctypes.c_void_p] * 2 + [_stream_t]),
+    # (R, C, B, cls_score, bbox_pred, labels, label_is_int64, targets, inside, outside, grad_losses, cls_grad_out, bbox_grad_out, stream)
+    "b200_fast_rcnn_loss_backward": (ctypes.c_int, [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 6 +
+                                     [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

@@ -109,6 +109,13 @@ int keypoint_candidates(const float*, const float*, const int*, int, const int*,
 int keypoint_targets(const float*, const int*, int, const int*, const int*, const int*, const int*, const int*, int, int, const int*,
                      const int*, const int*, const int*, const float*, const float*, float*, int*, float*, cudaStream_t);
 int image_blob(const unsigned char*, const b200_image_blob_desc*, int, const float*, int, int, float*, cudaStream_t);
+size_t loss_workspace_bytes(int);
+int rpn_loss_forward(int, const b200_rpn_loss_level*, int, float, void*, size_t, float*, float*, cudaStream_t);
+int rpn_loss_backward(int, const b200_rpn_loss_level*, int, const float*, const float*, cudaStream_t);
+int fast_rcnn_loss_forward(int, int, int, const float*, const float*, const void*, int, const float*, const float*, const float*, void*,
+                           size_t, float*, float*, cudaStream_t);
+int fast_rcnn_loss_backward(int, int, int, const float*, const float*, const void*, int, const float*, const float*, const float*,
+                            const float*, float*, float*, cudaStream_t);
 
 // B200_ROI_ALIGN_PATH=generic|tiled|stream|auto (default auto) -- test/benchmark override of the forward dispatch
 //   0 auto: streaming-strip path -> quad-strip path -> tiled path -> generic, each when it applies.  On H100 the streaming
@@ -795,6 +802,37 @@ int b200_box_proposal_match(int num_images, int num_props, int num_gt, int num_a
     return box_proposal_match(num_images, num_props, num_gt, num_areas, num_limits, num_thresholds, prop_box_dev, prop_begin_dev, gt_box_dev,
                               gt_area_dev, gt_begin_dev, prop_count_dev, area_range_host, thresholds_dev, workspace, workspace_bytes,
                               overlap_out_dev, excluded_out_dev, error_out_dev, count_out_dev, (cudaStream_t)stream);
+}
+
+size_t b200_loss_workspace_bytes(int num_levels) { return loss_workspace_bytes(num_levels); }
+
+int b200_rpn_loss_forward(int num_levels, const b200_rpn_loss_level* levels_host, int activation, float fixed_divisor, void* workspace,
+                          size_t workspace_bytes, float* losses_out_dev, float* divisor_out_dev, b200_stream_t stream) {
+    return rpn_loss_forward(num_levels, levels_host, activation, fixed_divisor, workspace, workspace_bytes, losses_out_dev, divisor_out_dev,
+                            (cudaStream_t)stream);
+}
+
+int b200_rpn_loss_backward(int num_levels, const b200_rpn_loss_level* levels_host, int activation, const float* grad_losses_dev,
+                           const float* divisor_dev, b200_stream_t stream) {
+    return rpn_loss_backward(num_levels, levels_host, activation, grad_losses_dev, divisor_dev, (cudaStream_t)stream);
+}
+
+int b200_fast_rcnn_loss_forward(int num_rois, int num_classes, int bbox_width, const float* cls_score_dev, const float* bbox_pred_dev,
+                                const void* labels_dev, int label_is_int64, const float* bbox_targets_dev, const float* inside_weights_dev,
+                                const float* outside_weights_dev, void* workspace, size_t workspace_bytes, float* losses_out_dev,
+                                float* accuracy_out_dev, b200_stream_t stream) {
+    return fast_rcnn_loss_forward(num_rois, num_classes, bbox_width, cls_score_dev, bbox_pred_dev, labels_dev, label_is_int64, bbox_targets_dev,
+                                  inside_weights_dev, outside_weights_dev, workspace, workspace_bytes, losses_out_dev, accuracy_out_dev,
+                                  (cudaStream_t)stream);
+}
+
+int b200_fast_rcnn_loss_backward(int num_rois, int num_classes, int bbox_width, const float* cls_score_dev, const float* bbox_pred_dev,
+                                 const void* labels_dev, int label_is_int64, const float* bbox_targets_dev, const float* inside_weights_dev,
+                                 const float* outside_weights_dev, const float* grad_losses_dev, float* cls_grad_out_dev,
+                                 float* bbox_grad_out_dev, b200_stream_t stream) {
+    return fast_rcnn_loss_backward(num_rois, num_classes, bbox_width, cls_score_dev, bbox_pred_dev, labels_dev, label_is_int64, bbox_targets_dev,
+                                   inside_weights_dev, outside_weights_dev, grad_losses_dev, cls_grad_out_dev, bbox_grad_out_dev,
+                                   (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -7,6 +7,8 @@ These are what the reference-shaped shims in `model/` and `modeling/` delegate t
   * allocates outputs with torch.empty (the kernels define every output element; the reference
     needed `.zero_()` passes, functions/roi_align.py:23,39-40).
 """
+import ctypes
+
 import numpy as np
 import torch
 from torch.autograd import Function
@@ -1219,3 +1221,215 @@ def box_proposal_match_raw(prop_box, prop_begin, gt_box, gt_area, gt_begin, prop
                                                ws.numel(), ptr(overlap), ptr(excluded), error.data_ptr(), ptr(counts), _stream()),
                    "b200_box_proposal_match")
     return overlap, excluded.bool(), error.bool(), counts
+
+
+# ------------------------------------------------------------------------------------------------
+# Training losses: RPN (single-scale and FPN) and Fast R-CNN, forward and backward in one launch each
+# ------------------------------------------------------------------------------------------------
+class _RpnLossLevel(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("cls_logits", "bbox_pred", "labels_wide", "bbox_targets_wide", "bbox_inside_wide",
+                                               "bbox_outside_wide", "cls_grad", "bbox_grad")] + \
+               [(n, ctypes.c_int) for n in ("num_images", "num_anchors", "cls_channels", "h", "w", "hb", "wb", "label_h", "label_w",
+                                            "target_h", "target_w")]
+
+
+RPN_LOSS_MAX_LEVELS = 8
+_loss_workspaces = {}
+
+
+def _loss_workspace(dev, num_levels):
+    """The zero-filled workspace of the loss kernels, one per (device, stream): the kernels leave it zero after every call, and
+    calls on one stream never overlap."""
+    key = (dev.index, _stream())
+    need = int(_lib.load().b200_loss_workspace_bytes(num_levels))
+    ws = _loss_workspaces.get(key)
+    if ws is None or ws.numel() < need:
+        ws = torch.zeros((max(need, int(_lib.load().b200_loss_workspace_bytes(RPN_LOSS_MAX_LEVELS))),), dtype=torch.uint8, device=dev)
+        _loss_workspaces[key] = ws
+    return ws
+
+
+def _target(x, dtype, dev, name):
+    """A target blob on `dev` in `dtype` (numpy arrays are uploaded); predictions are never converted."""
+    t = torch.as_tensor(x)
+    if t.device != dev or t.dtype != dtype:
+        t = t.to(device=dev, dtype=dtype)
+    return t.contiguous()
+
+
+def _rpn_levels_desc(cls, bbox, targets, softmax, grads=None):
+    descs = (_RpnLossLevel * len(cls))()
+    for l, (c, b, (lab, tg, wi, wo)) in enumerate(zip(cls, bbox, targets)):
+        d = descs[l]
+        d.cls_logits, d.bbox_pred, d.labels_wide = c.data_ptr(), b.data_ptr(), lab.data_ptr()
+        d.bbox_targets_wide, d.bbox_inside_wide, d.bbox_outside_wide = tg.data_ptr(), wi.data_ptr(), wo.data_ptr()
+        if grads is not None:
+            d.cls_grad, d.bbox_grad = grads[0][l].data_ptr(), grads[1][l].data_ptr()
+        d.num_images, d.cls_channels, d.h, d.w = c.shape
+        d.num_anchors = c.shape[1] // 2 if softmax else c.shape[1]
+        d.hb, d.wb = b.shape[2], b.shape[3]
+        d.label_h, d.label_w = lab.shape[2], lab.shape[3]
+        d.target_h, d.target_w = tg.shape[2], tg.shape[3]
+    return descs
+
+
+class RpnLossFunction(Function):
+    """losses (L, 2) = per level (loss_cls, loss_bbox), and the per-level cls divisor (not differentiable).
+    apply(L, softmax, fixed_divisor, *cls_logits, *bbox_pred, *(labels, targets, inside, outside) per level)."""
+
+    @staticmethod
+    def forward(ctx, L, softmax, fixed_divisor, *tensors):
+        cls, bbox = tensors[:L], tensors[L:2 * L]
+        targets = [tensors[2 * L + 4 * l:2 * L + 4 * l + 4] for l in range(L)]
+        dev = cls[0].device
+        descs = _rpn_levels_desc(cls, bbox, targets, softmax)
+        losses = torch.empty((L, 2), dtype=torch.float32, device=dev)
+        divisor = torch.empty((L,), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            ws = _loss_workspace(dev, L)
+            _lib.check(_lib.load().b200_rpn_loss_forward(L, ctypes.cast(descs, ctypes.c_void_p), int(softmax), float(fixed_divisor),
+                                                         ws.data_ptr(), ws.numel(), losses.data_ptr(), divisor.data_ptr(), _stream()),
+                       "b200_rpn_loss_forward")
+        ctx.mark_non_differentiable(divisor)
+        ctx.L, ctx.softmax = L, softmax
+        ctx.save_for_backward(divisor, *tensors)
+        return losses, divisor
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_losses, _grad_divisor):
+        divisor, *tensors = ctx.saved_tensors
+        L = ctx.L
+        cls, bbox = tensors[:L], tensors[L:2 * L]
+        targets = [tensors[2 * L + 4 * l:2 * L + 4 * l + 4] for l in range(L)]
+        grads = ([torch.empty_like(c) for c in cls], [torch.empty_like(b) for b in bbox])
+        descs = _rpn_levels_desc(cls, bbox, targets, ctx.softmax, grads)
+        g = grad_losses.to(torch.float32).contiguous()
+        with torch.cuda.device(g.device):
+            _lib.check(_lib.load().b200_rpn_loss_backward(L, ctypes.cast(descs, ctypes.c_void_p), int(ctx.softmax), g.data_ptr(),
+                                                          divisor.data_ptr(), _stream()), "b200_rpn_loss_backward")
+        return (None, None, None) + tuple(grads[0]) + tuple(grads[1]) + (None,) * (4 * L)
+
+
+def _shape4(t, name):
+    if t.dim() != 4:
+        raise ValueError("%s must be 4-D (N, C, H, W), got %s" % (name, tuple(t.shape)))
+    return tuple(t.shape)
+
+
+def rpn_losses(levels, softmax=False, fixed_divisor=0.0):
+    """The RPN losses of every level in one launch (and one for the backward).  levels: per level (rpn_cls_logits, rpn_bbox_pred,
+    labels_int32_wide, bbox_targets_wide, bbox_inside_weights_wide, bbox_outside_weights_wide): float32 CUDA predictions
+    (N, A or 2A (softmax), h, w) and (N, 4A, hb, wb); the wide target blobs (N, A, >= h, >= w) and (N, 4A, >= hb, >= wb), tensors or
+    numpy arrays, read in their [:h, :w] window in place.  fixed_divisor > 0 (sigmoid only) divides every level's cls sum by it
+    instead of by its count of labels >= 0.  Returns the (L, 2) tensor of (loss_cls, loss_bbox) per level."""
+    L = len(levels)
+    if not 1 <= L <= RPN_LOSS_MAX_LEVELS:
+        raise ValueError("rpn_losses takes 1 .. %d levels, got %d" % (RPN_LOSS_MAX_LEVELS, L))
+    cls, bbox, targets = [], [], []
+    dev = None
+    for l, lv in enumerate(levels):
+        if len(lv) != 6:
+            raise ValueError("level %d: expected (cls_logits, bbox_pred, labels, targets, inside, outside)" % l)
+        c, b = lv[0], lv[1]
+        _need_cuda_f32(c, "rpn_cls_logits"); _need_cuda_f32(b, "rpn_bbox_pred")
+        dev = c.device if dev is None else dev
+        if c.device != dev or b.device != dev:
+            raise ValueError("level %d: every prediction must be on %s" % (l, dev))
+        N, Cc, h, w = _shape4(c, "rpn_cls_logits")
+        Nb, Cb, hb, wb = _shape4(b, "rpn_bbox_pred")
+        if softmax and Cc % 2:
+            raise ValueError("level %d: softmax rpn_cls_logits needs 2A channels, got %d" % (l, Cc))
+        A = Cc // 2 if softmax else Cc
+        if Nb != N or Cb != 4 * A:
+            raise ValueError("level %d: rpn_bbox_pred %s does not match rpn_cls_logits %s (expected (%d, %d, h, w))"
+                             % (l, (Nb, Cb, hb, wb), (N, Cc, h, w), N, 4 * A))
+        lab = _target(lv[2], torch.int32, dev, "rpn_labels_int32_wide")
+        t3 = [_target(x, torch.float32, dev, "rpn_bbox_*_wide") for x in lv[3:]]
+        Nl, Al, Hl, Wl = _shape4(lab, "rpn_labels_int32_wide")
+        if Nl != N or Al != A or Hl < h or Wl < w:
+            raise ValueError("level %d: rpn_labels_int32_wide %s cannot be narrowed to (%d, %d, %d, %d)" % (l, (Nl, Al, Hl, Wl), N, A, h, w))
+        ts = _shape4(t3[0], "rpn_bbox_targets_wide")
+        if any(tuple(x.shape) != ts for x in t3) or ts[0] != N or ts[1] != 4 * A or ts[2] < hb or ts[3] < wb:
+            raise ValueError("level %d: the bbox target / weight blobs %s cannot be narrowed to (%d, %d, %d, %d)"
+                             % (l, [tuple(x.shape) for x in t3], N, 4 * A, hb, wb))
+        if N * Cc * h * w >= 2 ** 31 or N * 4 * A * hb * wb >= 2 ** 31:
+            raise ValueError("level %d: more than 2^31 - 1 prediction elements" % l)
+        cls.append(c.contiguous()); bbox.append(b.contiguous())
+        targets += [lab] + t3
+    losses, _ = RpnLossFunction.apply(L, bool(softmax), float(fixed_divisor), *cls, *bbox, *targets)
+    return losses
+
+
+class FastRcnnLossFunction(Function):
+    """apply(cls_score, bbox_pred, labels, targets, inside, outside) -> (losses (2,) = (loss_cls, loss_bbox), accuracy ())."""
+
+    @staticmethod
+    def forward(ctx, cls_score, bbox_pred, labels, targets, inside, outside):
+        dev = cls_score.device
+        R, C = cls_score.shape
+        B = bbox_pred.shape[1]
+        losses = torch.empty((2,), dtype=torch.float32, device=dev)
+        accuracy = torch.empty((), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            ws = _loss_workspace(dev, 1)
+            _lib.check(_lib.load().b200_fast_rcnn_loss_forward(R, C, B, cls_score.data_ptr(), bbox_pred.data_ptr(), labels.data_ptr(),
+                                                               int(labels.dtype == torch.int64), targets.data_ptr(), inside.data_ptr(),
+                                                               outside.data_ptr(), ws.data_ptr(), ws.numel(), losses.data_ptr(),
+                                                               accuracy.data_ptr(), _stream()), "b200_fast_rcnn_loss_forward")
+        ctx.mark_non_differentiable(accuracy)
+        ctx.save_for_backward(cls_score, bbox_pred, labels, targets, inside, outside)
+        return losses, accuracy
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_losses, _grad_accuracy):
+        cls_score, bbox_pred, labels, targets, inside, outside = ctx.saved_tensors
+        R, C = cls_score.shape
+        B = bbox_pred.shape[1]
+        d_cls = torch.empty_like(cls_score) if ctx.needs_input_grad[0] else None
+        d_bbox = torch.empty_like(bbox_pred) if ctx.needs_input_grad[1] else None
+        if d_cls is None and d_bbox is None:
+            return None, None, None, None, None, None
+        g = grad_losses.to(torch.float32).contiguous()
+        with torch.cuda.device(g.device):
+            _lib.check(_lib.load().b200_fast_rcnn_loss_backward(R, C, B, cls_score.data_ptr(), bbox_pred.data_ptr(), labels.data_ptr(),
+                                                                int(labels.dtype == torch.int64), targets.data_ptr(), inside.data_ptr(),
+                                                                outside.data_ptr(), g.data_ptr(), d_cls.data_ptr() if d_cls is not None else None,
+                                                                d_bbox.data_ptr() if d_bbox is not None else None, _stream()),
+                       "b200_fast_rcnn_loss_backward")
+        return d_cls, d_bbox, None, None, None, None
+
+
+def fast_rcnn_losses(cls_score, bbox_pred, label_int32, bbox_targets, bbox_inside_weights, bbox_outside_weights):
+    """(loss_cls, loss_bbox, accuracy_cls) as 0-d CUDA tensors, in one launch (one more for the backward).  cls_score (R, C) and
+    bbox_pred (R, B) float32 CUDA; labels (R,) int32 / int64 and the three (R, B) blobs as tensors or numpy arrays (uploaded).
+    Host labels outside [0, C) raise ValueError; a device label outside [0, C) gives a NaN loss_cls."""
+    _need_cuda_f32(cls_score, "cls_score"); _need_cuda_f32(bbox_pred, "bbox_pred")
+    dev = cls_score.device
+    if bbox_pred.device != dev:
+        raise ValueError("cls_score and bbox_pred must be on the same device")
+    if (cls_score.dim() != 2 or bbox_pred.dim() != 2 or bbox_pred.shape[0] != cls_score.shape[0] or bbox_pred.shape[1] % 4
+            or bbox_pred.shape[1] == 0):
+        raise ValueError("cls_score must be (R, C) and bbox_pred (R, 4 C'), got %s and %s" % (tuple(cls_score.shape), tuple(bbox_pred.shape)))
+    R, C = cls_score.shape
+    if R == 0 or C == 0:
+        raise ValueError("fast_rcnn_losses needs at least one RoI and one class, got cls_score %s" % (tuple(cls_score.shape),))
+    if not torch.is_tensor(label_int32):
+        lab_h = np.asarray(label_int32)
+        if lab_h.size and (lab_h.min() < 0 or lab_h.max() >= C):
+            raise ValueError("label_int32 must lie in [0, %d), got [%d, %d]" % (C, lab_h.min(), lab_h.max()))
+    labels = torch.as_tensor(label_int32)
+    if labels.dtype not in (torch.int32, torch.int64):
+        raise ValueError("label_int32 must be int32 or int64, got %s" % labels.dtype)
+    labels = _target(labels, labels.dtype, dev, "label_int32").reshape(-1)
+    if labels.numel() != R:
+        raise ValueError("label_int32 has %d entries for %d RoIs" % (labels.numel(), R))
+    blobs = [_target(x, torch.float32, dev, n) for x, n in ((bbox_targets, "bbox_targets"), (bbox_inside_weights, "bbox_inside_weights"),
+                                                           (bbox_outside_weights, "bbox_outside_weights"))]
+    for t, n in zip(blobs, ("bbox_targets", "bbox_inside_weights", "bbox_outside_weights")):
+        if tuple(t.shape) != tuple(bbox_pred.shape):
+            raise ValueError("%s %s does not match bbox_pred %s" % (n, tuple(t.shape), tuple(bbox_pred.shape)))
+    losses, accuracy = FastRcnnLossFunction.apply(cls_score.contiguous(), bbox_pred.contiguous(), labels, *blobs)
+    loss_cls, loss_bbox = losses.unbind(0)
+    return loss_cls, loss_bbox, accuracy

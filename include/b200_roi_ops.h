@@ -568,6 +568,67 @@ B200_API int b200_box_proposal_match(int num_images, int num_props, int num_gt, 
                                      unsigned char* excluded_out_dev, unsigned char* error_out_dev, long long* count_out_dev,
                                      b200_stream_t stream);
 
+/* ---- Training losses: RPN (lib/modeling/rpn_heads.py:130-161, lib/modeling/FPN.py:422-466) and Fast R-CNN
+ *      (lib/modeling/fast_rcnn_heads.py:50-68), with net_utils.smooth_l1_loss (lib/utils/net.py:15-32) ---------------------
+ * Element terms use the reference expression's float32 operations in its order (no FMA contraction, no element skipped for a
+ * zero weight: a non-finite prediction under a zero weight gives NaN as `0 * NaN` does there).  Sums are taken in float64, per
+ * CTA and then over the CTAs in a fixed order; the last CTA finishes them (integer ticket), so the results are bit-identical
+ * from run to run and no call reads the host.
+ * workspace: b200_loss_workspace_bytes(num_levels) bytes (the Fast R-CNN loss: num_levels = 1).  It must be zero-filled
+ *   before its first use and is left zero by every completed forward call; calls that may run concurrently need separate
+ *   workspaces.  Small or missing: B200_ROI_EWORKSPACE.
+ *
+ * RPN, one descriptor per level (num_levels 1 .. B200_RPN_LOSS_MAX_LEVELS, HOST array):
+ *   cls_logits (N, cls_channels, h, w) with cls_channels = A (activation 0, sigmoid) or 2A (activation 1, softmax: the pair
+ *   (a, A + a) of image n, the reference's view(N, 2, A, h, w)); bbox_pred (N, 4A, hb, wb); labels_wide int32 (N, A, label_h,
+ *   label_w) and the three float32 blobs (N, 4A, target_h, target_w), read in their [:h, :w] / [:hb, :wb] window in place.
+ * b200_rpn_loss_forward  losses_out (num_levels, 2) = (loss_cls, loss_bbox) per level; divisor_out (num_levels,) the cls
+ *   divisor: fixed_divisor when > 0 with activation 0 (FPN: RPN_BATCH_SIZE_PER_IM * IMS_PER_BATCH), else the count of labels
+ *   >= 0 (sigmoid) or != -1 (softmax, ignore_index = -1); 0 / 0 gives NaN, as in the reference.  Sigmoid: sum of
+ *   BCE-with-logits(x, float(label)) * (label >= 0).  Softmax: sum of -log_softmax at the label; a label other than -1, 0, 1
+ *   adds NaN.  Box: smooth L1 with beta = 1/9 summed, / N.  One launch.
+ * b200_rpn_loss_backward  writes every element of each level's cls_grad (shape of cls_logits) and bbox_grad (shape of bbox_pred)
+ *   from grad_losses_dev (num_levels, 2) and the forward's divisor_dev.  One launch (none when every level is empty).
+ * Bad sizes (a wide blob smaller than its prediction, cls_channels not A / 2A) or null pointers: B200_ROI_EINVAL before any
+ * launch. */
+#define B200_RPN_LOSS_MAX_LEVELS 8
+typedef struct b200_rpn_loss_level {
+    const float* cls_logits;
+    const float* bbox_pred;
+    const int* labels_wide;
+    const float* bbox_targets_wide;
+    const float* bbox_inside_wide;
+    const float* bbox_outside_wide;
+    float* cls_grad;              /* backward only */
+    float* bbox_grad;             /* backward only */
+    int num_images, num_anchors, cls_channels;
+    int h, w, hb, wb;
+    int label_h, label_w, target_h, target_w;
+} b200_rpn_loss_level;
+
+B200_API size_t b200_loss_workspace_bytes(int num_levels);
+B200_API int b200_rpn_loss_forward(int num_levels, const b200_rpn_loss_level* levels_host, int activation, float fixed_divisor,
+                                   void* workspace, size_t workspace_bytes, float* losses_out_dev, float* divisor_out_dev,
+                                   b200_stream_t stream);
+B200_API int b200_rpn_loss_backward(int num_levels, const b200_rpn_loss_level* levels_host, int activation, const float* grad_losses_dev,
+                                    const float* divisor_dev, b200_stream_t stream);
+
+/* Fast R-CNN: cls_score (R, C), bbox_pred / bbox_targets / inside / outside weights (R, B), B = 4 C' >= 4, labels (R,)
+ * int32 or int64 (label_is_int64), R >= 1.
+ * b200_fast_rcnn_loss_forward  losses_out (2,) = (loss_cls = mean over R of -log_softmax(cls_score)[label], loss_bbox = smooth L1
+ *   with beta = 1 summed, / R); accuracy_out (1,) = mean of (argmax == label), argmax the first maximal index with NaN
+ *   maximal.  A label outside [0, C) is never used as an index: loss_cls is NaN and the row counts as a miss.  One launch.
+ * b200_fast_rcnn_loss_backward  cls_grad (R, C) = (softmax - onehot) * grad_losses[0] / R (a row with a label outside [0, C) is
+ *   NaN) and bbox_grad (R, B) from grad_losses_dev (2,); either output may be null (not computed).  One launch. */
+B200_API int b200_fast_rcnn_loss_forward(int num_rois, int num_classes, int bbox_width, const float* cls_score_dev, const float* bbox_pred_dev,
+                                         const void* labels_dev, int label_is_int64, const float* bbox_targets_dev,
+                                         const float* inside_weights_dev, const float* outside_weights_dev, void* workspace,
+                                         size_t workspace_bytes, float* losses_out_dev, float* accuracy_out_dev, b200_stream_t stream);
+B200_API int b200_fast_rcnn_loss_backward(int num_rois, int num_classes, int bbox_width, const float* cls_score_dev, const float* bbox_pred_dev,
+                                          const void* labels_dev, int label_is_int64, const float* bbox_targets_dev,
+                                          const float* inside_weights_dev, const float* outside_weights_dev, const float* grad_losses_dev,
+                                          float* cls_grad_out_dev, float* bbox_grad_out_dev, b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
