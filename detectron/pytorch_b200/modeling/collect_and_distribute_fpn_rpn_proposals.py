@@ -18,9 +18,9 @@ _add_multilevel_rois).  Here the same blobs are produced on the device with roi_
 random draws are inputs (`choices`), see there.  With MODEL.MASK_ON the mask blobs (mask_rois, roi_has_mask_int32,
 masks_int32 and the mask_rois FPN blobs) come from roi_data/mask_rcnn.py, and with MODEL.KEYPOINTS_ON the keypoint blobs
 (keypoint_rois, keypoint_locations_int32, keypoint_weights, keypoint_loss_normalizer and the keypoint_rois FPN blobs) from
-roi_data/keypoint_rcnn.py, on the device too.  The keypoint candidates see the reference's merged roidb: a proposal keeps the
-assignment assign_rois gives it (the same one the Fast R-CNN blobs use), a ground-truth row maps to itself with overlap 1,
-or -1 when it is a crowd object.
+roi_data/keypoint_rcnn.py, on the device too.  Every blob sees the reference's merged roidb (fast_rcnn.roidb_assignment): a
+proposal takes its best ground-truth box, crowd objects included; a ground-truth row maps to itself with overlap 1 and its own
+class, or overlap -1 and class 0 when the entry's 'is_crowd' marks it, so that no crowd row is ever sampled.
 """
 import numpy as np
 import torch
@@ -81,12 +81,12 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
     def forward(self, inputs, roidb=None, im_info=None, choices=None, train=None):
         """inputs: [rpn_rois_fpn<min> .. rpn_rois_fpn<max>, rpn_roi_probs_fpn<min> .. rpn_roi_probs_fpn<max>] tensors.
         Training (module in training mode): roidb = one dict per image with the ground truth ('boxes' (G, 4) unscaled,
-        'gt_classes' (G,); numpy or tensors), im_info = (N, 3) [height, width, scale]; `train` = the TRAIN / MODEL keys
-        (dict, or taken from `cfg`): BATCH_SIZE_PER_IM, FG_FRACTION, FG_THRESH, BG_THRESH_HI, BG_THRESH_LO, NUM_CLASSES,
-        BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG, and for Mask R-CNN MASK_ON, MRCNN_RESOLUTION (default 14), CLS_SPECIFIC_MASK
-        (default True), with the roidb entries' 'segms' and 'is_crowd'; for Keypoint R-CNN KEYPOINTS_ON, HEATMAP_SIZE,
-        NUM_KEYPOINTS, IMS_PER_BATCH (default 2), MIN_KEYPOINT_COUNT (default 20), with the roidb entries' 'gt_keypoints'
-        (G, 3, K) and 'is_crowd' (where crowd objects exist); choices = per image (fg_choice, bg_choice) or, with keypoints,
+        'gt_classes' (G,), 'is_crowd' (G,) where crowd objects exist; numpy or tensors), im_info = (N, 3) [height, width,
+        scale]; `train` = the TRAIN / MODEL keys (dict, or taken from `cfg`): BATCH_SIZE_PER_IM, FG_FRACTION, FG_THRESH,
+        BG_THRESH_HI, BG_THRESH_LO, NUM_CLASSES, BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG, and for Mask R-CNN MASK_ON,
+        MRCNN_RESOLUTION (default 14), CLS_SPECIFIC_MASK (default True), with the roidb entries' 'segms'; for Keypoint R-CNN
+        KEYPOINTS_ON, HEATMAP_SIZE, NUM_KEYPOINTS, IMS_PER_BATCH (default 2), MIN_KEYPOINT_COUNT (default 20), with the roidb
+        entries' 'gt_keypoints' (G, 3, K); choices = per image (fg_choice, bg_choice) or, with keypoints,
         (fg_choice, bg_choice, keypoint_choice), or None (device randperm)."""
         p = self._params()
         n = p["rpn_max"] - p["rpn_min"] + 1
@@ -122,27 +122,24 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
             gcls = torch.as_tensor(entry["gt_classes"]).to(device=dev, dtype=torch.int32).reshape(-1)
             keep_gt = gcls > 0
             gt, gcls = gt[keep_gt], gcls[keep_gt]
+            crowd = torch.as_tensor(entry["is_crowd"]).to(dev).reshape(-1)[keep_gt] if "is_crowd" in entry else None
             inv = (torch.ones((), dtype=torch.float32) / scales[i]).item()           # json_dataset.py:420: 1. / scales[i] in float32
             props = rois[rois[:, 0] == i][:, 1:5] * inv                              # add_proposals: back to image coordinates
             boxes = torch.cat([gt, props]).contiguous()
             ch = tuple(choices[i]) if choices is not None else (None, None)
             fg_c, bg_c = ch[0], ch[1]
-            assignment = FR.assign_rois(boxes, gt, gcls) if kp_on else None
+            assignment = FR.roidb_assignment(boxes, gt, gcls, crowd)
             b, nf = FR._sample_rois(boxes, gt, gcls, float(scales[i]), i, t["NUM_CLASSES"], t["BATCH_SIZE_PER_IM"], t["FG_FRACTION"],
                                     t["FG_THRESH"], t["BG_THRESH_HI"], t["BG_THRESH_LO"], t["BBOX_REG_WEIGHTS"],
                                     t["CLS_AGNOSTIC_BBOX_REG"], fg_c, bg_c, assignment)
             if kp_on:
-                # json_dataset.py:429-490 + :513-531 as add_keypoint_rcnn_blobs reads them: gt rows map to themselves (their roidb
-                # row) with overlap 1 (-1 for crowd), proposals to gt_inds[argmax] with their max IoU, -1 without overlap
-                cls_h = np.asarray(entry["gt_classes"]).reshape(-1)
-                gt_inds = np.where(cls_h > 0)[0]
-                crowd = np.asarray(entry["is_crowd"]).reshape(-1)[gt_inds] if "is_crowd" in entry else np.zeros(gt_inds.size, bool)
+                # add_keypoint_rcnn_blobs reads box_to_gt_ind_map as roidb rows: the assigned gt index through gt_inds
+                gt_inds = np.where(np.asarray(entry["gt_classes"]).reshape(-1) > 0)[0]
                 gi = torch.from_numpy(gt_inds.astype(np.int32)).to(dev)
-                G = gt_inds.size
-                mo, am = assignment[0][G:], assignment[1][G:]
+                mo, am = assignment[0], assignment[1]
                 kp_boxes.append(boxes)
-                kp_overlaps.append(torch.cat([torch.from_numpy(np.where(crowd != 0, -1.0, 1.0).astype(np.float32)).to(dev), mo]))
-                kp_map.append(torch.cat([gi, torch.where(am >= 0, gi[am.clamp(min=0).long()] if G else am, torch.full_like(am, -1))]))
+                kp_overlaps.append(mo)
+                kp_map.append(torch.where(am >= 0, gi[am.clamp(min=0).long()], am) if gt_inds.size else am)
                 kp_choices.append(ch[2] if len(ch) > 2 else None)
             per_image.append(b)
             if mask_on:                                                              # add_mask_rcnn_blobs' sampled_boxes (unscaled)

@@ -3,6 +3,7 @@
 Mirrors, for proposals that already live on the GPU, what the reference does per image on the host:
   * `bbox_overlaps`          lib/utils/cython_bbox.pyx:32-73
   * `assign_rois`            lib/datasets/json_dataset.py:429-490 (_merge_proposal_boxes_into_roidb) + :514-531
+  * `roidb_assignment`       the same for a merged roidb entry, its ground-truth rows as :208-290 (_add_gt_annotations) left them
   * `sample_rois`            lib/roi_data/fast_rcnn.py:129-200 (_sample_rois), :203-248 (_compute_targets, _expand_bbox_targets)
 Mask targets are in roi_data/mask_rcnn.py (device polygon rasteriser), keypoint targets in roi_data/keypoint_rcnn.py.
 
@@ -55,6 +56,25 @@ def assign_rois(boxes, gt_boxes, gt_classes):
     return max_overlaps, argmax, max_classes
 
 
+def roidb_assignment(boxes, gt_boxes, gt_classes, is_crowd=None):
+    """assign_rois for the rows of a merged roidb entry, its G ground-truth boxes first: a ground-truth row keeps what
+    _add_gt_annotations gave it -- itself, overlap 1 with its own class, or overlap -1 and class 0 when it is a crowd object
+    (is_crowd: (G,) flags, host or device; None: no crowd) -- so that no crowd row is ever sampled and each of several
+    identical boxes keeps its own class.  Proposal rows keep the IoU assignment, crowd objects included."""
+    max_overlaps, argmax, max_classes = assign_rois(boxes, gt_boxes, gt_classes)
+    G = int(gt_boxes.size(0)) if gt_boxes is not None else 0
+    if G:
+        dev = max_overlaps.device
+        gcls = gt_classes.to(device=dev, dtype=torch.int32).reshape(-1)
+        crowd = torch.zeros(G, dtype=torch.bool, device=dev) if is_crowd is None else torch.as_tensor(is_crowd).to(dev).reshape(-1) != 0
+        if crowd.numel() != G:
+            raise ValueError("is_crowd has %d flags for %d ground-truth boxes" % (crowd.numel(), G))
+        max_overlaps[:G] = torch.where(crowd, -1.0, 1.0)
+        max_classes[:G] = torch.where(crowd, 0, gcls)
+        argmax[:G] = torch.arange(G, dtype=torch.int32, device=dev)
+    return max_overlaps, argmax, max_classes
+
+
 def select_fg_bg(max_overlaps, fg_thresh, bg_thresh_hi, bg_thresh_lo):
     """np.where(max_overlaps >= fg) and np.where((max_overlaps < hi) & (max_overlaps >= lo)) as ascending int32 index tensors
     (one host read of the two counts)."""
@@ -73,22 +93,23 @@ def select_fg_bg(max_overlaps, fg_thresh, bg_thresh_hi, bg_thresh_lo):
 
 def sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, batch_size_per_im=512, fg_fraction=0.25,
                 fg_thresh=0.5, bg_thresh_hi=0.5, bg_thresh_lo=0.0, bbox_reg_weights=(10.0, 10.0, 5.0, 5.0),
-                cls_agnostic_bbox_reg=False, fg_choice=None, bg_choice=None, assignment=None):
+                cls_agnostic_bbox_reg=False, fg_choice=None, bg_choice=None, assignment=None, is_crowd=None):
     """_sample_rois for one image.  `boxes`: the roidb's boxes (ground truth first, then proposals; unscaled image
-    coordinates).  Returns the reference's blob dict with CUDA tensors: labels_int32, rois, bbox_targets,
-    bbox_inside_weights, bbox_outside_weights (+ keep_inds, the rows of `boxes` that were sampled).
-    assignment: (max_overlaps, box_to_gt_ind, max_classes) when the caller already has them (assign_rois)."""
+    coordinates); is_crowd: the roidb's crowd flags of the ground-truth rows.  Returns the reference's blob dict with CUDA
+    tensors: labels_int32, rois, bbox_targets, bbox_inside_weights, bbox_outside_weights (+ keep_inds, the rows of `boxes`
+    that were sampled).  assignment: (max_overlaps, box_to_gt_ind, max_classes) when the caller already has them
+    (roidb_assignment)."""
     return _sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, batch_size_per_im, fg_fraction, fg_thresh,
-                        bg_thresh_hi, bg_thresh_lo, bbox_reg_weights, cls_agnostic_bbox_reg, fg_choice, bg_choice, assignment)[0]
+                        bg_thresh_hi, bg_thresh_lo, bbox_reg_weights, cls_agnostic_bbox_reg, fg_choice, bg_choice, assignment, is_crowd)[0]
 
 
 def _sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, batch_size_per_im, fg_fraction, fg_thresh, bg_thresh_hi,
-                 bg_thresh_lo, bbox_reg_weights, cls_agnostic_bbox_reg, fg_choice, bg_choice, assignment):
+                 bg_thresh_lo, bbox_reg_weights, cls_agnostic_bbox_reg, fg_choice, bg_choice, assignment, is_crowd=None):
     """sample_rois' blobs and the number of fg rows (a host int; they come first)."""
     boxes = _boxes4(boxes, "boxes")
     dev = boxes.device
     if assignment is None:
-        assignment = assign_rois(boxes, gt_boxes, gt_classes)
+        assignment = roidb_assignment(boxes, gt_boxes, gt_classes, is_crowd)
     max_overlaps, argmax, max_classes = assignment
     rois_per_image = int(batch_size_per_im)
     fg_rois_per_image = int(round(fg_fraction * rois_per_image))

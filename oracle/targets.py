@@ -2,7 +2,7 @@
 target generation for one image.
 
   bbox_overlaps     lib/utils/cython_bbox.pyx:32-73 (float32 arithmetic, +1 pixel convention)
-  assign_rois       lib/datasets/json_dataset.py:429-490, :514-531
+  assign_rois       lib/datasets/json_dataset.py:429-490, :514-531 (ground-truth rows: :208-290, _add_gt_annotations)
   sample_rois       lib/roi_data/fast_rcnn.py:129-200, :203-248; lib/utils/boxes.py:199-230
 
 Pinned by tests/golden/targets.npz, produced by the UNMODIFIED reference functions (tests/golden/make_golden_targets.py).
@@ -33,15 +33,23 @@ def bbox_overlaps(boxes, query):
     return out
 
 
-def assign_rois(boxes, gt_boxes, gt_classes):
+def assign_rois(boxes, gt_boxes, gt_classes, is_crowd=None):
+    """max_overlaps, box_to_gt_ind_map, max_classes of a merged roidb entry.  `boxes`: its rows, the G ground-truth boxes first.
+    A ground-truth row keeps what _add_gt_annotations gave it: itself, overlap 1 with its own class, or overlap -1 (class 0)
+    when it is a crowd object.  A proposal row takes the first maximum of its IoU with every ground-truth box, crowd
+    objects included (0: none)."""
     boxes = np.asarray(boxes, f32)
-    N = boxes.shape[0]
+    N, G = boxes.shape[0], len(gt_boxes)
     max_overlaps = np.zeros((N,), f32); argmax = -np.ones((N,), np.int32); max_classes = np.zeros((N,), np.int32)
-    if len(gt_boxes):
+    if G:
         ov = bbox_overlaps(boxes, gt_boxes)
         am = ov.argmax(axis=1); mx = ov.max(axis=1)
         hit = mx > 0
         max_overlaps[hit] = mx[hit]; argmax[hit] = am[hit]; max_classes[hit] = np.asarray(gt_classes)[am[hit]]
+        crowd = np.zeros(G, bool) if is_crowd is None else np.asarray(is_crowd).reshape(-1) != 0
+        max_overlaps[:G] = np.where(crowd, f32(-1), f32(1))
+        argmax[:G] = np.arange(G)
+        max_classes[:G] = np.where(crowd, 0, np.asarray(gt_classes).reshape(-1))
     return max_overlaps, argmax, max_classes
 
 
@@ -58,9 +66,9 @@ def bbox_transform_inv(ex, gt, weights):
 
 def sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, fg_choice, bg_choice, batch_size_per_im=512,
                 fg_fraction=0.25, fg_thresh=0.5, bg_thresh_hi=0.5, bg_thresh_lo=0.0, bbox_reg_weights=(10.0, 10.0, 5.0, 5.0),
-                cls_agnostic_bbox_reg=False):
+                cls_agnostic_bbox_reg=False, is_crowd=None):
     boxes = np.asarray(boxes, f32)
-    max_overlaps, argmax, max_classes = assign_rois(boxes, gt_boxes, gt_classes)
+    max_overlaps, argmax, max_classes = assign_rois(boxes, gt_boxes, gt_classes, is_crowd)
     fg_inds = np.where(max_overlaps >= f32(fg_thresh))[0]
     bg_inds = np.where((max_overlaps < f32(bg_thresh_hi)) & (max_overlaps >= f32(bg_thresh_lo)))[0]
     fg_per_image = int(np.round(fg_fraction * batch_size_per_im))

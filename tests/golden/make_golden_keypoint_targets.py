@@ -19,7 +19,8 @@ Single-image cases (key prefix "<case>/"):
                  gives an all -1 keypoint row (weights 0) once selected
   nocand         no visible keypoint anywhere: no candidate, empty blobs
 "train/": CollectAndDistributeFpnRpnProposalsOp.forward in training mode with MODEL.KEYPOINTS_ON, two images over five RPN
-levels (no crowd object and no duplicated gt box: the training branch assigns gt rows by IoU, see DESIGN section 7).
+levels, without crowd objects or duplicated gt boxes; make_golden_fast_rcnn_roidb.py runs the training branch with KEYPOINTS_ON
+on both.
 """
 import os
 import sys
