@@ -202,16 +202,22 @@ box_proposal_match_kernel(int num_images, int num_props, int num_gt, int num_are
 
 }  // namespace
 
-size_t box_proposal_match_workspace_bytes(int num_props, int num_gt, int num_areas, int num_limits) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+size_t b200_box_proposal_match_workspace_bytes(int num_props, int num_gt, int num_areas, int num_limits) {
     if (num_props < 0 || num_gt < 0 || num_areas < 0 || num_limits < 0) return 0;
     const size_t la = (size_t)num_areas * num_limits;
     return la * ((size_t)num_gt * (sizeof(float) + sizeof(int)) + (size_t)num_props) + 16;
 }
 
-int box_proposal_match(int num_images, int num_props, int num_gt, int num_areas, int num_limits, int num_thresholds, const float* prop_box,
-                       const int* prop_begin, const float* gt_box, const double* gt_area, const int* gt_begin, const int* prop_count,
-                       const double* area_range, const double* thresholds, void* workspace, size_t workspace_bytes, float* overlap,
-                       unsigned char* excluded, unsigned char* error, long long* counts, cudaStream_t stream) {
+int b200_box_proposal_match(int num_images, int num_props, int num_gt, int num_areas, int num_limits, int num_thresholds, const float* prop_box,
+                            const int* prop_begin, const float* gt_box, const double* gt_area, const int* gt_begin, const int* prop_count,
+                            const double* area_range, const double* thresholds, void* workspace, size_t workspace_bytes, float* overlap,
+                            unsigned char* excluded, unsigned char* error, long long* counts, b200_stream_t stream) {
     if (num_images < 0 || num_props < 0 || num_gt < 0 || num_areas < 0 || num_areas > B200_BOX_PROPOSAL_MAX_AREAS || num_limits < 0 ||
         num_thresholds < 0)
         return B200_ROI_EINVAL;
@@ -224,7 +230,7 @@ int box_proposal_match(int num_images, int num_props, int num_gt, int num_areas,
     if (num_thresholds > 0 && (!thresholds || !counts)) return B200_ROI_EINVAL;
     if (((uintptr_t)prop_box | (uintptr_t)gt_box) & 15) return B200_ROI_EINVAL;
     if (((uintptr_t)gt_area | (uintptr_t)thresholds | (uintptr_t)counts) & 7) return B200_ROI_EINVAL;
-    const size_t need = box_proposal_match_workspace_bytes(num_props, num_gt, num_areas, num_limits);
+    const size_t need = b200_box_proposal_match_workspace_bytes(num_props, num_gt, num_areas, num_limits);
     if (!workspace || workspace_bytes < need) return B200_ROI_EWORKSPACE;
     AreaTable areas;
     for (int a = 0; a < num_areas; ++a) {
@@ -245,4 +251,4 @@ int box_proposal_match(int num_images, int num_props, int num_gt, int num_areas,
     return finish_launch(1);
 }
 
-}  // namespace b200
+}  // extern "C"

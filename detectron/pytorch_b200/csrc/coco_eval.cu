@@ -509,8 +509,14 @@ coco_accumulate_kernel(const __grid_constant__ AccParams ap, const int* __restri
 
 }  // namespace
 
-int coco_rank(int num_pairs, const int* pair_det_begin, const int* pair_entry_begin, const double* det_score, int* entry_det, int* entry_rank,
-              double* entry_score, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_coco_rank(int num_pairs, const int* pair_det_begin, const int* pair_entry_begin, const double* det_score, int* entry_det, int* entry_rank,
+                   double* entry_score, b200_stream_t stream) {
     if (num_pairs < 0 || (num_pairs > 0 && (!pair_det_begin || !pair_entry_begin || !det_score || !entry_det || !entry_rank || !entry_score)))
         return B200_ROI_EINVAL;
     if (num_pairs == 0) return B200_ROI_OK;
@@ -518,8 +524,8 @@ int coco_rank(int num_pairs, const int* pair_det_begin, const int* pair_entry_be
     return finish_launch();
 }
 
-int coco_bbox_iou(int num_pairs, const int* pair_gt_begin, const int* pair_entry_begin, const long long* pair_iou_begin, const int* entry_det,
-                  const double* det_box, const double* gt_box, const int* gt_flags, double* ious, cudaStream_t stream) {
+int b200_coco_bbox_iou(int num_pairs, const int* pair_gt_begin, const int* pair_entry_begin, const long long* pair_iou_begin, const int* entry_det,
+                       const double* det_box, const double* gt_box, const int* gt_flags, double* ious, b200_stream_t stream) {
     if (num_pairs < 0 || (num_pairs > 0 && (!pair_gt_begin || !pair_entry_begin || !pair_iou_begin || !entry_det || !det_box || !gt_box ||
                                             !gt_flags || !ious)))
         return B200_ROI_EINVAL;
@@ -530,9 +536,9 @@ int coco_bbox_iou(int num_pairs, const int* pair_gt_begin, const int* pair_entry
     return finish_launch();
 }
 
-int coco_oks(int num_pairs, const double* vars_host, const int* pair_gt_begin, const int* pair_entry_begin, const long long* pair_iou_begin,
-             const int* entry_det, const double* det_kp, const double* gt_kp, const double* gt_box, const double* gt_area, double* ious,
-             cudaStream_t stream) {
+int b200_coco_oks(int num_pairs, const double* vars_host, const int* pair_gt_begin, const int* pair_entry_begin, const long long* pair_iou_begin,
+                  const int* entry_det, const double* det_kp, const double* gt_kp, const double* gt_box, const double* gt_area, double* ious,
+                  b200_stream_t stream) {
     if (num_pairs < 0 || !vars_host || (num_pairs > 0 && (!pair_gt_begin || !pair_entry_begin || !pair_iou_begin || !entry_det || !det_kp ||
                                                           !gt_kp || !gt_box || !gt_area || !ious)))
         return B200_ROI_EINVAL;
@@ -545,10 +551,10 @@ int coco_oks(int num_pairs, const double* vars_host, const int* pair_gt_begin, c
     return finish_launch();
 }
 
-int coco_masks(unsigned* words, long long num_words, int num_slots, const long long* slot_word, const int* slot_hw, int n_str,
-               const int* str_slot, const long long* str_begin, const unsigned char* str_bytes, int n_cnt, const int* cnt_slot,
-               const long long* cnt_begin, const unsigned* counts, int n_poly, int num_vertices, const int* poly_slot, const int* vtx_begin,
-               const double* xy, int n_masks, const int* mask_slot_begin, long long* mask_area, int* mask_range, cudaStream_t stream) {
+int b200_coco_masks(unsigned* words, long long num_words, int num_slots, const long long* slot_word, const int* slot_hw, int n_str,
+                    const int* str_slot, const long long* str_begin, const unsigned char* str_bytes, int n_cnt, const int* cnt_slot,
+                    const long long* cnt_begin, const unsigned* counts, int n_poly, int num_vertices, const int* poly_slot, const int* vtx_begin,
+                    const double* xy, int n_masks, const int* mask_slot_begin, long long* mask_area, int* mask_range, b200_stream_t stream) {
     if (num_slots < 0 || n_str < 0 || n_cnt < 0 || n_poly < 0 || n_masks < 0 || num_words < 0 || num_vertices < 0) return B200_ROI_EINVAL;
     if (n_masks == 0) return B200_ROI_OK;
     if (!words || !slot_word || !slot_hw || !mask_slot_begin || !mask_area || !mask_range || (n_str && (!str_slot || !str_begin || !str_bytes)) ||
@@ -568,10 +574,10 @@ int coco_masks(unsigned* words, long long num_words, int num_slots, const long l
     return finish_launch(launches + 1);
 }
 
-int coco_segm_iou(int pair_begin, int num_pairs, const int* pair_gt_begin, const int* pair_entry_begin, const long long* pair_iou_begin,
-                  const int* entry_det, int det0, int gt0, int gt_mask0, const int* mask_slot_begin, const long long* slot_word,
-                  const int* slot_hw, const unsigned* words, const long long* mask_area, const int* mask_range, const int* gt_flags,
-                  double* ious, cudaStream_t stream) {
+int b200_coco_segm_iou(int pair_begin, int num_pairs, const int* pair_gt_begin, const int* pair_entry_begin, const long long* pair_iou_begin,
+                       const int* entry_det, int det0, int gt0, int gt_mask0, const int* mask_slot_begin, const long long* slot_word,
+                       const int* slot_hw, const unsigned* words, const long long* mask_area, const int* mask_range, const int* gt_flags,
+                       double* ious, b200_stream_t stream) {
     if (pair_begin < 0 || num_pairs < 0) return B200_ROI_EINVAL;
     if (num_pairs == 0) return B200_ROI_OK;
     if (!pair_gt_begin || !pair_entry_begin || !pair_iou_begin || !entry_det || !mask_slot_begin || !slot_word || !slot_hw || !words ||
@@ -584,10 +590,10 @@ int coco_segm_iou(int pair_begin, int num_pairs, const int* pair_gt_begin, const
     return finish_launch();
 }
 
-int coco_match(int num_pairs, int T, const double* iou_thrs_host, int A, const double* area_rng_host, int max_gt, const int* pair_gt_begin,
-               const int* pair_entry_begin, const long long* pair_iou_begin, const int* pair_cat, const int* entry_det, const double* det_area,
-               const double* gt_area, const int* gt_flags, const double* ious, int num_entries, unsigned* entry_flags, int* npig,
-               cudaStream_t stream) {
+int b200_coco_match(int num_pairs, int T, const double* iou_thrs_host, int A, const double* area_rng_host, int max_gt, const int* pair_gt_begin,
+                    const int* pair_entry_begin, const long long* pair_iou_begin, const int* pair_cat, const int* entry_det, const double* det_area,
+                    const double* gt_area, const int* gt_flags, const double* ious, int num_entries, unsigned* entry_flags, int* npig,
+                    b200_stream_t stream) {
     if (num_pairs < 0 || T < 1 || T > 16 || A < 1 || A > 8 || A * T > 64 || max_gt < 0 || num_entries < 0 || !iou_thrs_host || !area_rng_host)
         return B200_ROI_EINVAL;
     const size_t smem = (size_t)A * T * max_gt;
@@ -607,10 +613,10 @@ int coco_match(int num_pairs, int T, const double* iou_thrs_host, int A, const d
     return finish_launch();
 }
 
-int coco_accumulate(int K, int A, int M, int T, int R, const int* max_dets_host, const int* cat_entry_begin, const int* cat_pairs,
-                    const int* order, const int* entry_rank, const double* entry_score, const unsigned* entry_flags, int num_entries,
-                    int max_cat_entries, const int* npig, const double* rec_thrs, void* workspace, size_t workspace_bytes, double* precision, double* recall,
-                    double* scores, cudaStream_t stream) {
+int b200_coco_accumulate(int K, int A, int M, int T, int R, const int* max_dets_host, const int* cat_entry_begin, const int* cat_pairs,
+                         const int* order, const int* entry_rank, const double* entry_score, const unsigned* entry_flags, int num_entries,
+                         int max_cat_entries, const int* npig, const double* rec_thrs, void* workspace, size_t workspace_bytes, double* precision, double* recall,
+                         double* scores, b200_stream_t stream) {
     if (K < 1 || A < 1 || A > 8 || M < 1 || M > 8 || T < 1 || T > 16 || R < 1 || num_entries < 0 || max_cat_entries < 0 ||
         max_cat_entries > num_entries || max_cat_entries >= (1 << kAccBits) || !max_dets_host)
         return B200_ROI_EINVAL;
@@ -631,4 +637,4 @@ int coco_accumulate(int K, int A, int M, int T, int R, const int* max_dets_host,
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

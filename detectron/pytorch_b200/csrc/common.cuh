@@ -34,6 +34,47 @@ enum Option {
 };
 int option_get(Option which);
 
+// ---- RoIAlign paths behind the dispatch in api.cu ----------------------------------------------------------------------------
+// Defined in roi_align_<path>.cu.  row_map (nullable) gives each RoI's output row; a fast path returns kPathDeclined when the
+// shape or the workspace does not suit it.
+int roi_align_forward_generic(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
+                              const float* rois, float* top, const int* row_map, cudaStream_t stream);
+int roi_align_backward_generic(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
+                               const float* rois, float* bottom_diff, const int* row_map, cudaStream_t stream);
+size_t roi_align_tiled_workspace_bytes(int N, int R, int H, int W, int PH, int PW, int sr);
+int roi_align_forward_tiled(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
+                            const float* rois, float* top, const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t roi_align_stream_workspace_bytes(int N, int R, int H, int W, int PH, int PW, int sr);
+int roi_align_forward_stream(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
+                             const float* rois, float* top, const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t roi_align_strip_workspace_bytes(int N, int R, int H, int W, int PH, int PW, int sr);
+int roi_align_forward_strip(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
+                            const float* rois, float* top, const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t roi_align_strip_fpn_workspace_bytes(int levels, const int* heights, const int* widths, int N, int R, int PH, int PW, int sr);
+int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const int* heights, const int* widths, const float* scales,
+                                const int* level_roi_begin, int N, int R, int C, int PH, int PW, int sr, const float* rois, float* top,
+                                const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+size_t roi_align_bwd_nhwc_workspace_bytes(int N, int C, int H, int W);
+int roi_align_backward_nhwc(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
+                            const float* rois, float* bottom_diff, const int* row_map, void* workspace, size_t workspace_bytes,
+                            cudaStream_t stream);
+size_t roi_align_bwd_rows_workspace_bytes(int N, int R, int C, int H, int W, int PH, int PW, int sr);
+int roi_align_backward_rows(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW, int sr,
+                            const float* rois, float* bottom_diff, const int* row_map, void* workspace, size_t workspace_bytes,
+                            cudaStream_t stream);
+// Transposes a channel-innermost gradient image back to NCHW (roi_align_bwd_nhwc.cu; RoICrop's backward uses it too).
+void launch_nhwc_to_nchw(const float* scratch, float* dx, int N, int C, int HW, cudaStream_t stream);
+
+// Debug records (b200_roi_ops_debug_timing_buffer): NMS timing (nms.cu) and the watchdogs of the streaming and quad-strip paths.
+void nms_set_timing_buffer(unsigned long long* buf);
+void roi_align_stream_set_debug_buffer(unsigned long long* host_pinned);
+void roi_align_strip_set_debug_buffer(unsigned long long* host_pinned);
+
+// Dimension check shared by the RoIAlign, legacy RoIAlign and RoIPool entry points.
+inline bool bad_dims(int N, int R, int H, int W, int C, int PH, int PW) {
+    return N < 0 || R < 0 || H <= 0 || W <= 0 || C < 0 || PH <= 0 || PW <= 0;
+}
+
 // ---- arithmetic that must round exactly like the reference kernels' SASS --------------------
 // All helpers use the _rn intrinsics, which nvcc never contracts or re-associates, so the
 // fusion pattern is exactly what is written here (see oracle/roi_ops_oracle.c for the recipes

@@ -154,16 +154,31 @@ bool det_batch(const int* counts, int num, DetBatch* b, long long* total) {
 }
 }  // namespace
 
-int soft_nms_batched(float* boxes, const int* counts, int num, float sigma, float Nt, float threshold, int method, int* inds, int* n_out,
-                     cudaStream_t stream) {
-    DetBatch b; long long total = 0;
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_soft_nms_batched(float* boxes, const int* counts, int num, float sigma, float Nt, float threshold, int method, int* inds,
+                          int* n_out, b200_stream_t stream) {
+    if (!counts || num < 1 || !n_out) return B200_ROI_EINVAL;
+    long long total = 0;
+    for (int p = 0; p < num && p < 128; ++p) total += counts[p] > 0 ? counts[p] : 0;
+    if (total > 0 && (!boxes || !inds)) return B200_ROI_EINVAL;
+    DetBatch b;
     if (!det_batch(counts, num, &b, &total)) return B200_ROI_EINVAL;
     soft_nms_kernel<<<num, 32, 0, stream>>>(boxes, inds, n_out, b, sigma, Nt, threshold, method);
     return finish_launch();
 }
 
-int box_voting_batched(const float* top, const int* top_counts, const float* all, const int* all_counts, int num, float thresh, int scoring,
-                       float beta, float* out, cudaStream_t stream) {
+int b200_box_voting_batched(const float* top, const int* top_counts, const float* all, const int* all_counts, int num, float thresh,
+                            int scoring, float beta, float* out, b200_stream_t stream) {
+    if (!top_counts || !all_counts || num < 1) return B200_ROI_EINVAL;
+    long long total = 0;
+    for (int p = 0; p < num && p < 128; ++p) total += top_counts[p] > 0 ? top_counts[p] : 0;
+    if (total > 0 && (!top || !all || !out)) return B200_ROI_EINVAL;
+    if (scoring < 0 || scoring > 5) return B200_ROI_EINVAL;
     DetBatch tb, ab; long long t1 = 0, t2 = 0;
     if (!det_batch(top_counts, num, &tb, &t1) || !det_batch(all_counts, num, &ab, &t2)) return B200_ROI_EINVAL;
     int mx = 0;
@@ -174,4 +189,4 @@ int box_voting_batched(const float* top, const int* top_counts, const float* all
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -122,8 +122,14 @@ image_blob_kernel(const unsigned char* __restrict__ src_base, const b200_image_b
 }
 }  // namespace
 
-int image_blob(const unsigned char* src, const b200_image_blob_desc* descs, int num_images, const float* mean_table, int blob_h,
-               int blob_w, float* out, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_image_blob(const unsigned char* src, const b200_image_blob_desc* descs, int num_images, const float* mean_table, int blob_h,
+                    int blob_w, float* out, b200_stream_t stream) {
     if (!src || !descs || !mean_table || !out) return B200_ROI_EINVAL;
     if (num_images < 1 || num_images > 65535 || blob_h < 1 || blob_w < 1 || (long long)blob_h * blob_w >= (1LL << 31)) return B200_ROI_EINVAL;
     const bool vec = blob_w % 4 == 0 && reinterpret_cast<uintptr_t>(out) % 16 == 0;
@@ -133,4 +139,4 @@ int image_blob(const unsigned char* src, const b200_image_blob_desc* descs, int 
     return finish_launch(1);
 }
 
-}  // namespace b200
+}  // extern "C"

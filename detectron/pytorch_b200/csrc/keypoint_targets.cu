@@ -152,9 +152,15 @@ bool kp_tables(KpImages& im, int num_images, const int* box_begin, const int* gt
 
 }  // namespace
 
-int keypoint_candidates(const float* boxes, const float* max_overlaps, const int* box_to_gt, int num_images, const int* box_begin,
-                        const int* gt_inds, const int* gt_begin, const int* keypoints, const int* person_begin, int num_keypoints,
-                        float fg_thresh, int* candidates_out, int* counts_out, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_keypoint_candidates(const float* boxes, const float* max_overlaps, const int* box_to_gt, int num_images, const int* box_begin,
+                             const int* gt_inds, const int* gt_begin, const int* keypoints, const int* person_begin, int num_keypoints,
+                             float fg_thresh, int* candidates_out, int* counts_out, b200_stream_t stream) {
     if (!boxes || !max_overlaps || !box_to_gt || !gt_inds || !keypoints || !candidates_out || !counts_out) return B200_ROI_EINVAL;
     if (num_keypoints < 1 || num_keypoints > kKpMaxKeypoints) return B200_ROI_EINVAL;
     KpImages im{};
@@ -164,10 +170,10 @@ int keypoint_candidates(const float* boxes, const float* max_overlaps, const int
     return finish_launch(1);
 }
 
-int keypoint_targets(const float* boxes, const int* box_to_gt, int num_images, const int* box_begin, const int* gt_inds,
-                     const int* gt_begin, const int* keypoints, const int* person_begin, int num_keypoints, int heatmap_size,
-                     const int* candidates, const int* counts, const int* picks, const int* roi_begin, const float* im_scales,
-                     const float* batch_index, float* rois_out, int* locations_out, float* weights_out, cudaStream_t stream) {
+int b200_keypoint_targets(const float* boxes, const int* box_to_gt, int num_images, const int* box_begin, const int* gt_inds,
+                          const int* gt_begin, const int* keypoints, const int* person_begin, int num_keypoints, int heatmap_size,
+                          const int* candidates, const int* counts, const int* picks, const int* roi_begin, const float* im_scales,
+                          const float* batch_index, float* rois_out, int* locations_out, float* weights_out, b200_stream_t stream) {
     if (!boxes || !box_to_gt || !gt_inds || !keypoints || !candidates || !counts || !picks || !roi_begin || !im_scales || !batch_index ||
         !rois_out || !locations_out || !weights_out)
         return B200_ROI_EINVAL;
@@ -191,4 +197,4 @@ int keypoint_targets(const float* boxes, const int* box_to_gt, int num_images, c
     return finish_launch(1);
 }
 
-}  // namespace b200
+}  // extern "C"

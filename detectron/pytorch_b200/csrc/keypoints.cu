@@ -235,23 +235,27 @@ nms_oks_kernel(const float* __restrict__ xy, const float* __restrict__ rois, int
 }
 }  // namespace
 
-bool keypoints_args_ok(int num_rois, int num_keypoints, int heatmap_size, int min_size) {
-    return num_rois >= 0 && num_keypoints >= 1 && heatmap_size >= 1 && heatmap_size <= kKpMaxM && min_size <= kKpMaxSide &&
-           (long long)num_rois * num_keypoints < (1LL << 31);
-}
+}  // namespace b200
 
-bool nms_oks_args_ok(int num_rois, int num_keypoints) {
-    return num_rois >= 0 && num_rois <= kOksMaxDets && num_keypoints == kOksKeypoints;
-}
+using namespace b200;
 
-int heatmaps_to_keypoints(const float* maps, const float* rois, int D, int K, int M, int min_size, float* out, cudaStream_t stream) {
+extern "C" {
+
+int b200_heatmaps_to_keypoints(const float* maps, const float* rois, int D, int K, int M, int min_size, float* out, b200_stream_t stream) {
+    if (!(D >= 0 && K >= 1 && M >= 1 && M <= kKpMaxM && min_size <= kKpMaxSide && (long long)D * K < (1LL << 31)))
+        return B200_ROI_EINVAL;
+    if (D == 0) return B200_ROI_OK;
+    if (!maps || !rois || !out) return B200_ROI_EINVAL;
     heatmaps_to_keypoints_kernel<<<D * K, kKpThreads, 0, stream>>>(maps, rois, K, M, min_size, out);
     return finish_launch();
 }
 
-int nms_oks(const float* xy, const float* rois, int D, double thresh, int* keep, int* num_keep, cudaStream_t stream) {
+int b200_nms_oks(const float* xy, const float* rois, int D, int K, double thresh, int* keep, int* num_keep, b200_stream_t stream) {
+    if (!(D >= 0 && D <= kOksMaxDets && K == kOksKeypoints)) return B200_ROI_EINVAL;
+    if (D == 0) return B200_ROI_OK;
+    if (!xy || !rois || !keep || !num_keep) return B200_ROI_EINVAL;
     nms_oks_kernel<<<1, kKpThreads, 0, stream>>>(xy, rois, D, thresh, keep, num_keep);
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -464,18 +464,24 @@ int rows_grid(int R) { return (int)std::min<long long>(((long long)R + kWarps - 
 
 }  // namespace
 
-size_t loss_workspace_bytes(int num_levels) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+size_t b200_loss_workspace_bytes(int num_levels) {
     if (num_levels < 1 || num_levels > kMaxLevels) return 0;
     return kTicketBytes + (size_t)kMaxCtas * 4 * num_levels * sizeof(double);
 }
 
-int rpn_loss_forward(int num_levels, const b200_rpn_loss_level* levels, int activation, float fixed_divisor, void* workspace,
-                     size_t workspace_bytes, float* losses_out, float* divisor_out, cudaStream_t stream) {
+int b200_rpn_loss_forward(int num_levels, const b200_rpn_loss_level* levels, int activation, float fixed_divisor, void* workspace,
+                          size_t workspace_bytes, float* losses_out, float* divisor_out, b200_stream_t stream) {
     RpnLossParams P;
     int st = rpn_params(num_levels, levels, activation, fixed_divisor, false, P);
     if (st != B200_ROI_OK) return st;
     if (!losses_out || !divisor_out) return B200_ROI_EINVAL;
-    if (!workspace || workspace_bytes < loss_workspace_bytes(num_levels)) return B200_ROI_EWORKSPACE;
+    if (!workspace || workspace_bytes < b200_loss_workspace_bytes(num_levels)) return B200_ROI_EWORKSPACE;
     const int chunks = P.seg_chunk_begin[2 * num_levels];
     const int grid = std::max(1, std::min(chunks, kMaxCtas));
     rpn_loss_forward_kernel<<<grid, kThreads, 0, stream>>>(P, (unsigned*)workspace, (double*)((char*)workspace + kTicketBytes), losses_out,
@@ -483,8 +489,8 @@ int rpn_loss_forward(int num_levels, const b200_rpn_loss_level* levels, int acti
     return finish_launch();
 }
 
-int rpn_loss_backward(int num_levels, const b200_rpn_loss_level* levels, int activation, const float* grad_losses, const float* divisor,
-                      cudaStream_t stream) {
+int b200_rpn_loss_backward(int num_levels, const b200_rpn_loss_level* levels, int activation, const float* grad_losses, const float* divisor,
+                           b200_stream_t stream) {
     RpnLossParams P;
     int st = rpn_params(num_levels, levels, activation, 0.f, true, P);
     if (st != B200_ROI_OK) return st;
@@ -495,22 +501,22 @@ int rpn_loss_backward(int num_levels, const b200_rpn_loss_level* levels, int act
     return finish_launch();
 }
 
-int fast_rcnn_loss_forward(int R, int C, int B, const float* cls, const float* bbox, const void* labels, int label_is_int64,
-                           const float* targets, const float* inside, const float* outside, void* workspace, size_t workspace_bytes,
-                           float* losses_out, float* accuracy_out, cudaStream_t stream) {
+int b200_fast_rcnn_loss_forward(int R, int C, int B, const float* cls, const float* bbox, const void* labels, int label_is_int64,
+                                const float* targets, const float* inside, const float* outside, void* workspace, size_t workspace_bytes,
+                                float* losses_out, float* accuracy_out, b200_stream_t stream) {
     FastRcnnArgs a;
     int st = fast_rcnn_args(R, C, B, cls, bbox, labels, label_is_int64, targets, inside, outside, a);
     if (st != B200_ROI_OK) return st;
     if (!losses_out || !accuracy_out) return B200_ROI_EINVAL;
-    if (!workspace || workspace_bytes < loss_workspace_bytes(1)) return B200_ROI_EWORKSPACE;
+    if (!workspace || workspace_bytes < b200_loss_workspace_bytes(1)) return B200_ROI_EWORKSPACE;
     fast_rcnn_loss_forward_kernel<<<rows_grid(R), kThreads, 0, stream>>>(a, (unsigned*)workspace, (double*)((char*)workspace + kTicketBytes),
                                                                         losses_out, accuracy_out);
     return finish_launch();
 }
 
-int fast_rcnn_loss_backward(int R, int C, int B, const float* cls, const float* bbox, const void* labels, int label_is_int64,
-                            const float* targets, const float* inside, const float* outside, const float* grad_losses, float* cls_grad,
-                            float* bbox_grad, cudaStream_t stream) {
+int b200_fast_rcnn_loss_backward(int R, int C, int B, const float* cls, const float* bbox, const void* labels, int label_is_int64,
+                                 const float* targets, const float* inside, const float* outside, const float* grad_losses, float* cls_grad,
+                                 float* bbox_grad, b200_stream_t stream) {
     FastRcnnArgs a;
     int st = fast_rcnn_args(R, C, B, cls, bbox, labels, label_is_int64, targets, inside, outside, a);
     if (st != B200_ROI_OK) return st;
@@ -519,4 +525,4 @@ int fast_rcnn_loss_backward(int R, int C, int B, const float* cls, const float* 
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

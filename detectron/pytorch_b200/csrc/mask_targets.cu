@@ -176,9 +176,15 @@ mask_targets_kernel(const __grid_constant__ MaskImages im, const float4* __restr
 
 }  // namespace
 
-int mask_targets(const float* rois, const int* roi_image, const int* roi_class, int num_rois, int num_images, const int* obj_begin,
-                 int num_polys, const int* poly_begin, int num_coords, const int* coord_begin, const float* coords, int M, int num_classes,
-                 float* obj_boxes, int* masks_out, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_mask_targets(const float* rois, const int* roi_image, const int* roi_class, int num_rois, int num_images, const int* obj_begin,
+                      int num_polys, const int* poly_begin, int num_coords, const int* coord_begin, const float* coords, int M, int num_classes,
+                      float* obj_boxes, int* masks_out, b200_stream_t stream) {
     if (!rois || !roi_image || !roi_class || !obj_begin || !poly_begin || !coord_begin || !coords || !obj_boxes || !masks_out)
         return B200_ROI_EINVAL;
     if (num_rois < 1 || num_images < 1 || num_images > kMaskMaxImages || M < 1 || M > kMaskMaxM || num_classes < 0 ||
@@ -205,4 +211,4 @@ int mask_targets(const float* rois, const int* roi_image, const int* roi_class, 
     return finish_launch(2);
 }
 
-}  // namespace b200
+}  // extern "C"

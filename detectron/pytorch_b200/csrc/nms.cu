@@ -417,20 +417,86 @@ __global__ void nms_empty_kernel(int* num_out) { *num_out = 0; }
 
 void nms_set_timing_buffer(unsigned long long* buf) { cudaMemcpyToSymbol(g_nms_timing, &buf, sizeof(buf)); }
 
-size_t nms_workspace_bytes(int n) {
+// ---- batched entry: `num_problems` independent score-sorted box sets, stored back to back in `boxes` ----
+static bool nms_batch_plan(const int* counts, int num_problems, NmsBatch* nb, size_t* ws_words, int* max_n) {
+    if (num_problems < 1 || num_problems > kNmsMaxProblems) return false;
+    nb->count = num_problems;
+    long long box = 0, tile = 0;
+    size_t words = 0;
+    int mx = 0;
+    for (int p = 0; p < num_problems; ++p) {
+        const int n = counts[p];
+        if (n < 0) return false;
+        const long long cb = (n + kNmsTile - 1) / kNmsTile;
+        nb->n[p] = n; nb->box_off[p] = (int)box; nb->tile_off[p] = (int)tile;
+        nb->mask_off[p] = words; words += (size_t)n * cb;
+        nb->diag_off[p] = words; words += (size_t)cb * kNmsTile;
+        box += n; tile += cb * (cb + 1) / 2;
+        if (box > 0x7fffffffLL || tile > 0x7fffffffLL) return false;
+        if (n > mx) mx = n;
+    }
+    nb->tile_off[num_problems] = (int)tile;
+    for (int p = num_problems; p < kNmsMaxProblems; ++p) { nb->n[p] = 0; nb->box_off[p] = (int)box; nb->tile_off[p + 1] = (int)tile; nb->mask_off[p] = nb->diag_off[p] = words; }
+    *ws_words = words; *max_n = mx;
+    return true;
+}
+
+// cython: the IoU test of lib/utils/cython_nms.pyx (see nms_bit) instead of the reference CUDA kernel's
+static int nms_batched(const float* boxes, const int* counts, int num_problems, int dim, float thresh, bool cython, int* keep_out,
+                       int* num_out, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+    if (!counts || num_problems < 1 || !num_out) return B200_ROI_EINVAL;
+    long long total = 0;
+    for (int p = 0; p < num_problems && p < 64; ++p) total += counts[p] > 0 ? counts[p] : 0;
+    if (total > 0 && (!boxes || !keep_out)) return B200_ROI_EINVAL;
+    NmsBatch nb; size_t words = 0; int mx = 0;
+    if (dim < 4 || !nms_batch_plan(counts, num_problems, &nb, &words, &mx)) return B200_ROI_EINVAL;
+    if (workspace == nullptr || workspace_bytes < (words * sizeof(u64) + 255) / 256 * 256) return B200_ROI_EWORKSPACE;
+    float lo = -INFINITY, hi = INFINITY;
+    if (thresh >= 9.5367431640625e-07f && thresh <= 1048576.f) {
+        lo = (float)((double)thresh * (1.0 - 3.814697265625e-06));
+        hi = (float)((double)thresh * (1.0 + 3.814697265625e-06));
+    }
+    const int cb = (mx + kNmsTile - 1) / kNmsTile;
+    int reach = 0;
+    size_t smem_res = 0;
+    for (int r = 4; r >= 2; --r) {
+        const size_t sm_r = sizeof(u64) * ((size_t)r * cb * kNmsTile + 4 * (size_t)cb) + 16;
+        if (sm_r <= 224 * 1024) { reach = r; smem_res = sm_r; break; }
+    }
+    if (reach == 0) return B200_ROI_EINVAL;                      // a problem too large for the pipelined scan: the caller loops over b200_nms
+    u64* ws = (u64*)workspace;
+    if (nb.tile_off[num_problems] > 0)
+        (cython ? nms_mask_batched_kernel<true> : nms_mask_batched_kernel<false>)<<<(unsigned)nb.tile_off[num_problems], kNmsTile, 0, stream>>>(
+            boxes, nb, dim, thresh, lo, hi, ws);
+    void (*kern)(const u64*, const NmsBatch, int*, int*) =
+        (reach == 4) ? nms_scan_resolver_batched_kernel<4> : (reach == 3) ? nms_scan_resolver_batched_kernel<3> : nms_scan_resolver_batched_kernel<2>;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_res);
+    if (e != cudaSuccess) return (int)e;
+    kern<<<num_problems, kScanThreads, smem_res, stream>>>(ws, nb, keep_out, num_out);
+    return finish_launch(2);
+}
+
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+size_t b200_nms_workspace_bytes(int n) {
     if (n <= 0) return 256;
     const size_t cb = (size_t)(n + kNmsTile - 1) / kNmsTile;
     return (((size_t)n * cb + cb * kNmsTile) * sizeof(u64) + 255) / 256 * 256;     // mask words + transposed diagonal words
 }
 
-int nms(const float* boxes, int n, int dim, float thresh, int* keep_out, int* num_out, void* workspace,
-        size_t workspace_bytes, cudaStream_t stream) {
+int b200_nms(const float* boxes, int n, int dim, float thresh, int* keep_out, int* num_out, void* workspace,
+             size_t workspace_bytes, b200_stream_t stream) {
+    if (!num_out || (n > 0 && (!boxes || !keep_out))) return B200_ROI_EINVAL;
     if (n < 0 || dim < 4) return B200_ROI_EINVAL;
     if (n == 0) {
         nms_empty_kernel<<<1, 1, 0, stream>>>(num_out);
         return finish_launch();
     }
-    if (workspace == nullptr || workspace_bytes < nms_workspace_bytes(n)) return B200_ROI_EWORKSPACE;
+    if (workspace == nullptr || workspace_bytes < b200_nms_workspace_bytes(n)) return B200_ROI_EWORKSPACE;
     const int cb = (n + kNmsTile - 1) / kNmsTile;
     u64* mask = (u64*)workspace;
     u64* diag_t = mask + (size_t)n * cb;
@@ -463,65 +529,21 @@ int nms(const float* boxes, int n, int dim, float thresh, int* keep_out, int* nu
     return finish_launch(2);
 }
 
-// ---- batched entry: `num_problems` independent score-sorted box sets, stored back to back in `boxes` ----
-static bool nms_batch_plan(const int* counts, int num_problems, NmsBatch* nb, size_t* ws_words, int* max_n) {
-    if (num_problems < 1 || num_problems > kNmsMaxProblems) return false;
-    nb->count = num_problems;
-    long long box = 0, tile = 0;
-    size_t words = 0;
-    int mx = 0;
-    for (int p = 0; p < num_problems; ++p) {
-        const int n = counts[p];
-        if (n < 0) return false;
-        const long long cb = (n + kNmsTile - 1) / kNmsTile;
-        nb->n[p] = n; nb->box_off[p] = (int)box; nb->tile_off[p] = (int)tile;
-        nb->mask_off[p] = words; words += (size_t)n * cb;
-        nb->diag_off[p] = words; words += (size_t)cb * kNmsTile;
-        box += n; tile += cb * (cb + 1) / 2;
-        if (box > 0x7fffffffLL || tile > 0x7fffffffLL) return false;
-        if (n > mx) mx = n;
-    }
-    nb->tile_off[num_problems] = (int)tile;
-    for (int p = num_problems; p < kNmsMaxProblems; ++p) { nb->n[p] = 0; nb->box_off[p] = (int)box; nb->tile_off[p + 1] = (int)tile; nb->mask_off[p] = nb->diag_off[p] = words; }
-    *ws_words = words; *max_n = mx;
-    return true;
-}
-
-size_t nms_batched_workspace_bytes(const int* counts, int num_problems) {
+size_t b200_nms_batched_workspace_bytes(const int* counts, int num_problems) {
+    if (!counts) return 0;
     NmsBatch nb; size_t words = 0; int mx = 0;
     if (!nms_batch_plan(counts, num_problems, &nb, &words, &mx)) return 0;
     return (words * sizeof(u64) + 255) / 256 * 256 + 256;
 }
 
-// cython: the IoU test of lib/utils/cython_nms.pyx (see nms_bit) instead of the reference CUDA kernel's
-int nms_batched(const float* boxes, const int* counts, int num_problems, int dim, float thresh, bool cython, int* keep_out, int* num_out,
-                void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-    NmsBatch nb; size_t words = 0; int mx = 0;
-    if (dim < 4 || !nms_batch_plan(counts, num_problems, &nb, &words, &mx)) return B200_ROI_EINVAL;
-    if (workspace == nullptr || workspace_bytes < (words * sizeof(u64) + 255) / 256 * 256) return B200_ROI_EWORKSPACE;
-    float lo = -INFINITY, hi = INFINITY;
-    if (thresh >= 9.5367431640625e-07f && thresh <= 1048576.f) {
-        lo = (float)((double)thresh * (1.0 - 3.814697265625e-06));
-        hi = (float)((double)thresh * (1.0 + 3.814697265625e-06));
-    }
-    const int cb = (mx + kNmsTile - 1) / kNmsTile;
-    int reach = 0;
-    size_t smem_res = 0;
-    for (int r = 4; r >= 2; --r) {
-        const size_t sm_r = sizeof(u64) * ((size_t)r * cb * kNmsTile + 4 * (size_t)cb) + 16;
-        if (sm_r <= 224 * 1024) { reach = r; smem_res = sm_r; break; }
-    }
-    if (reach == 0) return kPathDeclined;                        // a problem too large for the pipelined scan: the caller loops over b200_nms
-    u64* ws = (u64*)workspace;
-    if (nb.tile_off[num_problems] > 0)
-        (cython ? nms_mask_batched_kernel<true> : nms_mask_batched_kernel<false>)<<<(unsigned)nb.tile_off[num_problems], kNmsTile, 0, stream>>>(
-            boxes, nb, dim, thresh, lo, hi, ws);
-    void (*kern)(const u64*, const NmsBatch, int*, int*) =
-        (reach == 4) ? nms_scan_resolver_batched_kernel<4> : (reach == 3) ? nms_scan_resolver_batched_kernel<3> : nms_scan_resolver_batched_kernel<2>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_res);
-    if (e != cudaSuccess) return (int)e;
-    kern<<<num_problems, kScanThreads, smem_res, stream>>>(ws, nb, keep_out, num_out);
-    return finish_launch(2);
+int b200_nms_batched(const float* boxes, const int* counts, int num_problems, int dim, float thresh, int* keep_out, int* num_out,
+                     void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+    return nms_batched(boxes, counts, num_problems, dim, thresh, false, keep_out, num_out, workspace, workspace_bytes, stream);
 }
 
-}  // namespace b200
+int b200_nms_batched_cython(const float* boxes, const int* counts, int num_problems, int dim, float thresh, int* keep_out, int* num_out,
+                            void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+    return nms_batched(boxes, counts, num_problems, dim, thresh, true, keep_out, num_out, workspace, workspace_bytes, stream);
+}
+
+}  // extern "C"

@@ -65,12 +65,20 @@ proposal_decode_kernel(const float* __restrict__ deltas,        // (4A, H, W) of
     valid[t] = ok ? 1 : 0;
 }
 
-int proposal_decode(const float* deltas, const float* anchors, const long long* order, const float* scores, int k, int A, int H,
-                    int W, float feat_stride, float im_h, float im_w, float min_size, float* dets, int* valid, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_proposal_decode(const float* deltas, const float* anchors, const long long* order, const float* scores, int k, int A, int H,
+                         int W, float feat_stride, float im_h, float im_w, float min_size, float* dets, int* valid, b200_stream_t stream) {
+    if (k < 0 || A <= 0 || H <= 0 || W <= 0) return B200_ROI_EINVAL;
+    if (k > 0 && (!deltas || !anchors || !order || !scores || !dets || !valid)) return B200_ROI_EINVAL;
     if (k == 0) return B200_ROI_OK;
     proposal_decode_kernel<<<(k + 255) / 256, 256, 0, stream>>>(deltas, anchors, order, scores, k, A, H, W, feat_stride, im_h, im_w,
                                                                min_size, dets, valid);
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -109,8 +109,16 @@ static int legacy_c_per_cta(int R, int C, int bins) {
     return cpc;
 }
 
-int roi_align_legacy_forward(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW,
-                             const float* rois, float* top, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_roi_align_legacy_forward(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW,
+                                  const float* rois, float* top, b200_stream_t stream) {
+    if (bad_dims(N, R, H, W, C, PH, PW)) return B200_ROI_EINVAL;
+    if (R > 0 && C > 0 && (!bottom || !rois || !top)) return B200_ROI_EINVAL;
     if (R == 0 || C == 0) return B200_ROI_OK;
     const int cpc = legacy_c_per_cta(R, C, PH * PW);
     dim3 grid(R, (C + cpc - 1) / cpc);
@@ -118,8 +126,11 @@ int roi_align_legacy_forward(const float* bottom, float scale, int N, int R, int
     return finish_launch();
 }
 
-int roi_align_legacy_backward(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW,
-                              const float* rois, float* bottom_diff, cudaStream_t stream) {
+int b200_roi_align_legacy_backward(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW,
+                                   const float* rois, float* bottom_diff, b200_stream_t stream) {
+    if (bad_dims(N, R, H, W, C, PH, PW)) return B200_ROI_EINVAL;
+    if ((size_t)N * C == 0) return B200_ROI_OK;
+    if (!bottom_diff || (R > 0 && (!top_diff || !rois))) return B200_ROI_EINVAL;
     cudaError_t err = cudaMemsetAsync(bottom_diff, 0, sizeof(float) * (size_t)N * C * H * W, stream);
     if (err != cudaSuccess) return (int)err;
     if (R == 0 || C == 0) return B200_ROI_OK;
@@ -129,4 +140,4 @@ int roi_align_legacy_backward(const float* top_diff, float scale, int N, int R, 
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -87,17 +87,6 @@ static void crop_grid(int C, long npix, dim3& grid, int& cpc) {
     grid = dim3((unsigned)xb, (unsigned)((C + cpc - 1) / cpc));
 }
 
-int roi_crop_forward(const float* image, const float* grids, int N, int C, int H, int W, int R, int oh, int ow,
-                     float* output, cudaStream_t stream) {
-    const long npix = (long)R * oh * ow;
-    if (npix == 0 || C == 0) return B200_ROI_OK;
-    if (N <= 0) return B200_ROI_EINVAL;
-    dim3 grid; int cpc;
-    crop_grid(C, npix, grid, cpc);
-    roi_crop_kernel<false><<<grid, kCropThreads, 0, stream>>>(image, grids, output, N, C, H, W, R, oh, ow, cpc);
-    return finish_launch();
-}
-
 // ---- backward, vector-reduction path (same idea as roi_align_bwd_nhwc.cu) ------------------------------------------------
 // The sampling geometry of an output pixel is the same for every channel, so in a channel-innermost scratch image of the
 // gradient every tap updates C contiguous floats: one red.global.add.v4.f32 per tap per FOUR channels (6.4 M vector reductions
@@ -105,8 +94,6 @@ int roi_crop_forward(const float* image, const float* grids, int N, int C, int H
 // One CTA per (RoI, <= 256 channels): grad_output[r] (one contiguous block) is staged transposed to [pixel][channel] in shared
 // memory; thread = (pixel lane, channel quad).  The scratch image is transposed back to NCHW by the RoIAlign path's kernel.
 // Per-tap terms FMUL(go, w) as in the reference (roi_crop_cuda_kernel.cu:163-190); summation order undefined, as with atomicAdd.
-void launch_nhwc_to_nchw(const float* scratch, float* dx, int N, int C, int HW, cudaStream_t stream);
-
 constexpr int kCropChunk = 256;
 
 __global__ void __launch_bounds__(256)
@@ -153,11 +140,6 @@ static bool crop_nhwc_applies(int N, int C, int H, int W, int R, int oh, int ow)
     return taps >= 2LL * N * C * H * W;                        // zero + transpose of the whole image must pay off
 }
 
-size_t roi_crop_backward_workspace_bytes(int N, int C, int H, int W, int R, int oh, int ow) {
-    if (option_get(kOptBwdPath) == 'g' || !crop_nhwc_applies(N, C, H, W, R, oh, ow)) return 0;
-    return (sizeof(float) * (size_t)N * C * H * W + 255) / 256 * 256;
-}
-
 static int roi_crop_backward_nhwc(const float* grad_output, const float* grids, int N, int C, int H, int W, int R, int oh, int ow,
                                   float* grad_image, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     if (!crop_nhwc_applies(N, C, H, W, R, oh, ow)) return kPathDeclined;
@@ -183,8 +165,37 @@ static int roi_crop_backward_nhwc(const float* grad_output, const float* grids, 
     return finish_launch(2);
 }
 
-int roi_crop_backward(const float* grad_output, const float* grids, int N, int C, int H, int W, int R, int oh, int ow,
-                      float* grad_image, float* grad_grids, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_roi_crop_forward(const float* image, const float* grids, int N, int C, int H, int W, int R, int oh, int ow,
+                          float* output, b200_stream_t stream) {
+    if (N < 0 || C < 0 || H <= 0 || W <= 0 || R < 0 || oh < 0 || ow < 0) return B200_ROI_EINVAL;
+    if ((size_t)R * oh * ow * C > 0 && (!image || !grids || !output)) return B200_ROI_EINVAL;
+    const long npix = (long)R * oh * ow;
+    if (npix == 0 || C == 0) return B200_ROI_OK;
+    if (N <= 0) return B200_ROI_EINVAL;
+    dim3 grid; int cpc;
+    crop_grid(C, npix, grid, cpc);
+    roi_crop_kernel<false><<<grid, kCropThreads, 0, stream>>>(image, grids, output, N, C, H, W, R, oh, ow, cpc);
+    return finish_launch();
+}
+
+size_t b200_roi_crop_backward_workspace_bytes(int N, int C, int H, int W, int R, int oh, int ow) {
+    if (N <= 0 || C <= 0 || H <= 0 || W <= 0 || R <= 0 || oh <= 0 || ow <= 0) return 0;
+    if (option_get(kOptBwdPath) == 'g' || !crop_nhwc_applies(N, C, H, W, R, oh, ow)) return 0;
+    return (sizeof(float) * (size_t)N * C * H * W + 255) / 256 * 256;
+}
+
+int b200_roi_crop_backward_ws(const float* grad_output, const float* grids, int N, int C, int H, int W, int R, int oh, int ow,
+                              float* grad_image, float* grad_grids, void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+    if (N < 0 || C < 0 || H <= 0 || W <= 0 || R < 0 || oh < 0 || ow < 0) return B200_ROI_EINVAL;
+    if ((size_t)N * C == 0) return B200_ROI_OK;
+    if (!grad_image) return B200_ROI_EINVAL;
+    if ((size_t)R * oh * ow > 0 && (!grad_output || !grids)) return B200_ROI_EINVAL;
     if (grad_grids != nullptr) {
         const cudaError_t e0 = cudaMemsetAsync(grad_grids, 0, sizeof(float) * (size_t)R * oh * ow * 2, stream);
         if (e0 != cudaSuccess) return (int)e0;
@@ -212,4 +223,10 @@ int roi_crop_backward(const float* grad_output, const float* grids, int N, int C
     return finish_launch();
 }
 
-}  // namespace b200
+
+int b200_roi_crop_backward(const float* grad_output, const float* grids, int N, int C, int H, int W, int R, int oh, int ow,
+                           float* grad_image, float* grad_grids, b200_stream_t stream) {
+    return b200_roi_crop_backward_ws(grad_output, grids, N, C, H, W, R, oh, ow, grad_image, grad_grids, nullptr, 0, stream);
+}
+
+}  // extern "C"

@@ -179,8 +179,16 @@ static int pool_c_per_cta(int R, int C, int bins) {
     return cpc;
 }
 
-int roi_pool_forward(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW,
-                     const float* rois, float* top, int* argmax, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_roi_pool_forward(const float* bottom, float scale, int N, int R, int H, int W, int C, int PH, int PW,
+                          const float* rois, float* top, int* argmax, b200_stream_t stream) {
+    if (bad_dims(N, R, H, W, C, PH, PW)) return B200_ROI_EINVAL;
+    if (R > 0 && C > 0 && (!bottom || !rois || !top)) return B200_ROI_EINVAL;
     if (R == 0 || C == 0) return B200_ROI_OK;
     const int cpc = pool_c_per_cta(R, C, PH * PW);
     dim3 grid(R, (C + cpc - 1) / cpc);
@@ -188,8 +196,11 @@ int roi_pool_forward(const float* bottom, float scale, int N, int R, int H, int 
     return finish_launch();
 }
 
-int roi_pool_backward(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW,
-                      const float* rois, float* bottom_diff, const int* argmax, cudaStream_t stream) {
+int b200_roi_pool_backward(const float* top_diff, float scale, int N, int R, int H, int W, int C, int PH, int PW,
+                           const float* rois, float* bottom_diff, const int* argmax, b200_stream_t stream) {
+    if (bad_dims(N, R, H, W, C, PH, PW)) return B200_ROI_EINVAL;
+    if ((size_t)N * C == 0) return B200_ROI_OK;
+    if (!bottom_diff || (R > 0 && (!top_diff || !rois || !argmax))) return B200_ROI_EINVAL;
     if (N == 0 || C == 0 || H == 0 || W == 0) return B200_ROI_OK;
     const int tiles = ((H + kPbTileH - 1) / kPbTileH) * ((W + kPbTileW - 1) / kPbTileW);
     int cpc = C;
@@ -199,4 +210,4 @@ int roi_pool_backward(const float* top_diff, float scale, int N, int R, int H, i
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -405,26 +405,32 @@ bool rpn_geom(int L, const int* F, const int* A, const double* strides, const do
     return true;
 }
 
-}  // namespace
-
-int rpn_total_anchors(int L, const int* F, const int* A) {
-    if (L < 1 || L > kRpnMaxLevels || !F || !A) return -1;
-    long long t = 0;
-    for (int l = 0; l < L; ++l) {
-        if (F[l] < 1 || A[l] < 1 || F[l] > 46340) return -1;
-        t += (long long)F[l] * F[l] * A[l];
-    }
-    return t > (1LL << 30) ? -1 : (int)t;
-}
-
 size_t rpn_workspace_bytes(int N, int T, int sumG) {
     if (N < 1 || N > kRpnMaxImages || T < 1 || sumG < 0) return 0;
     return rpn_ws_layout(N, T, sumG, nullptr, nullptr);
 }
 
-int rpn_labels(int L, const int* F, const int* A, const double* strides, const double* cell, int N, const double* im_sizes,
-               const int* gt_begin, const float* gt_boxes, double straddle, float pos_thresh, float neg_thresh, int* counts_out,
-               void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+}  // namespace
+
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+size_t b200_rpn_targets_workspace_bytes(int L, const int* F, const int* A, int N, int sumG) {
+    if (L < 1 || L > kRpnMaxLevels || !F || !A) return 0;
+    long long t = 0;
+    for (int l = 0; l < L; ++l) {
+        if (F[l] < 1 || A[l] < 1 || F[l] > 46340) return 0;
+        t += (long long)F[l] * F[l] * A[l];
+    }
+    return t > (1LL << 30) ? 0 : rpn_workspace_bytes(N, (int)t, sumG);
+}
+
+int b200_rpn_labels(int L, const int* F, const int* A, const double* strides, const double* cell, int N, const double* im_sizes,
+                    const int* gt_begin, const float* gt_boxes, double straddle, float pos_thresh, float neg_thresh, int* counts_out,
+                    void* workspace, size_t workspace_bytes, b200_stream_t stream) {
     RpnGeom g;
     if (!gt_boxes || !counts_out || !rpn_geom(L, F, A, strides, cell, N, im_sizes, gt_begin, straddle, &g)) return B200_ROI_EINVAL;
     const int sumG = gt_begin[N];
@@ -440,10 +446,10 @@ int rpn_labels(int L, const int* F, const int* A, const double* strides, const d
     return finish_launch(4);                                             // the memset counts as one
 }
 
-int rpn_emit(int L, const int* F, const int* A, const double* strides, const double* cell, int N, const double* im_sizes,
-             const int* gt_begin, const float* gt_boxes, double straddle, const int* counts, const int* fg_disable, const int* dis_begin,
-             const int* bg_enable, const int* en_begin, void* workspace, size_t workspace_bytes, int* const* labels_out,
-             float* const* targets_out, float* const* inside_out, float* const* outside_out, cudaStream_t stream) {
+int b200_rpn_emit(int L, const int* F, const int* A, const double* strides, const double* cell, int N, const double* im_sizes,
+                  const int* gt_begin, const float* gt_boxes, double straddle, const int* counts, const int* fg_disable, const int* dis_begin,
+                  const int* bg_enable, const int* en_begin, void* workspace, size_t workspace_bytes, int* const* labels_out,
+                  float* const* targets_out, float* const* inside_out, float* const* outside_out, b200_stream_t stream) {
     RpnGeom g;
     if (!gt_boxes || !counts || !dis_begin || !en_begin || !labels_out || !targets_out || !inside_out || !outside_out ||
         !rpn_geom(L, F, A, strides, cell, N, im_sizes, gt_begin, straddle, &g))
@@ -483,4 +489,4 @@ int rpn_emit(int L, const int* F, const int* A, const double* strides, const dou
     return finish_launch(3);
 }
 
-}  // namespace b200
+}  // extern "C"

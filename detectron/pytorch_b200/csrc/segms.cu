@@ -281,34 +281,51 @@ paste_masks_kernel(const float* __restrict__ masks, const int* __restrict__ mask
 }
 }  // namespace
 
-size_t segm_workspace_bytes(int num_dets) {
+static bool segm_args_ok(int num_dets, int num_channels, int resolution, int im_h, int im_w) {
+    return num_dets >= 0 && num_channels >= 1 && resolution >= 1 && resolution <= kSegmMaxM && im_h > 0 && im_w > 0 &&
+           (long long)im_h * im_w < (1LL << 28);
+}
+
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+size_t b200_segm_workspace_bytes(int num_dets) {
     if (num_dets <= 0) return 0;
     const size_t b = (size_t)num_dets * kSegmThreads * sizeof(SegmThreadState);
     return (b + 255) & ~(size_t)255;
 }
 
-bool segm_args_ok(int num_dets, int num_channels, int resolution, int im_h, int im_w) {
-    return num_dets >= 0 && num_channels >= 1 && resolution >= 1 && resolution <= kSegmMaxM && im_h > 0 && im_w > 0 &&
-           (long long)im_h * im_w < (1LL << 28);
-}
-
-int segm_rle_sizes(const float* masks, const int* mask_class, const float* boxes, int D, int Kc, int M, int im_h, int im_w, float thresh,
-                   int* sizes, void* ws, cudaStream_t stream) {
+int b200_segm_rle_sizes(const float* masks, const int* mask_class, const float* boxes, int D, int Kc, int M, int im_h, int im_w,
+                        float thresh, int* sizes, void* ws, size_t workspace_bytes, b200_stream_t stream) {
+    if (!segm_args_ok(D, Kc, M, im_h, im_w)) return B200_ROI_EINVAL;
+    if (D == 0) return B200_ROI_OK;
+    if (!masks || !mask_class || !boxes || !sizes) return B200_ROI_EINVAL;
+    if (!ws || workspace_bytes < b200_segm_workspace_bytes(D)) return B200_ROI_EWORKSPACE;
     segm_rle_sizes_kernel<<<D, kSegmThreads, 0, stream>>>(masks, mask_class, boxes, Kc, M, im_h, im_w, thresh, (SegmThreadState*)ws,
                                                           (int2*)sizes);
     return finish_launch();
 }
 
-int segm_rle_emit(const float* masks, const int* mask_class, const float* boxes, int D, int Kc, int M, int im_h, int im_w, float thresh,
-                  const int* sizes, const void* ws, int* counts, long long* count_offs, unsigned char* strings, long long* string_offs,
-                  cudaStream_t stream) {
+int b200_segm_rle_emit(const float* masks, const int* mask_class, const float* boxes, int D, int Kc, int M, int im_h, int im_w,
+                       float thresh, const int* sizes, const void* ws, size_t workspace_bytes, int* counts, long long* count_offs,
+                       unsigned char* strings, long long* string_offs, b200_stream_t stream) {
+    if (!segm_args_ok(D, Kc, M, im_h, im_w)) return B200_ROI_EINVAL;
+    if (D == 0) return B200_ROI_OK;
+    if (!masks || !mask_class || !boxes || !sizes || !counts || !count_offs || !strings || !string_offs) return B200_ROI_EINVAL;
+    if (!ws || workspace_bytes < b200_segm_workspace_bytes(D)) return B200_ROI_EWORKSPACE;
     segm_rle_emit_kernel<<<D, kSegmThreads, 0, stream>>>(masks, mask_class, boxes, D, Kc, M, im_h, im_w, thresh, (const int2*)sizes,
                                                          (const SegmThreadState*)ws, counts, count_offs, strings, string_offs);
     return finish_launch();
 }
 
-int paste_masks(const float* masks, const int* mask_class, const float* boxes, int D, int Kc, int M, int im_h, int im_w, float thresh,
-                unsigned char* out, cudaStream_t stream) {
+int b200_paste_masks(const float* masks, const int* mask_class, const float* boxes, int D, int Kc, int M, int im_h, int im_w, float thresh,
+                     unsigned char* out, b200_stream_t stream) {
+    if (!segm_args_ok(D, Kc, M, im_h, im_w) || D > 65535) return B200_ROI_EINVAL;
+    if (D == 0) return B200_ROI_OK;
+    if (!masks || !mask_class || !boxes || !out) return B200_ROI_EINVAL;
     const long long N = (long long)im_h * im_w;
     const long long blocks = (N + 8LL * kSegmThreads - 1) / (8LL * kSegmThreads);
     dim3 grid((unsigned)(blocks < 1024 ? blocks : 1024), D);
@@ -316,4 +333,4 @@ int paste_masks(const float* masks, const int* mask_class, const float* boxes, i
     return finish_launch();
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -131,30 +131,46 @@ fast_rcnn_targets_kernel(const float4* __restrict__ boxes, const float4* __restr
 
 }  // namespace
 
-int bbox_overlaps(const float* boxes, int N, const float* query, int K, float* out, cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_bbox_overlaps(const float* boxes, int N, const float* query, int K, float* out, b200_stream_t stream) {
+    if (N < 0 || K < 0) return B200_ROI_EINVAL;
+    if ((long long)N * K > 0 && (!boxes || !query || !out)) return B200_ROI_EINVAL;
     const long long total = (long long)N * K;
     if (total == 0) return B200_ROI_OK;
     bbox_overlaps_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const float4*)boxes, N, (const float4*)query, K, out);
     return finish_launch(1);
 }
 
-int roi_assign(const float* boxes, int N, const float* gt, const int* gt_classes, int G, float* max_overlaps, int* argmax,
-               int* max_classes, cudaStream_t stream) {
+int b200_roi_assign(const float* boxes, int N, const float* gt, const int* gt_classes, int G, float* max_overlaps, int* argmax,
+                    int* max_classes, b200_stream_t stream) {
+    if (N < 0 || G < 0) return B200_ROI_EINVAL;
+    if (N > 0 && (!boxes || !max_overlaps || !argmax || !max_classes)) return B200_ROI_EINVAL;
+    if (N > 0 && G > 0 && (!gt || !gt_classes)) return B200_ROI_EINVAL;
     if (N == 0) return B200_ROI_OK;
     roi_assign_kernel<<<(N + 255) / 256, 256, 0, stream>>>((const float4*)boxes, N, (const float4*)gt, gt_classes, G, max_overlaps, argmax,
                                                           max_classes);
     return finish_launch(1);
 }
 
-int roi_select(const float* max_overlaps, int N, float fg_thresh, float bg_hi, float bg_lo, int* fg_inds, int* bg_inds, int* counts,
-               cudaStream_t stream) {
+int b200_roi_select(const float* max_overlaps, int N, float fg_thresh, float bg_hi, float bg_lo, int* fg_inds, int* bg_inds, int* counts,
+                    b200_stream_t stream) {
+    if (N < 0 || !counts) return B200_ROI_EINVAL;
+    if (N > 0 && (!max_overlaps || !fg_inds || !bg_inds)) return B200_ROI_EINVAL;
     roi_select_kernel<<<1, 1024, 0, stream>>>(max_overlaps, N, fg_thresh, bg_hi, bg_lo, fg_inds, bg_inds, counts);
     return finish_launch(1);
 }
 
-int fast_rcnn_targets(const float* boxes, const float* gt, const int* argmax, const int* max_classes, const int* keep, int n, int n_fg,
-                      const float* weights4_host, int reg_classes, int cls_agnostic, float im_scale, float batch_idx, int* labels,
-                      float* rois, float* bbox_targets, float* inside, float* outside, cudaStream_t stream) {
+int b200_fast_rcnn_targets(const float* boxes, const float* gt, const int* argmax, const int* max_classes, const int* keep, int n, int n_fg,
+                           const float* weights4_host, int reg_classes, int cls_agnostic, float im_scale, float batch_idx, int* labels,
+                           float* rois, float* bbox_targets, float* inside, float* outside, b200_stream_t stream) {
+    if (n < 0 || n_fg < 0 || n_fg > n || reg_classes < 1 || !weights4_host) return B200_ROI_EINVAL;
+    if (n > 0 && (!boxes || !argmax || !max_classes || !keep || !labels || !rois || !bbox_targets || !inside || !outside))
+        return B200_ROI_EINVAL;
     if (n == 0) return B200_ROI_OK;
     fast_rcnn_targets_kernel<<<n, 256, 0, stream>>>((const float4*)boxes, (const float4*)gt, argmax, max_classes, keep, n, n_fg,
                                                     weights4_host[0], weights4_host[1], weights4_host[2], weights4_host[3], reg_classes,
@@ -162,4 +178,4 @@ int fast_rcnn_targets(const float* boxes, const float* gt, const int* argmax, co
     return finish_launch(1);
 }
 
-}  // namespace b200
+}  // extern "C"

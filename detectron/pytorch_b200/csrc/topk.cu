@@ -207,23 +207,37 @@ topk_collect_sort_kernel(const __grid_constant__ TopkBatch tb, const int* __rest
 
 }  // namespace
 
-size_t topk_batched_workspace_bytes(int num_problems) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+size_t b200_topk_batched_workspace_bytes(int num_problems) {
     if (num_problems < 1 || num_problems > kTopkMaxProblems) return 0;
     return (size_t)num_problems * 3 * kBins * sizeof(int);
 }
 
-// returns kPathDeclined when the batch does not fit the kernel's limits (caller falls back)
-int topk_batched(const float* const* scores_dev_ptrs_host, const int* A_host, const int* HW_host, const int* k_host, int num_problems,
-                 long long* order_out, float* scores_out, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-    if (num_problems < 1 || num_problems > kTopkMaxProblems) return kPathDeclined;
-    if (workspace == nullptr || workspace_bytes < topk_batched_workspace_bytes(num_problems)) return kPathDeclined;
+// returns B200_ROI_EWORKSPACE when the batch does not fit the kernel's limits (caller falls back)
+int b200_topk_batched(const float* const* scores_dev_ptrs_host, const int* A_host, const int* HW_host, const int* k_host, int num_problems,
+                      long long* order_out, float* scores_out, void* workspace, size_t workspace_bytes, b200_stream_t stream) {
+    if (num_problems < 1 || !scores_dev_ptrs_host || !A_host || !HW_host || !k_host) return B200_ROI_EINVAL;
+    long long total = 0;
+    for (int p = 0; p < num_problems && p < 64; ++p) {
+        if (!scores_dev_ptrs_host[p] || k_host[p] < 0) return B200_ROI_EINVAL;
+        total += k_host[p];
+    }
+    if (total > 0 && (!order_out || !scores_out)) return B200_ROI_EINVAL;
+    if (num_problems > kTopkMaxProblems) return B200_ROI_EWORKSPACE;
+    if (workspace == nullptr || workspace_bytes < b200_topk_batched_workspace_bytes(num_problems)) return B200_ROI_EWORKSPACE;
     TopkBatch tb;
     memset(&tb, 0, sizeof(tb));
     tb.count = num_problems;
     int off = 0, chunks = 0, kmax = 0;
     for (int p = 0; p < num_problems; ++p) {
         const long long n = (long long)A_host[p] * HW_host[p];
-        if (A_host[p] < 1 || HW_host[p] < 1 || n >= (1LL << 30) || k_host[p] < 0 || k_host[p] > n || k_host[p] > kTopkMaxK) return kPathDeclined;
+        if (A_host[p] < 1 || HW_host[p] < 1 || n >= (1LL << 30) || k_host[p] < 0 || k_host[p] > n || k_host[p] > kTopkMaxK)
+            return B200_ROI_EWORKSPACE;
         tb.src[p] = scores_dev_ptrs_host[p]; tb.A[p] = A_host[p]; tb.HW[p] = HW_host[p]; tb.k[p] = k_host[p];
         tb.out_off[p] = off; off += k_host[p];
         tb.chunk_off[p] = chunks; chunks += (int)((n + kChunk - 1) / kChunk);
@@ -232,7 +246,7 @@ int topk_batched(const float* const* scores_dev_ptrs_host, const int* A_host, co
     for (int p = num_problems; p <= kTopkMaxProblems; ++p) tb.chunk_off[p] = chunks;
     if (kmax == 0) return B200_ROI_OK;
     int* hist = (int*)workspace;
-    cudaError_t err = cudaMemsetAsync(hist, 0, topk_batched_workspace_bytes(num_problems), stream);
+    cudaError_t err = cudaMemsetAsync(hist, 0, b200_topk_batched_workspace_bytes(num_problems), stream);
     if (err != cudaSuccess) return (int)err;
     topk_hist_kernel<0><<<chunks, kHistThreads, 0, stream>>>(tb, hist);
     topk_hist_kernel<1><<<chunks, kHistThreads, 0, stream>>>(tb, hist);
@@ -242,7 +256,7 @@ int topk_batched(const float* const* scores_dev_ptrs_host, const int* A_host, co
     const size_t smem = (size_t)m2 * sizeof(u64);
     static bool attr_done[64] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kPathDeclined;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return B200_ROI_EWORKSPACE;
     if (!__atomic_load_n(&attr_done[dev], __ATOMIC_ACQUIRE)) {
         if (cudaFuncSetAttribute(topk_collect_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTopkMaxK * (int)sizeof(u64)) != cudaSuccess)
             return (int)cudaGetLastError();
@@ -252,4 +266,4 @@ int topk_batched(const float* const* scores_dev_ptrs_host, const int* A_host, co
     return finish_launch(4);
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -79,9 +79,15 @@ voc_outcome_kernel(int num_dets, double ovthresh, const int* __restrict__ pair_g
 
 }  // namespace
 
-int voc_match(int num_dets, int num_pairs, int num_gt, double ovthresh, const int* pair_gt_begin, const double* gt_box,
-              const unsigned char* gt_difficult, const int* det_pair, const double* det_box, int* workspace, unsigned char* outcome,
-              cudaStream_t stream) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_voc_match(int num_dets, int num_pairs, int num_gt, double ovthresh, const int* pair_gt_begin, const double* gt_box,
+                   const unsigned char* gt_difficult, const int* det_pair, const double* det_box, int* workspace, unsigned char* outcome,
+                   b200_stream_t stream) {
     if (num_dets < 0 || num_pairs < 0 || num_gt < 0 || (num_dets > 0 && num_pairs == 0)) return B200_ROI_EINVAL;
     if (num_gt > 0 && (!gt_box || !gt_difficult || !workspace)) return B200_ROI_EINVAL;
     if (num_dets > 0 && (!pair_gt_begin || !det_pair || !det_box || !outcome)) return B200_ROI_EINVAL;
@@ -104,4 +110,4 @@ int voc_match(int num_dets, int num_pairs, int num_gt, double ovthresh, const in
     return finish_launch(launches);
 }
 
-}  // namespace b200
+}  // extern "C"

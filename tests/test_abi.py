@@ -27,6 +27,49 @@ def test_library_builds_and_exports_header_symbols():
     assert sorted(_lib.EXPORTED_SYMBOLS) == declared       # python binding covers exactly the header
 
 
+_CTYPES_OF = {"int": ctypes.c_int, "float": ctypes.c_float, "double": ctypes.c_double, "size_t": ctypes.c_size_t,
+              "long long": ctypes.c_longlong, "unsigned long long": ctypes.c_ulonglong, "b200_stream_t": ctypes.c_void_p}
+
+
+def _ctype(decl, is_return=False):
+    """ctypes class of one C parameter (or return type) of the header: pointers are c_void_p, char strings c_char_p."""
+    decl = " ".join(decl.split())
+    if "*" in decl:
+        return ctypes.c_char_p if re.fullmatch(r"(const )?char ?\*( ?\w+)?", decl) else ctypes.c_void_p
+    words = [w for w in decl.split() if w != "const"]
+    if is_return and words == ["void"]:
+        return None
+    if not is_return and len(words) > 1:
+        words = words[:-1]                                   # drop the parameter name
+    return _CTYPES_OF[" ".join(words)]
+
+
+def _header_prototypes():
+    text = open(os.path.join(ROOT, "include", "b200_roi_ops.h")).read()
+    text = re.sub(r"/\*.*?\*/", " ", text, flags=re.S)
+    text = re.sub(r"//[^\n]*", " ", text)
+    protos = {}
+    for ret, name, params in re.findall(r"B200_API\s+([^;(]*?)\s*\b(b200_\w+)\s*\(([^)]*)\)\s*;", text):
+        params = [p for p in params.split(",") if p.strip()]
+        if [p.strip() for p in params] == ["void"]:
+            params = []
+        protos[name] = (_ctype(ret, is_return=True), [_ctype(p) for p in params])
+    return protos
+
+
+def test_ctypes_signatures_match_the_header():
+    """Every prototype of include/b200_roi_ops.h has the same return type and the same argument count and types in the ctypes
+    table: an argument of the wrong width there would pass the wrong bits without any error."""
+    protos = _header_prototypes()
+    assert sorted(protos) == _declared_symbols()
+    for name, (restype, argtypes) in protos.items():
+        lib_restype, lib_argtypes = _lib._SIGNATURES[name]
+        assert lib_restype is restype, "%s returns %s in the header, %s in _lib" % (name, restype, lib_restype)
+        assert len(lib_argtypes) == len(argtypes), "%s takes %d arguments in the header, %d in _lib" % (name, len(argtypes), len(lib_argtypes))
+        for i, (want, got) in enumerate(zip(argtypes, lib_argtypes)):
+            assert got is want, "%s argument %d is %s in the header, %s in _lib" % (name, i, want, got)
+
+
 def test_reference_named_launchers_are_exported():
     """SURVEY 8b: the reference's own launcher names with the reference's argument lists (include/b200_ref_launchers.h),
     so that lib/.../src/*_cuda.c links unchanged.  Two libraries because the two RoIAlign flavours share their names."""
