@@ -29,7 +29,7 @@ import numpy as np
 import torch
 from torch import nn
 
-from detectron.pytorch_b200 import _lib, ops
+from detectron.pytorch_b200 import ops
 
 _DEFAULTS = {
     "TRAIN": dict(RPN_PRE_NMS_TOP_N=12000, RPN_POST_NMS_TOP_N=2000, RPN_NMS_THRESH=0.7, RPN_MIN_SIZE=0),
@@ -106,14 +106,11 @@ class GenerateProposalsOp(nn.Module):
         k = int(order.numel())
         dets = torch.empty((k, 5), dtype=torch.float32, device=dev)
         valid = torch.empty((k,), dtype=torch.int32, device=dev)
-        lib = _lib.load()
         min_size_scaled = float(np.float32(min_size) * np.float32(im_info[2]))
-        with torch.cuda.device(dev):
-            _lib.check(lib.b200_proposal_decode(bbox_deltas.data_ptr(), self._anchors_on(dev).data_ptr(), order.data_ptr(),
-                                                top_scores.contiguous().data_ptr(), k, A, H, W, float(self._feat_stride),
-                                                float(im_info[0]), float(im_info[1]), min_size_scaled, dets.data_ptr(),
-                                                valid.data_ptr(), torch.cuda.current_stream().cuda_stream),
-                       "b200_proposal_decode")
+        top_scores = top_scores.contiguous()
+        ops._launch("b200_proposal_decode", dev, bbox_deltas.data_ptr(), self._anchors_on(dev).data_ptr(), order.data_ptr(),
+                    top_scores.data_ptr(), k, A, H, W, float(self._feat_stride), float(im_info[0]), float(im_info[1]), min_size_scaled,
+                    dets.data_ptr(), valid.data_ptr())
         if run_nms and nms_thresh > 0 and k > 0:
             keep, num = ops.nms_raw(dets, float(nms_thresh))
             return dets, valid, keep, num

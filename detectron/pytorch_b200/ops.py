@@ -17,8 +17,36 @@ from torch.autograd.function import once_differentiable
 from . import _lib
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
+def _current_stream(device):
+    return torch.cuda.current_stream(device).cuda_stream
+
+
+def _launch(name, device, *args):
+    """Call the library's entry point `name` with `args` and the current torch stream of `device` (so that CUDA graph capture
+    and side streams see the work), under a guard for `device`.  A non-zero status raises RuntimeError naming `name`."""
+    with torch.cuda.device(device):
+        _lib.check(getattr(_lib.load(), name)(*args, _current_stream(device)), name)
+
+
+def _host_array(ctype, values):
+    """A host table for a `*_host` argument: a ctypes array of at least one element, so that it always has an address.  The
+    caller holds it until the call returns."""
+    values = list(values)
+    return (ctype * max(len(values), 1))(*values)
+
+
+def _ptr(t):
+    """The device pointer of a tensor; null for a missing or empty one."""
+    return None if t is None or t.numel() == 0 else t.data_ptr()
+
+
+def _workspace(nbytes, device):
+    """A `nbytes` scratch buffer from torch's stream-ordered caching allocator and the pointer to pass for it; (None, null) for
+    0 bytes.  The caller keeps the buffer referenced until the launch is enqueued."""
+    if not nbytes:
+        return None, None
+    ws = torch.empty((int(nbytes),), dtype=torch.uint8, device=device)
+    return ws, ws.data_ptr()
 
 
 def _need_cuda_f32(t, name):
@@ -42,14 +70,10 @@ def roi_align_forward(features, rois, aligned_height, aligned_width, spatial_sca
     N, C, H, W = features.shape
     R = rois.size(0)
     out = torch.empty((R, C, aligned_height, aligned_width), dtype=torch.float32, device=features.device)
-    lib = _lib.load()
-    ws_bytes = int(lib.b200_roi_align_workspace_bytes(N, R, H, W, aligned_height, aligned_width, sampling_ratio))
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=features.device) if ws_bytes else None   # caching allocator, stream-ordered
-    with torch.cuda.device(features.device):
-        _lib.check(lib.b200_roi_align_forward_ws(features.data_ptr(), spatial_scale, N, R, H, W, C, aligned_height,
-                                                 aligned_width, sampling_ratio, rois.data_ptr(), out.data_ptr(),
-                                                 ws.data_ptr() if ws is not None else None, ws_bytes, _stream()),
-                   "b200_roi_align_forward_ws")
+    ws_bytes = _lib.load().b200_roi_align_workspace_bytes(N, R, H, W, aligned_height, aligned_width, sampling_ratio)
+    ws, ws_ptr = _workspace(ws_bytes, features.device)
+    _launch("b200_roi_align_forward_ws", features.device, features.data_ptr(), spatial_scale, N, R, H, W, C, aligned_height,
+            aligned_width, sampling_ratio, rois.data_ptr(), out.data_ptr(), ws_ptr, ws_bytes)
     return out
 
 
@@ -58,16 +82,11 @@ def roi_align_backward(grad_output, rois, feature_size, aligned_height, aligned_
     grad_output = grad_output.contiguous(); rois = rois.contiguous()
     N, C, H, W = feature_size
     grad_input = torch.empty((N, C, H, W), dtype=torch.float32, device=grad_output.device)
-    lib = _lib.load()
-    ws_bytes = int(lib.b200_roi_align_backward_workspace_bytes(N, rois.size(0), C, H, W, aligned_height, aligned_width,
-                                                              sampling_ratio)) if rois.size(0) > 0 else 0
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=grad_output.device) if ws_bytes else None
-    with torch.cuda.device(grad_output.device):
-        _lib.check(lib.b200_roi_align_backward_ws(grad_output.data_ptr(), spatial_scale, N, rois.size(0), H, W, C,
-                                                  aligned_height, aligned_width, sampling_ratio, rois.data_ptr(),
-                                                  grad_input.data_ptr(), ws.data_ptr() if ws is not None else None,
-                                                  ws_bytes, _stream()),
-                   "b200_roi_align_backward_ws")
+    ws_bytes = _lib.load().b200_roi_align_backward_workspace_bytes(N, rois.size(0), C, H, W, aligned_height, aligned_width,
+                                                                   sampling_ratio) if rois.size(0) > 0 else 0
+    ws, ws_ptr = _workspace(ws_bytes, grad_output.device)
+    _launch("b200_roi_align_backward_ws", grad_output.device, grad_output.data_ptr(), spatial_scale, N, rois.size(0), H, W, C,
+            aligned_height, aligned_width, sampling_ratio, rois.data_ptr(), grad_input.data_ptr(), ws_ptr, ws_bytes)
     return grad_input
 
 
@@ -121,49 +140,29 @@ class _RoIAlignFPN(Function):
             if f.size(1) != C or f.size(0) != feats[0].size(0):
                 raise ValueError("every pyramid level must have the same batch size and number of channels")
         kept = [r.contiguous() for r in rois]
-        done = False
-        if total > 0:
-            # one launch sequence over the whole pyramid: levels without RoIs drop out, the rest go level-major
-            import ctypes
-            live = [l for l in range(num_levels) if counts[l] > 0]
-            fl = [feats[l].contiguous() for l in live]
-            Lc = len(live)
-            N = int(fl[0].size(0))
-            hs = (ctypes.c_int * Lc)(*[int(f.size(2)) for f in fl]); wd = (ctypes.c_int * Lc)(*[int(f.size(3)) for f in fl])
-            ws_bytes = int(lib.b200_roi_align_fpn_workspace_bytes(Lc, ctypes.cast(hs, ctypes.c_void_p), ctypes.cast(wd, ctypes.c_void_p), N,
-                                                                  total, P[0], P[1], sr))
-            if ws_bytes > 0:
-                ptrs = (ctypes.c_void_p * Lc)(*[f.data_ptr() for f in fl])
-                scs = (ctypes.c_float * Lc)(*[float(scales[l]) for l in live])
-                begins, acc = [], 0
-                for l in live:
-                    begins.append(acc); acc += counts[l]
-                begins.append(acc)
-                bg = (ctypes.c_int * (Lc + 1))(*begins)
-                all_rois = torch.cat([kept[l] for l in live], dim=0) if Lc > 1 else kept[live[0]]
-                # inv is indexed by the position in the FULL level-major order; empty levels contribute nothing, so it is the same order
-                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-                with torch.cuda.device(dev):
-                    _lib.check(lib.b200_roi_align_forward_fpn(Lc, ctypes.cast(ptrs, ctypes.c_void_p), ctypes.cast(hs, ctypes.c_void_p),
-                                                              ctypes.cast(wd, ctypes.c_void_p), ctypes.cast(scs, ctypes.c_void_p),
-                                                              ctypes.cast(bg, ctypes.c_void_p), N, total, C, P[0], P[1], sr,
-                                                              all_rois.data_ptr(), inv.data_ptr(), out.data_ptr(), ws.data_ptr(), ws_bytes,
-                                                              _stream()), "b200_roi_align_forward_fpn")
-                done = True
-        off = 0
-        with torch.cuda.device(dev):
-            for f, r, sc, n_l in zip(feats, kept, scales, counts):
-                if n_l and not done:
-                    f = f.contiguous()
-                    N, _, H, W = f.shape
-                    ws_bytes = int(lib.b200_roi_align_workspace_bytes(N, n_l, H, W, P[0], P[1], sr))
-                    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None
-                    rows = inv[off:off + n_l]
-                    _lib.check(lib.b200_roi_align_forward_indexed(f.data_ptr(), float(sc), N, n_l, H, W, C, P[0], P[1], sr,
-                                                                  r.data_ptr(), rows.data_ptr(), out.data_ptr(),
-                                                                  ws.data_ptr() if ws is not None else None, ws_bytes, _stream()),
-                               "b200_roi_align_forward_indexed")
-                off += n_l
+        # levels without RoIs drop out, the rest go level-major; inv is indexed by the position in the full level-major order, to
+        # which empty levels contribute nothing, so it is the same order
+        live = [l for l in range(num_levels) if counts[l] > 0]
+        fl = [feats[l].contiguous() for l in live]
+        begins = np.cumsum([0] + [counts[l] for l in live]).tolist()
+        N = feats[0].size(0)
+        hs = _host_array(ctypes.c_int, [f.size(2) for f in fl])
+        wd = _host_array(ctypes.c_int, [f.size(3) for f in fl])
+        fpn_bytes = lib.b200_roi_align_fpn_workspace_bytes(len(live), hs, wd, N, total, P[0], P[1], sr) if live else 0
+        if fpn_bytes:
+            # one launch sequence over the whole pyramid
+            all_rois = torch.cat([kept[l] for l in live], dim=0) if len(live) > 1 else kept[live[0]]
+            ws, ws_ptr = _workspace(fpn_bytes, dev)
+            _launch("b200_roi_align_forward_fpn", dev, len(live), _host_array(ctypes.c_void_p, [f.data_ptr() for f in fl]), hs, wd,
+                    _host_array(ctypes.c_float, [scales[l] for l in live]), _host_array(ctypes.c_int, begins), N, total, C, P[0], P[1],
+                    sr, all_rois.data_ptr(), inv.data_ptr(), out.data_ptr(), ws_ptr, fpn_bytes)
+        else:
+            for l, f, b in zip(live, fl, begins):
+                n_l, H, W = counts[l], f.size(2), f.size(3)
+                ws_bytes = lib.b200_roi_align_workspace_bytes(N, n_l, H, W, P[0], P[1], sr)
+                ws, ws_ptr = _workspace(ws_bytes, dev)
+                _launch("b200_roi_align_forward_indexed", dev, f.data_ptr(), float(scales[l]), N, n_l, H, W, C, P[0], P[1], sr,
+                        kept[l].data_ptr(), inv[b:b + n_l].data_ptr(), out.data_ptr(), ws_ptr, ws_bytes)
         ctx.meta = (P, sr, [float(sc) for sc in scales], counts, [tuple(f.shape) for f in feats], num_levels)
         ctx.save_for_backward(inv, *kept)
         return out
@@ -179,22 +178,18 @@ class _RoIAlignFPN(Function):
         lib = _lib.load()
         grads = []
         off = 0
-        with torch.cuda.device(dev):
-            for r, sc, n_l, shape in zip(rois, scales, counts, shapes):
-                N, C, H, W = shape
-                if n_l == 0:
-                    grads.append(torch.zeros(shape, dtype=torch.float32, device=dev))
-                    continue
-                g = torch.empty(shape, dtype=torch.float32, device=dev)
-                ws_bytes = int(lib.b200_roi_align_backward_workspace_bytes(N, n_l, C, H, W, P[0], P[1], sr))
-                ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev) if ws_bytes else None
-                rows = inv[off:off + n_l]
-                _lib.check(lib.b200_roi_align_backward_indexed(grad_output.data_ptr(), rows.data_ptr(), sc, N, n_l, H, W, C,
-                                                               P[0], P[1], sr, r.data_ptr(), g.data_ptr(),
-                                                               ws.data_ptr() if ws is not None else None, ws_bytes, _stream()),
-                           "b200_roi_align_backward_indexed")
-                grads.append(g)
-                off += n_l
+        for r, sc, n_l, shape in zip(rois, scales, counts, shapes):
+            N, C, H, W = shape
+            if n_l == 0:
+                grads.append(torch.zeros(shape, dtype=torch.float32, device=dev))
+                continue
+            g = torch.empty(shape, dtype=torch.float32, device=dev)
+            ws_bytes = lib.b200_roi_align_backward_workspace_bytes(N, n_l, C, H, W, P[0], P[1], sr)
+            ws, ws_ptr = _workspace(ws_bytes, dev)
+            _launch("b200_roi_align_backward_indexed", dev, grad_output.data_ptr(), inv[off:off + n_l].data_ptr(), sc, N, n_l, H, W, C,
+                    P[0], P[1], sr, r.data_ptr(), g.data_ptr(), ws_ptr, ws_bytes)
+            grads.append(g)
+            off += n_l
         return (None, None, None, None, None, None) + tuple(grads) + (None,) * num_levels
 
 
@@ -218,11 +213,8 @@ def roi_align_legacy_forward(features, rois, aligned_height, aligned_width, spat
     N, C, H, W = features.shape
     R = rois.size(0)
     out = torch.empty((R, C, aligned_height, aligned_width), dtype=torch.float32, device=features.device)
-    with torch.cuda.device(features.device):
-        _lib.check(_lib.load().b200_roi_align_legacy_forward(features.data_ptr(), spatial_scale, N, R, H, W, C,
-                                                             aligned_height, aligned_width, rois.data_ptr(),
-                                                             out.data_ptr(), _stream()),
-                   "b200_roi_align_legacy_forward")
+    _launch("b200_roi_align_legacy_forward", features.device, features.data_ptr(), spatial_scale, N, R, H, W, C, aligned_height,
+            aligned_width, rois.data_ptr(), out.data_ptr())
     return out
 
 
@@ -231,11 +223,8 @@ def roi_align_legacy_backward(grad_output, rois, feature_size, aligned_height, a
     grad_output = grad_output.contiguous(); rois = rois.contiguous()
     N, C, H, W = feature_size
     grad_input = torch.empty((N, C, H, W), dtype=torch.float32, device=grad_output.device)
-    with torch.cuda.device(grad_output.device):
-        _lib.check(_lib.load().b200_roi_align_legacy_backward(grad_output.data_ptr(), spatial_scale, N, rois.size(0), H, W, C,
-                                                              aligned_height, aligned_width, rois.data_ptr(),
-                                                              grad_input.data_ptr(), _stream()),
-                   "b200_roi_align_legacy_backward")
+    _launch("b200_roi_align_legacy_backward", grad_output.device, grad_output.data_ptr(), spatial_scale, N, rois.size(0), H, W, C,
+            aligned_height, aligned_width, rois.data_ptr(), grad_input.data_ptr())
     return grad_input
 
 
@@ -265,11 +254,8 @@ def roi_pool_forward(features, rois, pooled_height, pooled_width, spatial_scale)
     R = rois.size(0)
     out = torch.empty((R, C, pooled_height, pooled_width), dtype=torch.float32, device=features.device)
     argmax = torch.empty((R, C, pooled_height, pooled_width), dtype=torch.int32, device=features.device)
-    with torch.cuda.device(features.device):
-        _lib.check(_lib.load().b200_roi_pool_forward(features.data_ptr(), spatial_scale, N, R, H, W, C, pooled_height,
-                                                     pooled_width, rois.data_ptr(), out.data_ptr(), argmax.data_ptr(),
-                                                     _stream()),
-                   "b200_roi_pool_forward")
+    _launch("b200_roi_pool_forward", features.device, features.data_ptr(), spatial_scale, N, R, H, W, C, pooled_height, pooled_width,
+            rois.data_ptr(), out.data_ptr(), argmax.data_ptr())
     return out, argmax
 
 
@@ -278,11 +264,8 @@ def roi_pool_backward(grad_output, argmax, rois, feature_size, pooled_height, po
     grad_output = grad_output.contiguous(); rois = rois.contiguous(); argmax = argmax.contiguous()
     N, C, H, W = feature_size
     grad_input = torch.empty((N, C, H, W), dtype=torch.float32, device=grad_output.device)
-    with torch.cuda.device(grad_output.device):
-        _lib.check(_lib.load().b200_roi_pool_backward(grad_output.data_ptr(), spatial_scale, N, rois.size(0), H, W, C,
-                                                      pooled_height, pooled_width, rois.data_ptr(), grad_input.data_ptr(),
-                                                      argmax.data_ptr(), _stream()),
-                   "b200_roi_pool_backward")
+    _launch("b200_roi_pool_backward", grad_output.device, grad_output.data_ptr(), spatial_scale, N, rois.size(0), H, W, C,
+            pooled_height, pooled_width, rois.data_ptr(), grad_input.data_ptr(), argmax.data_ptr())
     return grad_input
 
 
@@ -316,10 +299,7 @@ def roi_crop_forward(input1, input2):
     N, C, H, W = input1.shape
     R, oh, ow, _ = input2.shape
     out = torch.empty((R, C, oh, ow), dtype=torch.float32, device=input1.device)
-    with torch.cuda.device(input1.device):
-        _lib.check(_lib.load().b200_roi_crop_forward(input1.data_ptr(), input2.data_ptr(), N, C, H, W, R, oh, ow,
-                                                     out.data_ptr(), _stream()),
-                   "b200_roi_crop_forward")
+    _launch("b200_roi_crop_forward", input1.device, input1.data_ptr(), input2.data_ptr(), N, C, H, W, R, oh, ow, out.data_ptr())
     return out
 
 
@@ -330,14 +310,10 @@ def roi_crop_backward(grad_output, input2, input1_size):
     R, oh, ow, _ = input2.shape
     grad_input1 = torch.empty((N, C, H, W), dtype=torch.float32, device=grad_output.device)
     grad_input2 = torch.empty_like(input2)
-    lib = _lib.load()
-    ws_bytes = int(lib.b200_roi_crop_backward_workspace_bytes(N, C, H, W, R, oh, ow))
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=grad_output.device) if ws_bytes else None
-    with torch.cuda.device(grad_output.device):
-        _lib.check(lib.b200_roi_crop_backward_ws(grad_output.data_ptr(), input2.data_ptr(), N, C, H, W, R, oh, ow,
-                                                 grad_input1.data_ptr(), grad_input2.data_ptr(),
-                                                 ws.data_ptr() if ws is not None else None, ws_bytes, _stream()),
-                   "b200_roi_crop_backward_ws")
+    ws_bytes = _lib.load().b200_roi_crop_backward_workspace_bytes(N, C, H, W, R, oh, ow)
+    ws, ws_ptr = _workspace(ws_bytes, grad_output.device)
+    _launch("b200_roi_crop_backward_ws", grad_output.device, grad_output.data_ptr(), input2.data_ptr(), N, C, H, W, R, oh, ow,
+            grad_input1.data_ptr(), grad_input2.data_ptr(), ws_ptr, ws_bytes)
     return grad_input1, grad_input2
 
 
@@ -367,7 +343,6 @@ def topk_batched_raw(score_maps, ks):
     """Top-k of several (A, H, W) float32 CUDA score maps in one batched call (b200_topk_batched: radix select + in-CTA sort,
     no host read).  ks: host ints, k_p <= min(A*H*W, 16384); <= 64 problems.  Returns (order int64 (sum k,), scores float32
     (sum k,)): problem p's slice holds, best first, the indices into its (H, W, A) flattening and the scores."""
-    import ctypes
     P = len(score_maps)
     if P < 1 or P > TOPK_MAX_PROBLEMS or len(ks) != P:
         raise ValueError("topk_batched_raw: 1..64 problems with one k each")
@@ -382,17 +357,11 @@ def topk_batched_raw(score_maps, ks):
     total = sum(ks)
     order = torch.empty((max(total, 1),), dtype=torch.int64, device=dev)
     scores = torch.empty((max(total, 1),), dtype=torch.float32, device=dev)
-    lib = _lib.load()
-    ptrs = (ctypes.c_void_p * P)(*[m.data_ptr() for m in maps])
-    A = (ctypes.c_int * P)(*[m.size(0) for m in maps])
-    HW = (ctypes.c_int * P)(*[m.size(1) * m.size(2) for m in maps])
-    K = (ctypes.c_int * P)(*ks)
-    ws_bytes = int(lib.b200_topk_batched_workspace_bytes(P))
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.b200_topk_batched(ctypes.cast(ptrs, ctypes.c_void_p), ctypes.cast(A, ctypes.c_void_p), ctypes.cast(HW, ctypes.c_void_p),
-                                         ctypes.cast(K, ctypes.c_void_p), P, order.data_ptr(), scores.data_ptr(), ws.data_ptr(), ws_bytes,
-                                         _stream()), "b200_topk_batched")
+    ws_bytes = _lib.load().b200_topk_batched_workspace_bytes(P)
+    ws, ws_ptr = _workspace(ws_bytes, dev)
+    _launch("b200_topk_batched", dev, _host_array(ctypes.c_void_p, [m.data_ptr() for m in maps]),
+            _host_array(ctypes.c_int, [m.size(0) for m in maps]), _host_array(ctypes.c_int, [m.size(1) * m.size(2) for m in maps]),
+            _host_array(ctypes.c_int, ks), P, order.data_ptr(), scores.data_ptr(), ws_ptr, ws_bytes)
     return order[:total], scores[:total]
 
 
@@ -402,7 +371,6 @@ def nms_batched_raw(dets, counts, thresh, cython=False):
     device: problem p's kept indices (relative to its first row) sit at keep[offset_p : offset_p + num_out[p]].
     cython=False: the reference CUDA kernel's IoU test (fused area, IoU > thresh, b200_nms_batched); True: the Cython
     NMS's (separately rounded areas, IoU >= thresh, b200_nms_batched_cython)."""
-    import ctypes
     _need_cuda_f32(dets, "dets")
     if dets.dim() != 2 or dets.size(1) < 4:
         raise ValueError("dets must be (N, >=4) = [x1, y1, x2, y2, score], got %s" % (tuple(dets.shape),))
@@ -410,19 +378,16 @@ def nms_batched_raw(dets, counts, thresh, cython=False):
     if sum(counts) != dets.size(0) or not counts:
         raise ValueError("counts %s do not add up to %d rows" % (counts, dets.size(0)))
     dets = dets.contiguous()
-    lib = _lib.load()
     P = len(counts)
-    c_arr = (ctypes.c_int * P)(*counts)
+    c_arr = _host_array(ctypes.c_int, counts)
     keep = torch.empty((max(dets.size(0), 1),), dtype=torch.int32, device=dets.device)
     num_out = torch.empty((P,), dtype=torch.int32, device=dets.device)
-    ws_bytes = int(lib.b200_nms_batched_workspace_bytes(ctypes.cast(c_arr, ctypes.c_void_p), P))
+    ws_bytes = _lib.load().b200_nms_batched_workspace_bytes(c_arr, P)
     if ws_bytes == 0:
         raise ValueError("b200_nms_batched: 1..64 problems expected, got %d" % P)
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dets.device)
-    with torch.cuda.device(dets.device):
-        fn, name = (lib.b200_nms_batched_cython, "b200_nms_batched_cython") if cython else (lib.b200_nms_batched, "b200_nms_batched")
-        _lib.check(fn(dets.data_ptr(), ctypes.cast(c_arr, ctypes.c_void_p), P, dets.size(1), float(thresh), keep.data_ptr(), num_out.data_ptr(),
-                      ws.data_ptr(), ws_bytes, _stream()), name)
+    ws, ws_ptr = _workspace(ws_bytes, dets.device)
+    _launch("b200_nms_batched_cython" if cython else "b200_nms_batched", dets.device, dets.data_ptr(), c_arr, P, dets.size(1),
+            float(thresh), keep.data_ptr(), num_out.data_ptr(), ws_ptr, ws_bytes)
     return keep, num_out
 
 
@@ -449,12 +414,10 @@ def soft_nms_batched(dets, counts, sigma=0.5, overlap_thresh=0.3, score_thresh=0
     """Soft-NMS (lib/utils/cython_nms.pyx:98-203) on `len(counts)` problems stored back to back in dets (sum(counts), 5).
     Returns (dets_out, inds, num_out): problem p's survivors are dets_out[off_p : off_p + num_out[p]] (decayed scores, the
     reference's output order), inds their original row indices within the problem."""
-    import ctypes
     _need_cuda_f32(dets, "dets")
     counts = [int(c) for c in counts]
     if dets.dim() != 2 or dets.size(1) != 5 or sum(counts) != dets.size(0):
         raise ValueError("dets must be (sum(counts), 5)")
-    lib = _lib.load()
     out = dets.contiguous().clone()
     P = len(counts)
     inds = torch.empty((max(out.size(0), 1),), dtype=torch.int32, device=dets.device)
@@ -463,33 +426,27 @@ def soft_nms_batched(dets, counts, sigma=0.5, overlap_thresh=0.3, score_thresh=0
     for c0 in range(0, P, 128):
         chunk = counts[c0:c0 + 128]
         n = sum(chunk)
-        c_arr = (ctypes.c_int * len(chunk))(*chunk)
-        with torch.cuda.device(dets.device):
-            _lib.check(lib.b200_soft_nms_batched(out.data_ptr() + offs * 20, ctypes.cast(c_arr, ctypes.c_void_p), len(chunk), float(sigma),
-                                                 float(overlap_thresh), float(score_thresh), int(method), inds.data_ptr() + offs * 4,
-                                                 num_out.data_ptr() + c0 * 4, _stream()), "b200_soft_nms_batched")
+        _launch("b200_soft_nms_batched", dets.device, out.data_ptr() + offs * 20, _host_array(ctypes.c_int, chunk), len(chunk),
+                float(sigma), float(overlap_thresh), float(score_thresh), int(method), inds.data_ptr() + offs * 4,
+                num_out.data_ptr() + c0 * 4)
         offs += n
     return out, inds, num_out
 
 
 def box_voting_batched(top_dets, top_counts, all_dets, all_counts, thresh, scoring=0, beta=1.0):
     """Box voting (lib/utils/boxes.py:268-317) for `len(top_counts)` class problems; returns the refined top_dets."""
-    import ctypes
     _need_cuda_f32(top_dets, "top_dets"); _need_cuda_f32(all_dets, "all_dets")
     top_counts = [int(c) for c in top_counts]; all_counts = [int(c) for c in all_counts]
     if len(top_counts) != len(all_counts) or sum(top_counts) != top_dets.size(0) or sum(all_counts) != all_dets.size(0):
         raise ValueError("counts do not match the detection tensors")
-    lib = _lib.load()
     top_dets = top_dets.contiguous(); all_dets = all_dets.contiguous()
     out = torch.empty_like(top_dets)
     to = ao = 0
     for c0 in range(0, len(top_counts), 128):
         tc, ac = top_counts[c0:c0 + 128], all_counts[c0:c0 + 128]
-        t_arr = (ctypes.c_int * len(tc))(*tc); a_arr = (ctypes.c_int * len(ac))(*ac)
-        with torch.cuda.device(top_dets.device):
-            _lib.check(lib.b200_box_voting_batched(top_dets.data_ptr() + to * 20, ctypes.cast(t_arr, ctypes.c_void_p),
-                                                   all_dets.data_ptr() + ao * 20, ctypes.cast(a_arr, ctypes.c_void_p), len(tc), float(thresh),
-                                                   int(scoring), float(beta), out.data_ptr() + to * 20, _stream()), "b200_box_voting_batched")
+        _launch("b200_box_voting_batched", top_dets.device, top_dets.data_ptr() + to * 20, _host_array(ctypes.c_int, tc),
+                all_dets.data_ptr() + ao * 20, _host_array(ctypes.c_int, ac), len(tc), float(thresh), int(scoring), float(beta),
+                out.data_ptr() + to * 20)
         to += sum(tc); ao += sum(ac)
     return out
 
@@ -501,15 +458,11 @@ def nms_raw(dets, thresh):
         raise ValueError("dets must be (N, >=4) = [x1, y1, x2, y2, score], got %s" % (tuple(dets.shape),))
     dets = dets.contiguous()
     n, dim = dets.shape
-    lib = _lib.load()
     keep = torch.empty((max(n, 1),), dtype=torch.int32, device=dets.device)
     num_out = torch.empty((1,), dtype=torch.int32, device=dets.device)
-    ws_bytes = int(lib.b200_nms_workspace_bytes(n))
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dets.device)
-    with torch.cuda.device(dets.device):
-        _lib.check(lib.b200_nms(dets.data_ptr(), n, dim, float(thresh), keep.data_ptr(), num_out.data_ptr(),
-                                ws.data_ptr(), ws_bytes, _stream()),
-                   "b200_nms")
+    ws_bytes = _lib.load().b200_nms_workspace_bytes(n)
+    ws, ws_ptr = _workspace(ws_bytes, dets.device)
+    _launch("b200_nms", dets.device, dets.data_ptr(), n, dim, float(thresh), keep.data_ptr(), num_out.data_ptr(), ws_ptr, ws_bytes)
     return keep, num_out
 
 
@@ -542,20 +495,19 @@ def segm_rle_raw(masks, mask_class, boxes, im_h, im_w, thresh):
     if D == 0:
         z = torch.zeros((1,), dtype=torch.int64, device=dev)
         return torch.empty((0,), dtype=torch.int32, device=dev), z, torch.empty((0,), dtype=torch.uint8, device=dev), z.clone()
-    lib = _lib.load()
-    ws_bytes = int(lib.b200_segm_workspace_bytes(D))
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    ws_bytes = _lib.load().b200_segm_workspace_bytes(D)
+    ws, ws_ptr = _workspace(ws_bytes, dev)
     sizes = torch.empty((D, 2), dtype=torch.int32, device=dev)
     args = (masks.data_ptr(), mask_class.data_ptr(), boxes.data_ptr(), D, Kc, M, int(im_h), int(im_w), float(thresh))
+    _launch("b200_segm_rle_sizes", dev, *args, sizes.data_ptr(), ws_ptr, ws_bytes)
     with torch.cuda.device(dev):
-        _lib.check(lib.b200_segm_rle_sizes(*args, sizes.data_ptr(), ws.data_ptr(), ws_bytes, _stream()), "b200_segm_rle_sizes")
         total = sizes.cpu().to(torch.int64).sum(dim=0)
-        counts = torch.empty((int(total[0]),), dtype=torch.int32, device=dev)
-        strings = torch.empty((int(total[1]),), dtype=torch.uint8, device=dev)
-        count_offs = torch.empty((D + 1,), dtype=torch.int64, device=dev)
-        string_offs = torch.empty((D + 1,), dtype=torch.int64, device=dev)
-        _lib.check(lib.b200_segm_rle_emit(*args, sizes.data_ptr(), ws.data_ptr(), ws_bytes, counts.data_ptr(), count_offs.data_ptr(),
-                                          strings.data_ptr(), string_offs.data_ptr(), _stream()), "b200_segm_rle_emit")
+    counts = torch.empty((int(total[0]),), dtype=torch.int32, device=dev)
+    strings = torch.empty((int(total[1]),), dtype=torch.uint8, device=dev)
+    count_offs = torch.empty((D + 1,), dtype=torch.int64, device=dev)
+    string_offs = torch.empty((D + 1,), dtype=torch.int64, device=dev)
+    _launch("b200_segm_rle_emit", dev, *args, sizes.data_ptr(), ws_ptr, ws_bytes, counts.data_ptr(), count_offs.data_ptr(),
+            strings.data_ptr(), string_offs.data_ptr())
     return counts, count_offs, strings, string_offs
 
 
@@ -565,9 +517,8 @@ def paste_masks(masks, mask_class, boxes, im_h, im_w, thresh):
     out = torch.empty((D, int(im_h), int(im_w)), dtype=torch.uint8, device=masks.device)
     if D == 0:
         return out
-    with torch.cuda.device(masks.device):
-        _lib.check(_lib.load().b200_paste_masks(masks.data_ptr(), mask_class.data_ptr(), boxes.data_ptr(), D, Kc, M, int(im_h), int(im_w),
-                                                float(thresh), out.data_ptr(), _stream()), "b200_paste_masks")
+    _launch("b200_paste_masks", masks.device, masks.data_ptr(), mask_class.data_ptr(), boxes.data_ptr(), D, Kc, M, int(im_h), int(im_w),
+            float(thresh), out.data_ptr())
     return out
 
 
@@ -595,10 +546,7 @@ def heatmaps_to_keypoints_raw(maps, rois, min_size=0):
     out = torch.empty((D, 4, K), dtype=torch.float32, device=maps.device)
     if D == 0:
         return out
-    with torch.cuda.device(maps.device):
-        _lib.check(_lib.load().b200_heatmaps_to_keypoints(maps.data_ptr(), rois.data_ptr(), D, K, M, int(min_size), out.data_ptr(),
-                                                          _stream()),
-                   "b200_heatmaps_to_keypoints")
+    _launch("b200_heatmaps_to_keypoints", maps.device, maps.data_ptr(), rois.data_ptr(), D, K, M, int(min_size), out.data_ptr())
     return out
 
 
@@ -609,8 +557,6 @@ def rpn_targets_raw(gt_boxes, gt_counts, im_sizes, levels, draw, straddle_thresh
     draw(counts) is called once with the (N, 3) host array (#fg candidates, #bg candidates, #inside anchors) -- the one host read
     of the call -- and returns, per image, (fg positions to disable, bg positions to enable): int sequences or CUDA tensors.
     Returns one (labels int32 (N, A, F, F), bbox_targets, inside_weights, outside_weights float32 (N, 4A, F, F)) per level."""
-    import ctypes
-    import numpy as np
     _need_cuda_f32(gt_boxes, "gt_boxes")
     if gt_boxes.dim() != 2 or gt_boxes.size(1) != 4:
         raise ValueError("gt_boxes must be (G, 4) = [x1, y1, x2, y2], got %s" % (tuple(gt_boxes.shape),))
@@ -625,27 +571,20 @@ def rpn_targets_raw(gt_boxes, gt_counts, im_sizes, levels, draw, straddle_thresh
     Fs = [int(F) for F, _, _ in levels]
     cells = [np.asarray(c, dtype=np.float64).reshape(-1, 4) for _, _, c in levels]
     As = [c.shape[0] for c in cells]
-
-    def arr(ctype, vals):
-        a = (ctype * max(len(vals), 1))(*vals)
-        return ctypes.cast(a, ctypes.c_void_p), a             # the array object keeps the memory alive during the call
-
-    F_p, F_a = arr(ctypes.c_int, Fs)
-    A_p, A_a = arr(ctypes.c_int, As)
-    S_p, S_a = arr(ctypes.c_double, [float(s) for _, s, _ in levels])
-    C_p, C_a = arr(ctypes.c_double, np.concatenate(cells).ravel().tolist() if cells else [])
-    I_p, I_a = arr(ctypes.c_double, im_sizes.ravel().tolist())
-    G_p, G_a = arr(ctypes.c_int, np.concatenate([[0], np.cumsum(gt_counts)]).astype(int).tolist())
-    lib = _lib.load()
-    ws_bytes = int(lib.b200_rpn_targets_workspace_bytes(L, F_p, A_p, N, gt_boxes.size(0)))
+    F_a = _host_array(ctypes.c_int, Fs)
+    A_a = _host_array(ctypes.c_int, As)
+    ws_bytes = _lib.load().b200_rpn_targets_workspace_bytes(L, F_a, A_a, N, gt_boxes.size(0))
     if ws_bytes == 0:
         raise ValueError("rpn_targets_raw: unsupported geometry (1..8 levels, <= 32 cell anchors, 1..64 images)")
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    ws, ws_ptr = _workspace(ws_bytes, dev)
     counts = torch.empty((N, 3), dtype=torch.int32, device=dev)
-    common = (L, F_p, A_p, S_p, C_p, N, I_p, G_p, gt_boxes.data_ptr(), float(straddle_thresh))
-    with torch.cuda.device(dev):
-        _lib.check(lib.b200_rpn_labels(*common, float(positive_overlap), float(negative_overlap), counts.data_ptr(), ws.data_ptr(), ws_bytes,
-                                       _stream()), "b200_rpn_labels")
+    common = (L, F_a, A_a, _host_array(ctypes.c_double, [float(s) for _, s, _ in levels]),
+              _host_array(ctypes.c_double, np.concatenate(cells).ravel().tolist() if cells else []),
+              N, _host_array(ctypes.c_double, im_sizes.ravel().tolist()),
+              _host_array(ctypes.c_int, np.concatenate([[0], np.cumsum(gt_counts)]).astype(int).tolist()),
+              gt_boxes.data_ptr(), float(straddle_thresh))
+    _launch("b200_rpn_labels", dev, *common, float(positive_overlap), float(negative_overlap), counts.data_ptr(), ws_ptr, ws_bytes)
+    with torch.cuda.device(dev):                  # draw may create CUDA tensors: they belong on dev
         picks = draw(counts.cpu().numpy())
         dis_parts, en_parts = [], []
         for dis, en in picks:
@@ -653,8 +592,6 @@ def rpn_targets_raw(gt_boxes, gt_counts, im_sizes, levels, draw, straddle_thresh
             en_parts.append(torch.as_tensor(np.asarray(en) if not torch.is_tensor(en) else en).reshape(-1))
         if len(dis_parts) != N:
             raise ValueError("draw returned %d entries for %d images" % (len(dis_parts), N))
-        D_p, D_a = arr(ctypes.c_int, np.concatenate([[0], np.cumsum([d.numel() for d in dis_parts])]).astype(int).tolist())
-        E_p, E_a = arr(ctypes.c_int, np.concatenate([[0], np.cumsum([e.numel() for e in en_parts])]).astype(int).tolist())
         # one int32 device buffer for both draws (a single upload when they come from the host)
         parts = dis_parts + en_parts
         if all(not p.is_cuda for p in parts):
@@ -662,16 +599,18 @@ def rpn_targets_raw(gt_boxes, gt_counts, im_sizes, levels, draw, straddle_thresh
         else:
             flat = torch.cat([p.to(device=dev, dtype=torch.int32) for p in parts])
         flat = torch.cat([flat, flat.new_zeros((1,))])            # never empty: a valid pointer even without draws
-        n_dis = sum(d.numel() for d in dis_parts)
-        outs = []
-        for F, A in zip(Fs, As):
-            outs.append((torch.empty((N, A, F, F), dtype=torch.int32, device=dev),
-                         torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev),
-                         torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev),
-                         torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev)))
-        tables = [arr(ctypes.c_void_p, [o[k].data_ptr() for o in outs]) for k in range(4)]
-        _lib.check(lib.b200_rpn_emit(*common, counts.data_ptr(), flat.data_ptr(), D_p, flat.data_ptr() + 4 * n_dis, E_p, ws.data_ptr(),
-                                     ws_bytes, *[t[0] for t in tables], _stream()), "b200_rpn_emit")
+    D_a = _host_array(ctypes.c_int, np.concatenate([[0], np.cumsum([d.numel() for d in dis_parts])]).astype(int).tolist())
+    E_a = _host_array(ctypes.c_int, np.concatenate([[0], np.cumsum([e.numel() for e in en_parts])]).astype(int).tolist())
+    n_dis = sum(d.numel() for d in dis_parts)
+    outs = []
+    for F, A in zip(Fs, As):
+        outs.append((torch.empty((N, A, F, F), dtype=torch.int32, device=dev),
+                     torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev),
+                     torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev),
+                     torch.empty((N, 4 * A, F, F), dtype=torch.float32, device=dev)))
+    tables = [_host_array(ctypes.c_void_p, [o[k].data_ptr() for o in outs]) for k in range(4)]
+    _launch("b200_rpn_emit", dev, *common, counts.data_ptr(), flat.data_ptr(), D_a, flat.data_ptr() + 4 * n_dis, E_a, ws_ptr, ws_bytes,
+            *tables)
     return outs
 
 
@@ -686,7 +625,6 @@ def pack_polygons(objects_per_image):
     coordinates beyond +-2^20.  The reference's pycocotools frPyObjects dispatches on the first polygon's length: 4 values
     read every polygon of the object as [x, y, w, h] boxes, fewer fail, and an odd count silently drops the last value --
     none of which is a polygon mask, so all are rejected here."""
-    import numpy as np
     obj_begin, poly_begin, coord_begin, parts = [0], [0], [0], []
     for objs in objects_per_image:
         for polys in objs:
@@ -713,8 +651,6 @@ def mask_targets_raw(rois, roi_image, roi_class, packed, resolution, num_classes
     device-to-host read).  rois: float32 CUDA (R, 4) unscaled (x1, y1, x2, y2); roi_image: host ints (R,) (image index);
     roi_class: int32 CUDA (R,) -- a class <= 0 gives an all -1 row; packed: pack_polygons' tables; num_classes: 0 for
     class-agnostic masks.  Returns masks_int32 (R, max(num_classes, 1) * M * M) on the device."""
-    import ctypes
-    import numpy as np
     _need_cuda_f32(rois, "rois")
     if rois.dim() != 2 or rois.size(1) != 4:
         raise ValueError("rois must be (R, 4) = [x1, y1, x2, y2], got %s" % (tuple(rois.shape),))
@@ -739,18 +675,14 @@ def mask_targets_raw(rois, roi_image, roi_class, packed, resolution, num_classes
     ptr, i4 = buf.data_ptr(), 4
     boxes = torch.empty((max(O, 1), 4), dtype=torch.float32, device=dev)
     masks = torch.empty((R, max(K, 1) * M * M), dtype=torch.int32, device=dev)
-    ob = (ctypes.c_int * obj_begin.size)(*obj_begin.tolist())
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_mask_targets(rois.data_ptr(), ptr, roi_class.data_ptr(), R,
-                                                 obj_begin.size - 1, ob, P, ptr + i4 * R, C, ptr + i4 * (R + O + 1),
-                                                 ptr + i4 * (R + O + P + 2), M, K, boxes.data_ptr(), masks.data_ptr(), _stream()),
-                   "b200_mask_targets")
+    _launch("b200_mask_targets", dev, rois.data_ptr(), ptr, roi_class.data_ptr(), R, obj_begin.size - 1,
+            _host_array(ctypes.c_int, obj_begin.tolist()), P, ptr + i4 * R, C, ptr + i4 * (R + O + 1), ptr + i4 * (R + O + P + 2), M, K,
+            boxes.data_ptr(), masks.data_ptr())
     return masks
 
 
 def _host_or_device(x, dtype, dev, name):
     """A host array (returned as numpy, for the one upload) or a CUDA tensor of `dtype` (returned as is, contiguous)."""
-    import numpy as np
     if torch.is_tensor(x):
         if not x.is_cuda:
             raise NotImplementedError("%s must be a CUDA tensor or a host array, not a CPU tensor" % name)
@@ -772,15 +704,14 @@ def keypoint_targets_raw(boxes, box_begin, max_overlaps, box_to_gt_ind_map, gt_i
     A host box_to_gt_ind_map is checked against gt_inds first (numpy's IndexError becomes ValueError); a device one is read
     with the same bounds, an out-of-range entry meaning no person.  Returns (keypoint_rois (R, 5) float32,
     keypoint_locations_int32 (R * K,) int32, keypoint_weights (R * K,) float32, all CUDA; counts (N,) numpy)."""
-    import ctypes
-    import numpy as np
     box_begin = np.asarray(box_begin, np.int64).reshape(-1)
     N = box_begin.size - 1
     if not 1 <= N <= 64 or box_begin[0] != 0 or (np.diff(box_begin) < 0).any():
         raise ValueError("keypoint_targets_raw: box_begin must start at 0 and not decrease over 1..64 images, got %s" % box_begin.tolist())
-    if len(gt_inds) != N or len(gt_keypoints) != N or np.asarray(im_scales).size != N:
-        raise ValueError("keypoint_targets_raw: %d images but %d gt_inds, %d gt_keypoints, %d im_scales"
-                         % (N, len(gt_inds), len(gt_keypoints), np.asarray(im_scales).size))
+    batch_index = np.arange(N) if batch_index is None else np.asarray(batch_index).reshape(-1)
+    if len(gt_inds) != N or len(gt_keypoints) != N or np.asarray(im_scales).size != N or batch_index.size != N:
+        raise ValueError("keypoint_targets_raw: %d images but %d gt_inds, %d gt_keypoints, %d im_scales, %d batch indices"
+                         % (N, len(gt_inds), len(gt_keypoints), np.asarray(im_scales).size, batch_index.size))
     HS, fg = int(heatmap_size), int(fg_rois_per_image)
     kps = [np.asarray(k) for k in gt_keypoints]
     K = kps[0].shape[2] if kps[0].ndim == 3 else -1
@@ -822,23 +753,16 @@ def keypoint_targets_raw(boxes, box_begin, max_overlaps, box_to_gt_ind_map, gt_i
     put("kps", np.concatenate([k.astype(np.int32).reshape(-1) for k in kps]))
     parts.append(np.zeros((1,), np.int32))
     buf = torch.from_numpy(np.concatenate(parts)).pin_memory().to(dev, non_blocking=True)
-    base = buf.data_ptr()
-
-    def ptr(name, a):
-        return a.data_ptr() if torch.is_tensor(a) else base + 4 * offs[name]
-
-    def tab(vals):
-        return (ctypes.c_int * len(vals))(*[int(v) for v in vals])
-    bb = tab(box_begin)
-    gb = tab(np.concatenate([[0], np.cumsum([g.size for g in gis])]))
-    pb = tab(np.concatenate([[0], np.cumsum([k.shape[0] for k in kps])]))
-    cand =torch.empty((max(B, 1),), dtype=torch.int32, device=dev)
+    addr = {name: buf.data_ptr() + 4 * off for name, off in offs.items()}
+    addr.update((name, a.data_ptr()) for name, a in (("boxes", bx), ("mo", mo), ("map", bm)) if torch.is_tensor(a))
+    bb = _host_array(ctypes.c_int, box_begin.tolist())
+    gb = _host_array(ctypes.c_int, np.cumsum([0] + [g.size for g in gis]).tolist())
+    pb = _host_array(ctypes.c_int, np.cumsum([0] + [k.shape[0] for k in kps]).tolist())
+    cand = torch.empty((max(B, 1),), dtype=torch.int32, device=dev)
     counts = torch.empty((N,), dtype=torch.int32, device=dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        _lib.check(lib.b200_keypoint_candidates(ptr("boxes", bx), ptr("mo", mo), ptr("map", bm), N, bb, base + 4 * offs["gt_inds"], gb,
-                                                base + 4 * offs["kps"], pb, K, float(fg_thresh), cand.data_ptr(), counts.data_ptr(),
-                                                _stream()), "b200_keypoint_candidates")
+    _launch("b200_keypoint_candidates", dev, addr["boxes"], addr["mo"], addr["map"], N, bb, addr["gt_inds"], gb, addr["kps"], pb, K,
+            float(fg_thresh), cand.data_ptr(), counts.data_ptr())
+    with torch.cuda.device(dev):                  # draw may create CUDA tensors: they belong on dev
         counts_h = counts.cpu().numpy()
         picks = list(draw(counts_h))
         if len(picks) != N:
@@ -859,16 +783,15 @@ def keypoint_targets_raw(boxes, box_begin, max_overlaps, box_to_gt_ind_map, gt_i
             flat = torch.cat([p.to(torch.int32) for p in sel] + [torch.zeros((1,), dtype=torch.int32)]).to(dev)
         else:
             flat = torch.cat([p.to(device=dev, dtype=torch.int32) for p in sel] + [torch.zeros((1,), dtype=torch.int32, device=dev)])
-        R = sum(sizes)
-        rb = tab(np.concatenate([[0], np.cumsum(sizes)]))
-        sc = (ctypes.c_float * N)(*[float(np.float32(s)) for s in np.asarray(im_scales).reshape(-1)])
-        bi = (ctypes.c_float * N)(*[float(np.float32(b)) for b in (np.arange(N) if batch_index is None else np.asarray(batch_index).reshape(-1))])
-        rois = torch.empty((max(R, 1), 5), dtype=torch.float32, device=dev)
-        loc = torch.empty((max(R * K, 1),), dtype=torch.int32, device=dev)
-        w = torch.empty((max(R * K, 1),), dtype=torch.float32, device=dev)
-        _lib.check(lib.b200_keypoint_targets(ptr("boxes", bx), ptr("map", bm), N, bb, base + 4 * offs["gt_inds"], gb, base + 4 * offs["kps"],
-                                             pb, K, HS, cand.data_ptr(), counts.data_ptr(), flat.data_ptr(), rb, sc, bi, rois.data_ptr(),
-                                             loc.data_ptr(), w.data_ptr(), _stream()), "b200_keypoint_targets")
+    R = sum(sizes)
+    rb = _host_array(ctypes.c_int, np.cumsum([0] + sizes).tolist())
+    sc = _host_array(ctypes.c_float, [float(np.float32(s)) for s in np.asarray(im_scales).reshape(-1)])
+    bi = _host_array(ctypes.c_float, [float(np.float32(b)) for b in batch_index])
+    rois = torch.empty((max(R, 1), 5), dtype=torch.float32, device=dev)
+    loc = torch.empty((max(R * K, 1),), dtype=torch.int32, device=dev)
+    w = torch.empty((max(R * K, 1),), dtype=torch.float32, device=dev)
+    _launch("b200_keypoint_targets", dev, addr["boxes"], addr["map"], N, bb, addr["gt_inds"], gb, addr["kps"], pb, K, HS, cand.data_ptr(),
+            counts.data_ptr(), flat.data_ptr(), rb, sc, bi, rois.data_ptr(), loc.data_ptr(), w.data_ptr())
     return rois[:R], loc[:R * K], w[:R * K], counts_h
 
 
@@ -877,8 +800,6 @@ def keypoints_to_heatmap_labels_raw(keypoints, rois, heatmap_size):
     CUDA tensor), rois CUDA float32 (R, >=4) = [x1, y1, x2, y2].  Returns (heats (R, K) int32 = the reference's result after
     `.astype(np.int32)`, weights (R, K) float32), CUDA.  One launch (the emit of keypoint_targets_raw, each RoI its own
     candidate)."""
-    import ctypes
-    import numpy as np
     _need_cuda_f32(rois, "rois")
     if rois.dim() != 2 or rois.size(1) < 4:
         raise ValueError("rois must be (R, >=4) = [x1, y1, x2, y2, ...], got %s" % (tuple(rois.shape),))
@@ -897,17 +818,13 @@ def keypoints_to_heatmap_labels_raw(keypoints, rois, heatmap_size):
     kp = kp.contiguous()
     ident = torch.arange(R + 1, dtype=torch.int32, device=dev)            # map, gt_inds, candidates and picks; ident[R] = count
     ident[R] = R
-    tab = (ctypes.c_int * 2)(0, R)
-    one = (ctypes.c_float * 1)(1.0)
-    zero = (ctypes.c_float * 1)(0.0)
+    tab = _host_array(ctypes.c_int, [0, R])
     rows = torch.empty((R, 5), dtype=torch.float32, device=dev)
     heats = torch.empty((R, K), dtype=torch.int32, device=dev)
     weights = torch.empty((R, K), dtype=torch.float32, device=dev)
     p = ident.data_ptr()
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_keypoint_targets(boxes.data_ptr(), p, 1, tab, p, tab, kp.data_ptr(), tab, K, HS, p, p + 4 * R, p, tab, one,
-                                                     zero, rows.data_ptr(), heats.data_ptr(), weights.data_ptr(), _stream()),
-                   "b200_keypoint_targets")
+    _launch("b200_keypoint_targets", dev, boxes.data_ptr(), p, 1, tab, p, tab, kp.data_ptr(), tab, K, HS, p, p + 4 * R, p, tab,
+            _host_array(ctypes.c_float, [1.0]), _host_array(ctypes.c_float, [0.0]), rows.data_ptr(), heats.data_ptr(), weights.data_ptr())
     return heats, weights
 
 
@@ -925,10 +842,7 @@ def nms_oks_raw(xy_preds, rois, thresh):
     if D == 0:
         return keep[:0], torch.zeros((1,), dtype=torch.int32, device=xy_preds.device)
     num_keep = torch.empty((1,), dtype=torch.int32, device=xy_preds.device)
-    with torch.cuda.device(xy_preds.device):
-        _lib.check(_lib.load().b200_nms_oks(xy_preds.data_ptr(), rois.data_ptr(), D, K, float(thresh), keep.data_ptr(), num_keep.data_ptr(),
-                                            _stream()),
-                   "b200_nms_oks")
+    _launch("b200_nms_oks", xy_preds.device, xy_preds.data_ptr(), rois.data_ptr(), D, K, float(thresh), keep.data_ptr(), num_keep.data_ptr())
     return keep, num_keep
 
 
@@ -943,8 +857,7 @@ _BLOB_DESC = [("src_offset", "<i8"), ("row_pitch", "<i8"), ("inv_scale", "<f8"),
 def pixel_mean_table(pixel_means):
     """(3, 256) float32: channel c of a uint8 value v after the reference's `im = im.astype(np.float32); im -= pixel_means`
     (with the default float64 means, float32(float64(v) - mean)), evaluated by numpy itself."""
-    import numpy as np
-    t = np.empty((256, 1, 3), np.float32)
+    t =np.empty((256, 1, 3), np.float32)
     t[...] = np.arange(256, dtype=np.float32).reshape(256, 1, 1)
     t -= np.asarray(pixel_means)
     return np.ascontiguousarray(t.reshape(256, 3).T)
@@ -953,7 +866,6 @@ def pixel_mean_table(pixel_means):
 def resized_size(h, w, im_scale):
     """cv2.resize's output size for fx = fy = im_scale: (rint(h * s), rint(w * s)), half to even.  A zero side raises
     ValueError where cv2 raises."""
-    import numpy as np
     oh, ow = int(np.rint(h * float(im_scale))), int(np.rint(w * float(im_scale)))
     if oh <= 0 or ow <= 0:
         raise ValueError("resizing a %d x %d image by %r leaves an empty side (cv2.resize raises)" % (h, w, im_scale))
@@ -967,7 +879,6 @@ def image_blob_raw(images, scales, flipped, pixel_means, stride, out=None):
     None: FPN.COARSEST_STRIDE) and stored NCHW.  Host images go up in one asynchronous copy from one pinned buffer; CUDA
     images are read where they are.  Returns (blob float32 CUDA (N, 3, Hp, Wp), [(h, w) resized size per image]).
     `out`: an optional float32 CUDA tensor of that shape to write into (every element is written)."""
-    import numpy as np
     N = len(images)
     if N < 1 or len(scales) != N or len(flipped) != N:
         raise ValueError("image_blob_raw: %d images, %d scales, %d flip flags" % (N, len(scales), len(flipped)))
@@ -1024,22 +935,16 @@ def image_blob_raw(images, scales, flipped, pixel_means, stride, out=None):
     st[descs.nbytes:head] = table.view(np.uint8).reshape(-1)
     for i, im, off in host:
         st[head + off:head + off + im.nbytes] = im.reshape(-1)
-    with torch.cuda.device(dev):
-        # Asynchronous: torch's pinned-memory allocator records this copy on the stream and does not hand `staging` out again
-        # before it has completed, so dropping the last reference on return is safe.
-        buf.copy_(staging, non_blocking=True)
-        _lib.check(_lib.load().b200_image_blob(base, base, N, base + descs.nbytes, Hp, Wp, out.data_ptr(), _stream()),
-                   "b200_image_blob")
+    # Asynchronous, on dev's current stream: torch's pinned-memory allocator records this copy on the stream and does not hand
+    # `staging` out again before it has completed, so dropping the last reference on return is safe.
+    buf.copy_(staging, non_blocking=True)
+    _launch("b200_image_blob", dev, base, base, N, base + descs.nbytes, Hp, Wp, out.data_ptr())
     return out, sizes
 
 
 # ------------------------------------------------------------------------------------------------
 # COCO evaluation stages (pycocotools COCOeval.evaluate / accumulate; datasets/coco_eval.py drives them)
 # ------------------------------------------------------------------------------------------------
-def _ptr(t):
-    return 0 if t is None else t.data_ptr()
-
-
 def coco_rank_raw(pair_det_begin, pair_entry_begin, det_score, num_entries):
     """Stable descending-score rank per (image, category) pair, cut to each pair's entry count (COCOeval.computeIoU /
     evaluateImg's mergesort on -score and [0:maxDets[-1]]).  Returns (entry_det int32, entry_rank int32, entry_score f64)."""
@@ -1048,33 +953,25 @@ def coco_rank_raw(pair_det_begin, pair_entry_begin, det_score, num_entries):
     entry_det = torch.empty((max(num_entries, 1),), dtype=torch.int32, device=dev)
     entry_rank = torch.empty_like(entry_det)
     entry_score = torch.empty((max(num_entries, 1),), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_coco_rank(P, pair_det_begin.data_ptr(), pair_entry_begin.data_ptr(), det_score.data_ptr(),
-                                              entry_det.data_ptr(), entry_rank.data_ptr(), entry_score.data_ptr(), _stream()),
-                   "b200_coco_rank")
+    _launch("b200_coco_rank", dev, P, pair_det_begin.data_ptr(), pair_entry_begin.data_ptr(), det_score.data_ptr(), entry_det.data_ptr(),
+            entry_rank.data_ptr(), entry_score.data_ptr())
     return entry_det, entry_rank, entry_score
 
 
 def coco_bbox_iou_raw(pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_box, gt_box, gt_flags, ious):
     """computeIoU for iouType 'bbox' (maskApi bbIou) of every pair into `ious` (float64, rows = entries)."""
-    with torch.cuda.device(ious.device):
-        _lib.check(_lib.load().b200_coco_bbox_iou(pair_gt_begin.numel() - 1, pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(),
-                                                  pair_iou_begin.data_ptr(), entry_det.data_ptr(), det_box.data_ptr(), gt_box.data_ptr(),
-                                                  gt_flags.data_ptr(), ious.data_ptr(), _stream()), "b200_coco_bbox_iou")
+    _launch("b200_coco_bbox_iou", ious.device, pair_gt_begin.numel() - 1, pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(),
+            pair_iou_begin.data_ptr(), entry_det.data_ptr(), det_box.data_ptr(), gt_box.data_ptr(), gt_flags.data_ptr(), ious.data_ptr())
 
 
 def coco_oks_raw(vars, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_kp, gt_kp, gt_box, gt_area, ious):
     """computeOks of every pair into `ious`; vars = (sigmas * 2) ** 2 as a host float64 array of 17."""
-    import ctypes
-    import numpy as np
     v = np.ascontiguousarray(vars, np.float64)
     if v.size != 17:
         raise ValueError("OKS needs 17 keypoint variances, got %d" % v.size)
-    with torch.cuda.device(ious.device):
-        _lib.check(_lib.load().b200_coco_oks(pair_gt_begin.numel() - 1, v.ctypes.data_as(ctypes.c_void_p), pair_gt_begin.data_ptr(),
-                                             pair_entry_begin.data_ptr(), pair_iou_begin.data_ptr(), entry_det.data_ptr(), det_kp.data_ptr(),
-                                             gt_kp.data_ptr(), gt_box.data_ptr(), gt_area.data_ptr(), ious.data_ptr(), _stream()),
-                   "b200_coco_oks")
+    _launch("b200_coco_oks", ious.device, pair_gt_begin.numel() - 1, v.ctypes.data, pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(),
+            pair_iou_begin.data_ptr(), entry_det.data_ptr(), det_kp.data_ptr(), gt_kp.data_ptr(), gt_box.data_ptr(), gt_area.data_ptr(),
+            ious.data_ptr())
 
 
 def coco_masks_raw(words, slot_word, slot_hw, strings, counts, polys, mask_slot_begin, mask_area, mask_range):
@@ -1085,41 +982,30 @@ def coco_masks_raw(words, slot_word, slot_hw, strings, counts, polys, mask_slot_
     ns, ss, sb, sd = parts(strings)
     nc, cs, cb, cd = parts(counts)
     npl, ps, pb, pd = parts(polys)
-    with torch.cuda.device(words.device):
-        _lib.check(_lib.load().b200_coco_masks(words.data_ptr(), words.numel(), slot_hw.size(0), slot_word.data_ptr(), slot_hw.data_ptr(),
-                                               ns, _ptr(ss), _ptr(sb), _ptr(sd), nc, _ptr(cs), _ptr(cb), _ptr(cd),
-                                               npl, 0 if pd is None else pd.numel() // 2, _ptr(ps), _ptr(pb), _ptr(pd),
-                                               mask_slot_begin.numel() - 1, mask_slot_begin.data_ptr(), mask_area.data_ptr(),
-                                               mask_range.data_ptr(), _stream()), "b200_coco_masks")
+    _launch("b200_coco_masks", words.device, words.data_ptr(), words.numel(), slot_hw.size(0), slot_word.data_ptr(), slot_hw.data_ptr(),
+            ns, _ptr(ss), _ptr(sb), _ptr(sd), nc, _ptr(cs), _ptr(cb), _ptr(cd), npl, 0 if pd is None else pd.numel() // 2, _ptr(ps), _ptr(pb),
+            _ptr(pd), mask_slot_begin.numel() - 1, mask_slot_begin.data_ptr(), mask_area.data_ptr(), mask_range.data_ptr())
 
 
 def coco_segm_iou_raw(pair_begin, num_pairs, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det0, gt0, gt_mask0,
                       mask_slot_begin, slot_word, slot_hw, words, mask_area, mask_range, gt_flags, ious):
     """computeIoU for iouType 'segm' (rleIou) of pairs pair_begin .. + num_pairs - 1 on the bitmaps of one coco_masks_raw call."""
-    with torch.cuda.device(ious.device):
-        _lib.check(_lib.load().b200_coco_segm_iou(pair_begin, num_pairs, pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(),
-                                                  pair_iou_begin.data_ptr(), entry_det.data_ptr(), det0, gt0, gt_mask0,
-                                                  mask_slot_begin.data_ptr(), slot_word.data_ptr(), slot_hw.data_ptr(), words.data_ptr(),
-                                                  mask_area.data_ptr(), mask_range.data_ptr(), gt_flags.data_ptr(), ious.data_ptr(),
-                                                  _stream()), "b200_coco_segm_iou")
+    _launch("b200_coco_segm_iou", ious.device, pair_begin, num_pairs, pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(),
+            pair_iou_begin.data_ptr(), entry_det.data_ptr(), det0, gt0, gt_mask0, mask_slot_begin.data_ptr(), slot_word.data_ptr(),
+            slot_hw.data_ptr(), words.data_ptr(), mask_area.data_ptr(), mask_range.data_ptr(), gt_flags.data_ptr(), ious.data_ptr())
 
 
 def coco_match_raw(iou_thrs, area_rng, max_gt, num_cats, pair_gt_begin, pair_entry_begin, pair_iou_begin, pair_cat, entry_det, det_area,
                    gt_area, gt_flags, ious, num_entries):
     """evaluateImg at maxDets[-1] for every pair and area range.  Returns (entry_flags (A, E) uint32 as int32 bits, npig (K, A))."""
-    import ctypes
-    import numpy as np
     thr = np.ascontiguousarray(iou_thrs, np.float64)
     rng = np.ascontiguousarray(area_rng, np.float64).reshape(-1)
     A, dev = rng.size // 2, ious.device
     flags = torch.zeros((A, max(num_entries, 1)), dtype=torch.int32, device=dev)
     npig = torch.zeros((num_cats, A), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_coco_match(pair_gt_begin.numel() - 1, thr.size, thr.ctypes.data_as(ctypes.c_void_p), A,
-                                               rng.ctypes.data_as(ctypes.c_void_p), int(max_gt), pair_gt_begin.data_ptr(),
-                                               pair_entry_begin.data_ptr(), pair_iou_begin.data_ptr(), pair_cat.data_ptr(), entry_det.data_ptr(),
-                                               det_area.data_ptr(), gt_area.data_ptr(), gt_flags.data_ptr(), ious.data_ptr(), num_entries,
-                                               flags.data_ptr(), npig.data_ptr(), _stream()), "b200_coco_match")
+    _launch("b200_coco_match", dev, pair_gt_begin.numel() - 1, thr.size, thr.ctypes.data, A, rng.ctypes.data, int(max_gt),
+            pair_gt_begin.data_ptr(), pair_entry_begin.data_ptr(), pair_iou_begin.data_ptr(), pair_cat.data_ptr(), entry_det.data_ptr(),
+            det_area.data_ptr(), gt_area.data_ptr(), gt_flags.data_ptr(), ious.data_ptr(), num_entries, flags.data_ptr(), npig.data_ptr())
     return flags, npig
 
 
@@ -1127,8 +1013,6 @@ def coco_accumulate_raw(max_dets, cat_entry_begin, cat_pairs, order, entry_rank,
                         max_cat_entries):
     """accumulate(): precision / scores (T, R, K, A, M) and recall (T, K, A, M) float64 on the device, -1 where COCOeval skips.
     max_cat_entries: the largest category's entry count (host int, < 2^21)."""
-    import ctypes
-    import numpy as np
     md = np.ascontiguousarray(max_dets, np.int32)
     K, A = npig.shape
     M, R, dev = md.size, rec_thrs.numel(), npig.device
@@ -1137,12 +1021,9 @@ def coco_accumulate_raw(max_dets, cat_entry_begin, cat_pairs, order, entry_rank,
     recall = torch.full((T, K, A, M), -1.0, dtype=torch.float64, device=dev)
     ws_bytes = A * M * num_entries * 20
     ws = torch.empty((max(ws_bytes // 8, 1),), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_coco_accumulate(K, A, M, T, R, md.ctypes.data_as(ctypes.c_void_p), cat_entry_begin.data_ptr(),
-                                                    cat_pairs.data_ptr(), order.data_ptr(), entry_rank.data_ptr(), entry_score.data_ptr(),
-                                                    entry_flags.data_ptr(), num_entries, int(max_cat_entries), npig.data_ptr(), rec_thrs.data_ptr(), ws.data_ptr(),
-                                                    ws_bytes, precision.data_ptr(), recall.data_ptr(), scores.data_ptr(), _stream()),
-                   "b200_coco_accumulate")
+    _launch("b200_coco_accumulate", dev, K, A, M, T, R, md.ctypes.data, cat_entry_begin.data_ptr(), cat_pairs.data_ptr(), order.data_ptr(),
+            entry_rank.data_ptr(), entry_score.data_ptr(), entry_flags.data_ptr(), num_entries, int(max_cat_entries), npig.data_ptr(),
+            rec_thrs.data_ptr(), ws.data_ptr(), ws_bytes, precision.data_ptr(), recall.data_ptr(), scores.data_ptr())
     return precision, recall, scores
 
 
@@ -1155,10 +1036,8 @@ def voc_match_raw(pair_gt_begin, gt_box, gt_difficult, det_pair, det_box, ovthre
     D, G, dev = det_pair.numel(), gt_difficult.numel(), det_pair.device
     outcome = torch.empty((max(D, 1),), dtype=torch.uint8, device=dev)
     ws = torch.empty((max(G, 1),), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_voc_match(D, pair_gt_begin.numel() - 1, G, float(ovthresh), pair_gt_begin.data_ptr(), gt_box.data_ptr(),
-                                              gt_difficult.data_ptr(), det_pair.data_ptr(), det_box.data_ptr(), ws.data_ptr(),
-                                              outcome.data_ptr(), _stream()), "b200_voc_match")
+    _launch("b200_voc_match", dev, D, pair_gt_begin.numel() - 1, G, float(ovthresh), pair_gt_begin.data_ptr(), gt_box.data_ptr(),
+            gt_difficult.data_ptr(), det_pair.data_ptr(), det_box.data_ptr(), ws.data_ptr(), outcome.data_ptr())
     return outcome[:D]
 
 
@@ -1212,14 +1091,11 @@ def box_proposal_match_raw(prop_box, prop_begin, gt_box, gt_area, gt_begin, prop
     excluded = torch.empty((L, A, G), dtype=torch.uint8, device=dev)
     error = torch.empty((L, A, N), dtype=torch.uint8, device=dev)
     counts = torch.zeros((L, A, T), dtype=torch.int64, device=dev)
-    lib = _lib.load()
-    ws = torch.empty((lib.b200_box_proposal_match_workspace_bytes(P, G, A, L),), dtype=torch.uint8, device=dev)
-    ptr = lambda t: t.data_ptr() if t.numel() else None  # noqa: E731
-    with torch.cuda.device(dev):
-        _lib.check(lib.b200_box_proposal_match(N, P, G, A, L, T, ptr(prop_box), prop_begin.data_ptr(), ptr(gt_box), ptr(gt_area),
-                                               gt_begin.data_ptr(), prop_count.data_ptr(), ranges.ctypes.data, ptr(thr), ws.data_ptr(),
-                                               ws.numel(), ptr(overlap), ptr(excluded), error.data_ptr(), ptr(counts), _stream()),
-                   "b200_box_proposal_match")
+    ws_bytes = _lib.load().b200_box_proposal_match_workspace_bytes(P, G, A, L)
+    ws, ws_ptr = _workspace(ws_bytes, dev)
+    _launch("b200_box_proposal_match", dev, N, P, G, A, L, T, _ptr(prop_box), prop_begin.data_ptr(), _ptr(gt_box), _ptr(gt_area),
+            gt_begin.data_ptr(), prop_count.data_ptr(), ranges.ctypes.data, _ptr(thr), ws_ptr, ws_bytes, _ptr(overlap), _ptr(excluded),
+            error.data_ptr(), _ptr(counts))
     return overlap, excluded.bool(), error.bool(), counts
 
 
@@ -1240,7 +1116,7 @@ _loss_workspaces = {}
 def _loss_workspace(dev, num_levels):
     """The zero-filled workspace of the loss kernels, one per (device, stream): the kernels leave it zero after every call, and
     calls on one stream never overlap."""
-    key = (dev.index, _stream())
+    key = (dev.index, _current_stream(dev))
     need = int(_lib.load().b200_loss_workspace_bytes(num_levels))
     ws = _loss_workspaces.get(key)
     if ws is None or ws.numel() < need:
@@ -1285,11 +1161,9 @@ class RpnLossFunction(Function):
         descs = _rpn_levels_desc(cls, bbox, targets, softmax)
         losses = torch.empty((L, 2), dtype=torch.float32, device=dev)
         divisor = torch.empty((L,), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            ws = _loss_workspace(dev, L)
-            _lib.check(_lib.load().b200_rpn_loss_forward(L, ctypes.cast(descs, ctypes.c_void_p), int(softmax), float(fixed_divisor),
-                                                         ws.data_ptr(), ws.numel(), losses.data_ptr(), divisor.data_ptr(), _stream()),
-                       "b200_rpn_loss_forward")
+        ws = _loss_workspace(dev, L)
+        _launch("b200_rpn_loss_forward", dev, L, descs, int(softmax), float(fixed_divisor), ws.data_ptr(), ws.numel(), losses.data_ptr(),
+                divisor.data_ptr())
         ctx.mark_non_differentiable(divisor)
         ctx.L, ctx.softmax = L, softmax
         ctx.save_for_backward(divisor, *tensors)
@@ -1305,9 +1179,7 @@ class RpnLossFunction(Function):
         grads = ([torch.empty_like(c) for c in cls], [torch.empty_like(b) for b in bbox])
         descs = _rpn_levels_desc(cls, bbox, targets, ctx.softmax, grads)
         g = grad_losses.to(torch.float32).contiguous()
-        with torch.cuda.device(g.device):
-            _lib.check(_lib.load().b200_rpn_loss_backward(L, ctypes.cast(descs, ctypes.c_void_p), int(ctx.softmax), g.data_ptr(),
-                                                          divisor.data_ptr(), _stream()), "b200_rpn_loss_backward")
+        _launch("b200_rpn_loss_backward", g.device, L, descs, int(ctx.softmax), g.data_ptr(), divisor.data_ptr())
         return (None, None, None) + tuple(grads[0]) + tuple(grads[1]) + (None,) * (4 * L)
 
 
@@ -1371,12 +1243,10 @@ class FastRcnnLossFunction(Function):
         B = bbox_pred.shape[1]
         losses = torch.empty((2,), dtype=torch.float32, device=dev)
         accuracy = torch.empty((), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            ws = _loss_workspace(dev, 1)
-            _lib.check(_lib.load().b200_fast_rcnn_loss_forward(R, C, B, cls_score.data_ptr(), bbox_pred.data_ptr(), labels.data_ptr(),
-                                                               int(labels.dtype == torch.int64), targets.data_ptr(), inside.data_ptr(),
-                                                               outside.data_ptr(), ws.data_ptr(), ws.numel(), losses.data_ptr(),
-                                                               accuracy.data_ptr(), _stream()), "b200_fast_rcnn_loss_forward")
+        ws = _loss_workspace(dev, 1)
+        _launch("b200_fast_rcnn_loss_forward", dev, R, C, B, cls_score.data_ptr(), bbox_pred.data_ptr(), labels.data_ptr(),
+                int(labels.dtype == torch.int64), targets.data_ptr(), inside.data_ptr(), outside.data_ptr(), ws.data_ptr(), ws.numel(),
+                losses.data_ptr(), accuracy.data_ptr())
         ctx.mark_non_differentiable(accuracy)
         ctx.save_for_backward(cls_score, bbox_pred, labels, targets, inside, outside)
         return losses, accuracy
@@ -1392,12 +1262,9 @@ class FastRcnnLossFunction(Function):
         if d_cls is None and d_bbox is None:
             return None, None, None, None, None, None
         g = grad_losses.to(torch.float32).contiguous()
-        with torch.cuda.device(g.device):
-            _lib.check(_lib.load().b200_fast_rcnn_loss_backward(R, C, B, cls_score.data_ptr(), bbox_pred.data_ptr(), labels.data_ptr(),
-                                                                int(labels.dtype == torch.int64), targets.data_ptr(), inside.data_ptr(),
-                                                                outside.data_ptr(), g.data_ptr(), d_cls.data_ptr() if d_cls is not None else None,
-                                                                d_bbox.data_ptr() if d_bbox is not None else None, _stream()),
-                       "b200_fast_rcnn_loss_backward")
+        _launch("b200_fast_rcnn_loss_backward", g.device, R, C, B, cls_score.data_ptr(), bbox_pred.data_ptr(), labels.data_ptr(),
+                int(labels.dtype == torch.int64), targets.data_ptr(), inside.data_ptr(), outside.data_ptr(), g.data_ptr(), _ptr(d_cls),
+                _ptr(d_bbox))
         return d_cls, d_bbox, None, None, None, None
 
 

@@ -15,8 +15,7 @@ import ctypes
 
 import torch
 
-from .. import _lib
-from ..ops import _need_cuda_f32, _stream
+from ..ops import _host_array, _launch, _need_cuda_f32, _ptr
 
 
 def _boxes4(t, name):
@@ -31,9 +30,7 @@ def bbox_overlaps(boxes, query_boxes):
     boxes = _boxes4(boxes, "boxes"); query_boxes = _boxes4(query_boxes, "query_boxes")
     N, K = boxes.size(0), query_boxes.size(0)
     out = torch.empty((N, K), dtype=torch.float32, device=boxes.device)
-    with torch.cuda.device(boxes.device):
-        _lib.check(_lib.load().b200_bbox_overlaps(boxes.data_ptr(), N, query_boxes.data_ptr(), K, out.data_ptr(), _stream()),
-                   "b200_bbox_overlaps")
+    _launch("b200_bbox_overlaps", boxes.device, boxes.data_ptr(), N, query_boxes.data_ptr(), K, out.data_ptr())
     return out
 
 
@@ -49,10 +46,8 @@ def assign_rois(boxes, gt_boxes, gt_classes):
     if G:
         gt_boxes = _boxes4(gt_boxes, "gt_boxes")
         gt_classes = gt_classes.to(device=dev, dtype=torch.int32).contiguous()
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_roi_assign(boxes.data_ptr(), N, gt_boxes.data_ptr() if G else None,
-                                               gt_classes.data_ptr() if G else None, G, max_overlaps.data_ptr(), argmax.data_ptr(),
-                                               max_classes.data_ptr(), _stream()), "b200_roi_assign")
+    _launch("b200_roi_assign", dev, boxes.data_ptr(), N, gt_boxes.data_ptr() if G else None, gt_classes.data_ptr() if G else None, G,
+            max_overlaps.data_ptr(), argmax.data_ptr(), max_classes.data_ptr())
     return max_overlaps, argmax, max_classes
 
 
@@ -84,9 +79,8 @@ def select_fg_bg(max_overlaps, fg_thresh, bg_thresh_hi, bg_thresh_lo):
     fg = torch.empty((N,), dtype=torch.int32, device=dev)
     bg = torch.empty((N,), dtype=torch.int32, device=dev)
     counts = torch.empty((2,), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_roi_select(max_overlaps.data_ptr(), N, float(fg_thresh), float(bg_thresh_hi), float(bg_thresh_lo),
-                                               fg.data_ptr(), bg.data_ptr(), counts.data_ptr(), _stream()), "b200_roi_select")
+    _launch("b200_roi_select", dev, max_overlaps.data_ptr(), N, float(fg_thresh), float(bg_thresh_hi), float(bg_thresh_lo), fg.data_ptr(),
+            bg.data_ptr(), counts.data_ptr())
     nf, nb = counts.tolist()
     return fg[:nf], bg[:nb]
 
@@ -138,14 +132,13 @@ def _sample_rois(boxes, gt_boxes, gt_classes, im_scale, batch_idx, num_classes, 
     targets = torch.empty((n, 4 * reg_classes), dtype=torch.float32, device=dev)
     inside = torch.empty_like(targets)
     outside = torch.empty_like(targets)
-    w = (ctypes.c_float * 4)(*[float(v) for v in bbox_reg_weights])
+    if len(bbox_reg_weights) != 4:
+        raise ValueError("bbox_reg_weights must be 4 values (wx, wy, ww, wh), got %d" % len(bbox_reg_weights))
+    w = _host_array(ctypes.c_float, [float(v) for v in bbox_reg_weights])
     G = int(gt_boxes.size(0)) if gt_boxes is not None else 0
     gt = _boxes4(gt_boxes, "gt_boxes") if G else None
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().b200_fast_rcnn_targets(boxes.data_ptr(), gt.data_ptr() if G else None, argmax.data_ptr(),
-                                                      max_classes.data_ptr(), keep.data_ptr(), n, n_fg, w, reg_classes,
-                                                      1 if cls_agnostic_bbox_reg else 0, float(im_scale), float(batch_idx),
-                                                      labels.data_ptr(), rois.data_ptr(), targets.data_ptr(), inside.data_ptr(),
-                                                      outside.data_ptr(), _stream()), "b200_fast_rcnn_targets")
+    _launch("b200_fast_rcnn_targets", dev, boxes.data_ptr(), _ptr(gt), argmax.data_ptr(), max_classes.data_ptr(), keep.data_ptr(), n, n_fg,
+            w, reg_classes, 1 if cls_agnostic_bbox_reg else 0, float(im_scale), float(batch_idx), labels.data_ptr(), rois.data_ptr(),
+            targets.data_ptr(), inside.data_ptr(), outside.data_ptr())
     return dict(labels_int32=labels, rois=rois, bbox_targets=targets, bbox_inside_weights=inside, bbox_outside_weights=outside,
                 keep_inds=keep), n_fg

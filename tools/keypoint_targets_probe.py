@@ -19,7 +19,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from detectron.pytorch_b200 import _lib, ops  # noqa: E402
+from detectron.pytorch_b200 import _lib  # noqa: E402
 from detectron.pytorch_b200.roi_data import keypoint_rcnn as KR  # noqa: E402
 from oracle import keypoint_targets as OK  # noqa: E402
 from tests.test_keypoint_targets import coco_image  # noqa: E402
@@ -105,7 +105,7 @@ def main():
     w = torch.empty((2 * FG * K,), device="cuda")
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     ktimes = []
-    s = ops._stream()
+    s = torch.cuda.current_stream().cuda_stream
     for _ in range(a.steps):
         ev[0].record()
         _lib.check(lib.b200_keypoint_candidates(boxes.data_ptr(), mo.data_ptr(), bm.data_ptr(), 2, bb, gi.data_ptr(), gb, kp.data_ptr(), pb,
