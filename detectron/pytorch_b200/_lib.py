@@ -91,6 +91,22 @@ _SIGNATURES = {
     "b200_fast_rcnn_targets": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int,
                                               ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
                                               ctypes.c_void_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _stream_t]),
+    # (rois5, prop_off, gt, gt_off, im_scales, N, box_off, max_rows, boxes, stream)
+    "b200_roi_merge_proposals": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, _c_float_p, ctypes.c_void_p, _c_float_p, ctypes.c_int,
+                                                ctypes.c_void_p, ctypes.c_int, _c_float_p, _stream_t]),
+    # (boxes, box_off, N, max_rows, gt, gt_classes, is_crowd, gt_off, gt_rows_first, max_overlaps, argmax, max_classes, stream)
+    "b200_roi_assign_batched": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, _c_float_p, ctypes.c_void_p,
+                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, _c_float_p, ctypes.c_void_p, ctypes.c_void_p,
+                                               _stream_t]),
+    # (max_overlaps, box_off, N, fg, bg_hi, bg_lo, fg_inds, bg_inds, counts, stream)
+    "b200_roi_select_batched": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_float,
+                                               ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, _stream_t]),
+    # (boxes, gt, argmax, max_classes, keep, keep_off, num_fg, im_scales, batch_idx, N, n, weights4_host, reg_classes, agnostic,
+    #  labels, rois, targets, inside, outside, stream)
+    "b200_fast_rcnn_targets_batched": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p,
+                                                      ctypes.c_void_p, ctypes.c_void_p, _c_float_p, _c_float_p, ctypes.c_int, ctypes.c_int,
+                                                      ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_void_p, _c_float_p, _c_float_p,
+                                                      _c_float_p, _c_float_p, _stream_t]),
     "b200_segm_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int]),
     # (masks, mask_class, boxes, D, Kc, M, im_h, im_w, thresh, sizes_out, workspace, workspace_bytes, stream)
     "b200_segm_rle_sizes": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, _c_float_p] + [ctypes.c_int] * 5 + [ctypes.c_float, ctypes.c_void_p,

@@ -15,14 +15,15 @@ Training branch (:49-63).  The reference "reuses the data loader code": json_dat
 merged into every roidb entry behind its ground-truth boxes, best-gt assignment through cython_bbox.bbox_overlaps,
 crowd_thresh = 0 so nothing is filtered) and roi_data.fast_rcnn.add_fast_rcnn_blobs (_sample_rois per image, concatenation,
 _add_multilevel_rois).  Here the same blobs are produced on the device with roi_data/fast_rcnn.py (SURVEY.md 8f N4); the
-random draws are inputs (`choices`), see there.  With MODEL.MASK_ON the mask blobs (mask_rois, roi_has_mask_int32,
+random draws are inputs (`choices`), see there.  One batched sampler
+(fast_rcnn.add_fast_rcnn_blobs, shared with modeling/generate_proposal_labels.py) labels every image of the minibatch with a
+single host read.  With MODEL.MASK_ON the mask blobs (mask_rois, roi_has_mask_int32,
 masks_int32 and the mask_rois FPN blobs) come from roi_data/mask_rcnn.py, and with MODEL.KEYPOINTS_ON the keypoint blobs
 (keypoint_rois, keypoint_locations_int32, keypoint_weights, keypoint_loss_normalizer and the keypoint_rois FPN blobs) from
 roi_data/keypoint_rcnn.py, on the device too.  Every blob sees the reference's merged roidb (fast_rcnn.roidb_assignment): a
 proposal takes its best ground-truth box, crowd objects included; a ground-truth row maps to itself with overlap 1 and its own
 class, or overlap -1 and class 0 when the entry's 'is_crowd' marks it, so that no crowd row is ever sampled.
 """
-import numpy as np
 import torch
 from torch import nn
 
@@ -99,82 +100,27 @@ class CollectAndDistributeFpnRpnProposalsOp(nn.Module):
         from detectron.pytorch_b200.roi_data import fast_rcnn as FR
         t = dict(train) if train is not None else None
         if t is None:
-            c = self._cfg
-            if c is None:
+            if self._cfg is None:
                 raise ValueError("training needs `train=` (or cfg=) for the TRAIN.* / MODEL.* keys")
-            t = dict(BATCH_SIZE_PER_IM=c.TRAIN.BATCH_SIZE_PER_IM, FG_FRACTION=c.TRAIN.FG_FRACTION, FG_THRESH=c.TRAIN.FG_THRESH,
-                     BG_THRESH_HI=c.TRAIN.BG_THRESH_HI, BG_THRESH_LO=c.TRAIN.BG_THRESH_LO, NUM_CLASSES=c.MODEL.NUM_CLASSES,
-                     BBOX_REG_WEIGHTS=c.MODEL.BBOX_REG_WEIGHTS, CLS_AGNOSTIC_BBOX_REG=c.MODEL.CLS_AGNOSTIC_BBOX_REG)
-            if getattr(c.MODEL, "MASK_ON", False):
-                t.update(MASK_ON=True, MRCNN_RESOLUTION=c.MRCNN.RESOLUTION, CLS_SPECIFIC_MASK=c.MRCNN.CLS_SPECIFIC_MASK)
-            if getattr(c.MODEL, "KEYPOINTS_ON", False):
-                t.update(KEYPOINTS_ON=True, HEATMAP_SIZE=c.KRCNN.HEATMAP_SIZE, NUM_KEYPOINTS=c.KRCNN.NUM_KEYPOINTS,
-                         IMS_PER_BATCH=c.TRAIN.IMS_PER_BATCH, MIN_KEYPOINT_COUNT=c.KRCNN.MIN_KEYPOINT_COUNT_FOR_VALID_MINIBATCH)
-        dev = rois.device
-        im_info = torch.as_tensor(im_info, dtype=torch.float32)
-        scales = im_info[:, 2].cpu()
+            t = FR.train_keys(self._cfg)
+        scales = torch.as_tensor(im_info, dtype=torch.float32)[:, 2].cpu()
+        blobs = FR.add_fast_rcnn_blobs(rois, roidb, [float(s) for s in scales], t, choices)
         mask_on = bool(t.get("MASK_ON", False))
         kp_on = bool(t.get("KEYPOINTS_ON", False))
-        per_image, sampled, num_fg = [], [], []
-        kp_boxes, kp_overlaps, kp_map, kp_choices = [], [], [], []
-        for i, entry in enumerate(roidb):
-            gt = torch.as_tensor(entry["boxes"], dtype=torch.float32).to(dev).reshape(-1, 4)
-            gcls = torch.as_tensor(entry["gt_classes"]).to(device=dev, dtype=torch.int32).reshape(-1)
-            keep_gt = gcls > 0
-            gt, gcls = gt[keep_gt], gcls[keep_gt]
-            crowd = torch.as_tensor(entry["is_crowd"]).to(dev).reshape(-1)[keep_gt] if "is_crowd" in entry else None
-            inv = (torch.ones((), dtype=torch.float32) / scales[i]).item()           # json_dataset.py:420: 1. / scales[i] in float32
-            props = rois[rois[:, 0] == i][:, 1:5] * inv                              # add_proposals: back to image coordinates
-            boxes = torch.cat([gt, props]).contiguous()
-            ch = tuple(choices[i]) if choices is not None else (None, None)
-            fg_c, bg_c = ch[0], ch[1]
-            assignment = FR.roidb_assignment(boxes, gt, gcls, crowd)
-            b, nf = FR._sample_rois(boxes, gt, gcls, float(scales[i]), i, t["NUM_CLASSES"], t["BATCH_SIZE_PER_IM"], t["FG_FRACTION"],
-                                    t["FG_THRESH"], t["BG_THRESH_HI"], t["BG_THRESH_LO"], t["BBOX_REG_WEIGHTS"],
-                                    t["CLS_AGNOSTIC_BBOX_REG"], fg_c, bg_c, assignment)
-            if kp_on:
-                # add_keypoint_rcnn_blobs reads box_to_gt_ind_map as roidb rows: the assigned gt index through gt_inds
-                gt_inds = np.where(np.asarray(entry["gt_classes"]).reshape(-1) > 0)[0]
-                gi = torch.from_numpy(gt_inds.astype(np.int32)).to(dev)
-                mo, am = assignment[0], assignment[1]
-                kp_boxes.append(boxes)
-                kp_overlaps.append(mo)
-                kp_map.append(torch.where(am >= 0, gi[am.clamp(min=0).long()], am) if gt_inds.size else am)
-                kp_choices.append(ch[2] if len(ch) > 2 else None)
-            per_image.append(b)
-            if mask_on:                                                              # add_mask_rcnn_blobs' sampled_boxes (unscaled)
-                sampled.append(boxes[b["keep_inds"].long()])
-                num_fg.append(nf)
-        blobs = {k: torch.cat([b[k] for b in per_image]) for k in
-                 ("labels_int32", "rois", "bbox_targets", "bbox_inside_weights", "bbox_outside_weights")}
         # roi_data/fast_rcnn.py:251-283 (_add_multilevel_rois): the sampled rois go to their FPN levels
         d = distribute(blobs["rois"], p["roi_min"], p["roi_max"], p["s0"], p["k0"])
         for k, v in d.items():
             if k != "rois":
                 blobs[k] = v
         if mask_on:
-            # roi_data/mask_rcnn.py:34-122 per image, concatenated, then fast_rcnn.py:275-276: mask_rois to their FPN levels
-            from detectron.pytorch_b200.roi_data import mask_rcnn as MR
-            mb = MR.mask_rcnn_blobs([b["labels_int32"] for b in per_image], [b["rois"] for b in per_image], sampled, num_fg, roidb,
-                                    t.get("MRCNN_RESOLUTION", 14), t.get("CLS_SPECIFIC_MASK", True), t["NUM_CLASSES"])
-            blobs.update(mb)
-            d = distribute(mb["mask_rois"], p["roi_min"], p["roi_max"], p["s0"], p["k0"])
+            # fast_rcnn.py:275-276: mask_rois to their FPN levels
+            d = distribute(blobs["mask_rois"], p["roi_min"], p["roi_max"], p["s0"], p["k0"])
             for k, v in d.items():
                 if k not in ("rois", "counts"):
                     blobs["mask_" + k] = v
         if kp_on:
-            # roi_data/keypoint_rcnn.py:33-96 for every image in one device call, then fast_rcnn.py:277-278: keypoint_rois to their
-            # FPN levels
-            from detectron.pytorch_b200.roi_data import keypoint_rcnn as KR
-            box_begin = np.concatenate([[0], np.cumsum([bx.size(0) for bx in kp_boxes])])
-            kb = KR.keypoint_rcnn_blobs(torch.cat(kp_boxes), box_begin, torch.cat(kp_overlaps), torch.cat(kp_map), roidb,
-                                        [float(s) for s in scales], int(round(t["FG_FRACTION"] * int(t["BATCH_SIZE_PER_IM"]))),
-                                        t["HEATMAP_SIZE"], t["NUM_KEYPOINTS"], t["FG_THRESH"], choices=kp_choices)
-            KR.finalize_keypoint_minibatch(kb, True, ims_per_batch=t.get("IMS_PER_BATCH", 2), batch_size_per_im=t["BATCH_SIZE_PER_IM"],
-                                           fg_fraction=t["FG_FRACTION"], num_keypoints=t["NUM_KEYPOINTS"],
-                                           min_count=t.get("MIN_KEYPOINT_COUNT", 20))
-            blobs.update(kb)
-            d = distribute(kb["keypoint_rois"], p["roi_min"], p["roi_max"], p["s0"], p["k0"])
+            # fast_rcnn.py:277-278: keypoint_rois to their FPN levels
+            d = distribute(blobs["keypoint_rois"], p["roi_min"], p["roi_max"], p["s0"], p["k0"])
             for k, v in d.items():
                 if k not in ("rois", "counts"):
                     blobs["keypoint_" + k] = v

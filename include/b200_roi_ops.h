@@ -323,7 +323,20 @@ B200_API int b200_topk_batched(const float* const* scores_dev_ptrs_host, const i
  *                       background ([bg_lo, bg_hi)) boxes, counts_out = {num_fg, num_bg}.
  * b200_fast_rcnn_targets  fast_rcnn.py:161-187 + :203-248 for the kept rows (the first num_fg are foreground): labels
  *                       (int32), rois (batch_idx, box * im_scale), regression targets (utils/boxes.py:199-230) expanded
- *                       to 4 * num_reg_classes columns, inside / outside weights.  bbox_reg_weights_host: 4 floats. */
+ *                       to 4 * num_reg_classes columns, inside / outside weights.  bbox_reg_weights_host: 4 floats.
+ * The *_batched entry points do the same for a minibatch of N images in one launch each.  Image b owns the rows
+ * box_off[b] .. box_off[b + 1] - 1 of the merged boxes (its ground truth first, then its proposals, unscaled) and the rows
+ * gt_off[b] .. gt_off[b + 1] - 1 of the concatenated ground truth; offsets are (N + 1) ascending int32 in device memory, and
+ * max_rows bounds box_off[N] (rows past box_off[N] are left alone).
+ * b200_roi_merge_proposals  json_dataset.py:417-425: the merged boxes from rois5_dev (R, 5), grouped by image (image b's in
+ *                       rows prop_off[b] .. prop_off[b + 1] - 1), each times the float32 1 / im_scales[b].
+ * b200_roi_assign_batched   b200_roi_assign against the row's own image's ground truth (argmax indexes the concatenated
+ *                       ground truth); gt_rows_first: a ground-truth row keeps overlap 1 and its class, or -1 and class 0
+ *                       where is_crowd (int32 flags; may be null) marks it.
+ * b200_roi_select_batched   b200_roi_select per image (one CTA each): image b's lists hold its own row indices, written
+ *                       from row box_off[b] on; counts_out (N, 2).
+ * b200_fast_rcnn_targets_batched  b200_fast_rcnn_targets for n kept merged rows, image b's being keep_off[b] ..
+ *                       keep_off[b + 1] - 1 with its first num_fg[b] foreground, im_scales[b] and batch_idx[b]. */
 B200_API int b200_bbox_overlaps(const float* boxes_dev, int num_boxes, const float* query_boxes_dev, int num_query,
                                 float* overlaps_out_dev, b200_stream_t stream);
 B200_API int b200_roi_assign(const float* boxes_dev, int num_boxes, const float* gt_boxes_dev, const int* gt_classes_dev, int num_gt,
@@ -335,6 +348,21 @@ B200_API int b200_fast_rcnn_targets(const float* boxes_dev, const float* gt_boxe
                                     int num_reg_classes, int cls_agnostic, float im_scale, float batch_idx, int* labels_out_dev,
                                     float* rois_out_dev, float* bbox_targets_out_dev, float* inside_weights_out_dev,
                                     float* outside_weights_out_dev, b200_stream_t stream);
+B200_API int b200_roi_merge_proposals(const float* rois5_dev, const int* prop_off_dev, const float* gt_boxes_dev, const int* gt_off_dev,
+                                      const float* im_scales_dev, int num_images, const int* box_off_dev, int max_rows,
+                                      float* boxes_out_dev, b200_stream_t stream);
+B200_API int b200_roi_assign_batched(const float* boxes_dev, const int* box_off_dev, int num_images, int max_rows, const float* gt_boxes_dev,
+                                     const int* gt_classes_dev, const int* is_crowd_dev, const int* gt_off_dev, int gt_rows_first,
+                                     float* max_overlaps_out_dev, int* argmax_out_dev, int* max_classes_out_dev, b200_stream_t stream);
+B200_API int b200_roi_select_batched(const float* max_overlaps_dev, const int* box_off_dev, int num_images, float fg_thresh,
+                                     float bg_thresh_hi, float bg_thresh_lo, int* fg_inds_out_dev, int* bg_inds_out_dev,
+                                     int* counts_out_dev, b200_stream_t stream);
+B200_API int b200_fast_rcnn_targets_batched(const float* boxes_dev, const float* gt_boxes_dev, const int* argmax_dev,
+                                            const int* max_classes_dev, const int* keep_inds_dev, const int* keep_off_dev,
+                                            const int* num_fg_dev, const float* im_scales_dev, const float* batch_idx_dev, int num_images,
+                                            int num_keep, const float* bbox_reg_weights_host, int num_reg_classes, int cls_agnostic,
+                                            int* labels_out_dev, float* rois_out_dev, float* bbox_targets_out_dev,
+                                            float* inside_weights_out_dev, float* outside_weights_out_dev, b200_stream_t stream);
 
 /* ---- RPN anchor labels and box-regression targets (training, lib/roi_data/rpn.py:40-261) -------------------------------
  * add_rpn_blobs / _get_rpn_blobs for all images and all anchor levels of a step, in a fixed number of launches.
