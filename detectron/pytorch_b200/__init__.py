@@ -13,7 +13,8 @@ or, to make an unmodified checkout of the reference pick these up under ITS impo
 __version__ = "0.1.0"
 
 
-def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False, voc=False, losses=False):
+def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False, voc=False, losses=False,
+                              test_aug=False):
     """Register this package's op modules in sys.modules under the reference's import paths.
 
     After this, `from modeling.roi_xfrom.roi_align.functions.roi_align import RoIAlignFunction`
@@ -80,6 +81,14 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
         ref_boxes = importlib.import_module("utils.boxes")          # the reference's module
         ref_boxes.nms = importlib.import_module(__name__ + ".utils.boxes").nms
         installed.append("utils.boxes.nms")
+    segms = segms or test_aug
+    keypoints = keypoints or test_aug
+    if test_aug:
+        ref_test = importlib.import_module("core.test")              # the reference's module
+        ours_test = importlib.import_module(__name__ + ".core.test")
+        for name in ("im_detect_mask", "im_detect_mask_aug", "im_detect_keypoints", "im_detect_keypoints_aug"):
+            setattr(ref_test, name, (lambda f: lambda *a: f(*a, cfg=ref_test.cfg))(getattr(ours_test, name)))
+            installed.append("core.test." + name)
     if segms:
         ref_test = importlib.import_module("core.test")              # the reference's module
         ours = importlib.import_module(__name__ + ".core.test").segm_results

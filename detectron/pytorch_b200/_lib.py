@@ -149,6 +149,12 @@ _SIGNATURES = {
     # (src, descs, N, mean_table, blob_h, blob_w, out, stream)
     "b200_image_blob": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_int,
                                        _c_float_p, _stream_t]),
+    # (src, acc, R, C, M, channel_perm, row_op, op, hflip, heur, stream)
+    "b200_tta_combine": (ctypes.c_int, [_c_float_p, _c_float_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] * 2 + [ctypes.c_int] * 3 + [_stream_t]),
+    # (acc, R, C, M, row_count, count, heur, stream)
+    "b200_tta_finish": (ctypes.c_int, [_c_float_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] + [ctypes.c_int] * 2 + [_stream_t]),
+    # (src, src_pitch, height, width, out_width, dst, stream)
+    "b200_resize_width_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_longlong] + [ctypes.c_int] * 3 + [ctypes.c_void_p, _stream_t]),
     # (P, pair_det_begin, pair_entry_begin, det_score, entry_det, entry_rank, entry_score, stream)
     "b200_coco_rank": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 6 + [_stream_t]),
     # (P, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_box, gt_box, gt_flags, ious, stream)

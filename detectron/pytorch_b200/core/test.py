@@ -32,6 +32,10 @@ the optional OKS NMS), with one host read of the (R, 4, 17) result; the result i
 
 `get_blobs(im, rois, target_scale, target_max_size)` is _get_blobs with _get_rois_blob (lib/core/test.py:869-929): the `data` blob
 is built on the device from the uint8 image (utils/blob.py).
+
+`im_detect_mask_aug` / `im_detect_keypoints_aug` (lib/core/test.py:365-729) run the heads over the test-time transforms in the
+reference's order, build every transform's blob on the device and fold each head output into one running CUDA accumulator
+(ops.tta_combine_raw); the combined masks / heatmaps are CUDA tensors for segm_results / keypoint_results.
 """
 import numpy as np
 import torch
@@ -238,3 +242,315 @@ def get_blobs(im, rois, target_scale, target_max_size, cfg=None, **kw):
         levels = np.zeros((r.shape[0], 1), dtype=np.int64)
         blobs["rois"] = np.hstack((levels, r)).astype(np.float32, copy=False)
     return blobs, im_scale
+
+
+# ------------------------------------------------------------------------------------------------
+# Test-time augmentation of the mask and keypoint heads (lib/core/test.py:365-729)
+# ------------------------------------------------------------------------------------------------
+_MASK_HEURS = ("SOFT_AVG", "SOFT_MAX", "LOGIT_AVG")
+_KPS_HEURS = ("HM_AVG", "HM_MAX")
+
+
+def _aug_params(cfg, kw):
+    """The configuration the mask / keypoint test-time functions read (flat keys; `mask_aug` / `kps_aug` hold TEST.MASK_AUG /
+    TEST.KPS_AUG as dicts of lower-case keys).  From the reference's `cfg` at call time, else the reference's defaults
+    (lib/core/config.py), then the keyword arguments.  Blob keys (pixel_means, fpn_on, coarsest_stride) go to utils/blob.py."""
+    def aug(a):
+        return dict(heur=a.HEUR, h_flip=a.H_FLIP, scales=tuple(a.SCALES), max_size=a.MAX_SIZE, scale_h_flip=a.SCALE_H_FLIP,
+                    scale_size_dep=a.SCALE_SIZE_DEP, area_th=a.AREA_TH, aspect_ratios=tuple(a.ASPECT_RATIOS),
+                    aspect_ratio_h_flip=a.ASPECT_RATIO_H_FLIP)
+    if cfg is not None:
+        p = dict(num_classes=cfg.MODEL.NUM_CLASSES, resolution=cfg.MRCNN.RESOLUTION, cls_specific_mask=cfg.MRCNN.CLS_SPECIFIC_MASK,
+                 num_keypoints=cfg.KRCNN.NUM_KEYPOINTS, heatmap_size=cfg.KRCNN.HEATMAP_SIZE, test_scale=cfg.TEST.SCALE,
+                 test_max_size=cfg.TEST.MAX_SIZE, multilevel_rois=cfg.FPN.MULTILEVEL_ROIS, roi_min_level=cfg.FPN.ROI_MIN_LEVEL,
+                 roi_max_level=cfg.FPN.ROI_MAX_LEVEL, roi_canonical_scale=cfg.FPN.ROI_CANONICAL_SCALE,
+                 roi_canonical_level=cfg.FPN.ROI_CANONICAL_LEVEL, mask_aug=aug(cfg.TEST.MASK_AUG), kps_aug=aug(cfg.TEST.KPS_AUG),
+                 blob=dict(pixel_means=cfg.PIXEL_MEANS, fpn_on=bool(cfg.FPN.FPN_ON), coarsest_stride=int(cfg.FPN.COARSEST_STRIDE)))
+    else:
+        from ..utils.blob import blob_params
+        defaults = dict(heur=None, h_flip=False, scales=(), max_size=4000, scale_h_flip=False, scale_size_dep=False, area_th=180 ** 2,
+                        aspect_ratios=(), aspect_ratio_h_flip=False)             # lib/core/config.py:289-354
+        p = dict(num_classes=None, resolution=14, cls_specific_mask=True, num_keypoints=17, heatmap_size=56, test_scale=600,
+                 test_max_size=1000, multilevel_rois=False, roi_min_level=2, roi_max_level=5, roi_canonical_scale=224,
+                 roi_canonical_level=4, mask_aug=dict(defaults, heur="SOFT_AVG"), kps_aug=dict(defaults, heur="HM_AVG"),
+                 blob=blob_params())
+    for key in ("mask_aug", "kps_aug", "blob"):
+        p[key] = dict(p[key], **kw.pop(key, {}))
+    for key in ("pixel_means", "fpn_on", "coarsest_stride"):
+        if key in kw:
+            p["blob"][key] = kw.pop(key)
+    unknown = set(kw) - set(p)
+    if unknown:
+        raise TypeError("unexpected configuration keywords %s" % sorted(unknown))
+    p.update(kw)
+    return p
+
+
+def _get_rois_blob(im_rois, im_scale):
+    """lib/core/test.py:869-898: (R, 5) float32 [0, x1, y1, x2, y2], the boxes multiplied by im_scale in float64."""
+    rois = np.asarray(im_rois).astype(np.float64, copy=False) * im_scale
+    levels = np.zeros((rois.shape[0], 1), dtype=np.int64)
+    return np.hstack((levels, rois)).astype(np.float32, copy=False)
+
+
+def _add_multilevel_rois_for_test(blobs, name, p):
+    """lib/core/test.py:901-920 with lib/utils/fpn.py: blobs[name + '_fpn<l>'] the rows of blobs[name] whose FPN level is l
+    (numpy's float32 Eqn. (1) of the FPN paper, as the reference evaluates it) and blobs[name + '_idx_restore_int32'] the
+    permutation back to the original order.  Host numpy: these are a few hundred rows, and the RoI transform reads them there."""
+    lvl_min, lvl_max = int(p["roi_min_level"]), int(p["roi_max_level"])
+    rois = blobs[name]
+    boxes = rois[:, 1:5]
+    areas = (boxes[:, 2] - boxes[:, 0] + 1) * (boxes[:, 3] - boxes[:, 1] + 1)
+    areas[areas < 0] = 0
+    s = np.sqrt(areas)
+    lvls = np.clip(np.floor(p["roi_canonical_level"] + np.log2(s / p["roi_canonical_scale"] + 1e-6)), lvl_min, lvl_max)
+    idx_order = np.empty((0,))
+    for lvl in range(lvl_min, lvl_max + 1):
+        idx_lvl = np.where(lvls == lvl)[0]
+        blobs[name + "_fpn" + str(lvl)] = rois[idx_lvl, :]
+        idx_order = np.concatenate((idx_order, idx_lvl))
+    blobs[name + "_idx_restore_int32"] = np.argsort(idx_order).astype(np.int32, copy=False)
+
+
+class _RunningCombine:
+    """The reference's list of per-transform head outputs and its np.mean / np.amax (or logit mean) over them, kept as one
+    running (R, C, M, M) CUDA accumulator that each transform is folded into as it arrives (ops.tta_combine_raw): a transform is
+    read once, mirrored and channel-permuted in that read when it came from a flipped image.  `include` (R,) bool selects the
+    rows a transform takes part in (combine_heatmaps_size_dep); every row must be included at least once."""
+
+    def __init__(self, heur):
+        self.heur = ops.TTA_HEURISTICS[heur]
+        self.acc = None
+        self.count = None
+
+    def add(self, out, hflip=False, perm=None, include=None):
+        if self.acc is None:
+            self.acc = torch.empty(out.shape, dtype=torch.float32, device=out.device)
+            self.count = np.zeros((out.shape[0],), dtype=np.int64)
+        if self.acc.numel() == 0:
+            return
+        row_op, op = None, ops.TTA_FOLD if self.count.any() else ops.TTA_START
+        if include is not None:
+            include = np.asarray(include, dtype=bool)
+            ops_host = np.where(include, np.where(self.count == 0, ops.TTA_START, ops.TTA_FOLD), ops.TTA_SKIP).astype(np.uint8)
+            row_op = torch.from_numpy(ops_host).to(out.device)
+            self.count += include
+        else:
+            if self.count.any() and not self.count.all():
+                raise ValueError("a transform for every row after one for some rows")
+            self.count += 1
+        ops.tta_combine_raw(out, self.acc, self.heur, op=op, hflip=hflip, channel_perm=perm, row_op=row_op)
+
+    def result(self):
+        if self.acc.numel() == 0:
+            return self.acc
+        if (self.count < 1).any():
+            raise ValueError("every row needs at least one transform")
+        if (self.count == self.count[0]).all():
+            return ops.tta_finish_raw(self.acc, self.heur, count=int(self.count[0]))
+        return ops.tta_finish_raw(self.acc, self.heur, row_count=torch.from_numpy(self.count.astype(np.int32)))
+
+
+def _conv_body(model, im, target_scale, target_max_size, hflip, p):
+    """im_conv_body_only on the image, or on im[:, ::-1, :] when hflip (the blob kernel's flip flag reads it mirrored)."""
+    from ..utils import blob as blob_utils
+    h, w = int(im.shape[0]), int(im.shape[1])
+    im_scale = blob_utils.get_target_scale(min(h, w), max(h, w), target_scale, target_max_size)
+    bp = p["blob"]
+    data, _ = ops.image_blob_raw([im], [im_scale], [hflip], bp["pixel_means"], bp["coarsest_stride"] if bp["fpn_on"] else None)
+    blob_conv = model.module.convbody_net(data=data)
+    return blob_conv, im_scale
+
+
+def im_conv_body_only(model, im, target_scale, target_max_size, cfg=None, **kw):
+    """lib/core/test.py:117-129: the backbone on the device blob of im (uint8 (H, W, 3), host or CUDA).  Returns (blob_conv, im_scale)."""
+    return _conv_body(model, im, target_scale, target_max_size, False, _aug_params(cfg, kw))
+
+
+def _head_inputs(name, boxes, im_scale, p):
+    inputs = {name: _get_rois_blob(boxes, im_scale)}
+    if p["multilevel_rois"]:
+        _add_multilevel_rois_for_test(inputs, name, p)
+    return inputs
+
+
+def _detect_mask(model, im_scale, boxes, blob_conv, p):
+    M = int(p["resolution"])
+    if boxes.shape[0] == 0:
+        return torch.zeros((0, M, M), dtype=torch.float32, device=torch.device("cuda", torch.cuda.current_device()))
+    pred_masks = model.module.mask_net(blob_conv, _head_inputs("mask_rois", boxes, im_scale, p))
+    return pred_masks.detach().to(torch.float32).reshape(boxes.shape[0], -1, M, M)
+
+
+def _detect_keypoints(model, im_scale, boxes, blob_conv, p):
+    M = int(p["heatmap_size"])
+    if boxes.shape[0] == 0:
+        return torch.zeros((0, int(p["num_keypoints"]), M, M), dtype=torch.float32, device=torch.device("cuda", torch.cuda.current_device()))
+    pred_heatmaps = model.module.keypoint_net(blob_conv, _head_inputs("keypoint_rois", boxes, im_scale, p))
+    return pred_heatmaps.detach().to(torch.float32).reshape(boxes.shape[0], -1, M, M)
+
+
+def _transform(out, hflip, perm):
+    """A flipped transform's output as the reference returns it (masks[..., ::-1] / flip_heatmaps), in one copy kernel."""
+    if not hflip:
+        return out
+    return ops.tta_combine_raw(out, torch.empty(out.shape, dtype=torch.float32, device=out.device), ops.TTA_HEURISTICS["HM_MAX"],
+                               op=ops.TTA_START, hflip=True, channel_perm=perm)
+
+
+def _flip_perm(kind, J):
+    if kind == "mask":
+        return None
+    from ..utils.keypoints import flip_permutation
+    return flip_permutation(J)
+
+
+def _detect(kind, model, im_scale, boxes, blob_conv, p):
+    return (_detect_mask if kind == "mask" else _detect_keypoints)(model, im_scale, boxes, blob_conv, p)
+
+
+def _hflip_raw(kind, model, im, target_scale, target_max_size, boxes, p):
+    """im_detect_<kind>_hflip without the final inversion: the head output on the flipped image (the caller mirrors it)."""
+    from ..utils.boxes import flip_boxes
+    boxes_hf = flip_boxes(boxes, int(im.shape[1]))
+    blob_conv, im_scale = _conv_body(model, im, target_scale, target_max_size, True, p)
+    return _detect(kind, model, im_scale, boxes_hf, blob_conv, p)
+
+
+def _scale_raw(kind, model, im, target_scale, target_max_size, boxes, hflip, p):
+    if hflip:
+        return _hflip_raw(kind, model, im, target_scale, target_max_size, boxes, p)
+    blob_conv, im_scale = _conv_body(model, im, target_scale, target_max_size, False, p)
+    return _detect(kind, model, im_scale, boxes, blob_conv, p)
+
+
+def _aspect_ratio_raw(kind, model, im, aspect_ratio, boxes, hflip, p):
+    from ..utils.boxes import aspect_ratio as boxes_aspect_ratio
+    from ..utils.image import aspect_ratio_rel
+    im_ar = aspect_ratio_rel(im, aspect_ratio)
+    boxes_ar = boxes_aspect_ratio(boxes, aspect_ratio)
+    return _scale_raw(kind, model, im_ar, p["test_scale"], p["test_max_size"], boxes_ar, hflip, p)
+
+
+def _size_dep_include(boxes, ds_t, us_t, area_th):
+    """combine_heatmaps_size_dep's selection: a downscaled transform is left out for small and medium objects (area < AREA_TH),
+    an upscaled one for large objects.  Areas are the reference's float32 `+ 1` box areas."""
+    b = np.asarray(boxes)
+    areas = (b[:, 2] - b[:, 0] + 1) * (b[:, 3] - b[:, 1] + 1)
+    sm_objs = areas < area_th
+    l_objs = areas >= area_th
+    return ~((sm_objs & bool(ds_t)) | (l_objs & bool(us_t)))
+
+
+def _aug(kind, model, im, boxes, im_scale, blob_conv, p):
+    """The transform loop of im_detect_mask_aug / im_detect_keypoints_aug, in the reference's order, folding each output into
+    the running combine as it arrives."""
+    a = p["mask_aug" if kind == "mask" else "kps_aug"]
+    if kind == "mask":
+        assert not a["scale_size_dep"], 'Size dependent scaling not implemented'
+    if a["heur"] not in (_MASK_HEURS if kind == "mask" else _KPS_HEURS):
+        raise NotImplementedError('Heuristic {} not supported'.format(a["heur"]))
+    size_dep = kind == "keypoints" and a["scale_size_dep"]
+    comb = _RunningCombine(a["heur"])
+    perm = [None]
+
+    def add(out, hflip=False, ds_t=False, us_t=False):
+        if hflip and perm[0] is None and kind != "mask":
+            perm[0] = _flip_perm(kind, out.shape[1])
+        comb.add(out, hflip=hflip, perm=perm[0] if hflip else None,
+                 include=_size_dep_include(boxes, ds_t, us_t, a["area_th"]) if size_dep else None)
+
+    add(_detect(kind, model, im_scale, boxes, blob_conv, p))
+    if a["h_flip"]:
+        add(_hflip_raw(kind, model, im, p["test_scale"], p["test_max_size"], boxes, p), hflip=True)
+    for scale in a["scales"]:
+        ds_scl, us_scl = scale < p["test_scale"], scale > p["test_scale"]
+        add(_scale_raw(kind, model, im, scale, a["max_size"], boxes, False, p), ds_t=ds_scl, us_t=us_scl)
+        if a["scale_h_flip"]:
+            add(_scale_raw(kind, model, im, scale, a["max_size"], boxes, True, p), hflip=True, ds_t=ds_scl, us_t=us_scl)
+    for aspect_ratio in a["aspect_ratios"]:
+        add(_aspect_ratio_raw(kind, model, im, aspect_ratio, boxes, False, p))
+        if a["aspect_ratio_h_flip"]:
+            add(_aspect_ratio_raw(kind, model, im, aspect_ratio, boxes, True, p), hflip=True)
+    return comb.result()
+
+
+def im_detect_mask(model, im_scale, boxes, blob_conv, cfg=None, **kw):
+    """lib/core/test.py:365-401: the mask head on boxes (R, 4) projected by im_scale (host rois / FPN blobs, like the reference).
+    Returns the soft masks as a float32 CUDA tensor (R, Kc, M, M), which segm_results takes without a copy to the host."""
+    return _detect_mask(model, im_scale, boxes, blob_conv, _aug_params(cfg, kw))
+
+
+def im_detect_mask_aug(model, im, boxes, im_scale, blob_conv, cfg=None, **kw):
+    """lib/core/test.py:404-475: the soft masks combined over TEST.MASK_AUG's transforms (identity, H_FLIP, SCALES with
+    SCALE_H_FLIP, ASPECT_RATIOS with ASPECT_RATIO_H_FLIP) by HEUR, the model called in the reference's order.  The
+    transforms are combined on the device as they arrive.  Returns a float32 CUDA tensor (R, Kc, M, M).  An unknown HEUR
+    raises NotImplementedError before the first transform runs (the reference raises after the last)."""
+    return _aug("mask", model, im, boxes, im_scale, blob_conv, _aug_params(cfg, kw))
+
+
+def im_detect_mask_hflip(model, im, target_scale, target_max_size, boxes, cfg=None, **kw):
+    """lib/core/test.py:478-492: masks of the flipped image, mirrored back.  float32 CUDA (R, Kc, M, M)."""
+    return _transform(_hflip_raw("mask", model, im, target_scale, target_max_size, boxes, _aug_params(cfg, kw)), True, None)
+
+
+def im_detect_mask_scale(model, im, target_scale, target_max_size, boxes, hflip=False, cfg=None, **kw):
+    """lib/core/test.py:495-505."""
+    return _transform(_scale_raw("mask", model, im, target_scale, target_max_size, boxes, hflip, _aug_params(cfg, kw)), hflip, None)
+
+
+def im_detect_mask_aspect_ratio(model, im, aspect_ratio, boxes, hflip=False, cfg=None, **kw):
+    """lib/core/test.py:508-526: the image resized by utils/image.py aspect_ratio_rel on the device."""
+    return _transform(_aspect_ratio_raw("mask", model, im, aspect_ratio, boxes, hflip, _aug_params(cfg, kw)), hflip, None)
+
+
+def im_detect_keypoints(model, im_scale, boxes, blob_conv, cfg=None, **kw):
+    """lib/core/test.py:529-563: the keypoint head's logits as a float32 CUDA tensor (R, J, M, M), which keypoint_results takes
+    without a copy to the host."""
+    return _detect_keypoints(model, im_scale, boxes, blob_conv, _aug_params(cfg, kw))
+
+
+def im_detect_keypoints_aug(model, im, boxes, im_scale, blob_conv, cfg=None, **kw):
+    """lib/core/test.py:566-647: the heatmaps combined over TEST.KPS_AUG's transforms by HEUR (HM_AVG / HM_MAX), with
+    SCALE_SIZE_DEP's per-object selection, on the device.  Returns a float32 CUDA tensor (R, J, M, M).
+
+    With SCALE_SIZE_DEP the reference's combine_heatmaps_size_dep fails under this version of its utils.boxes.boxes_area,
+    which returns (areas, negative indices); here the areas are used, as the selection intends."""
+    return _aug("keypoints", model, im, boxes, im_scale, blob_conv, _aug_params(cfg, kw))
+
+
+def im_detect_keypoints_hflip(model, im, target_scale, target_max_size, boxes, cfg=None, **kw):
+    """lib/core/test.py:650-664: heatmaps of the flipped image, inverted by flip_heatmaps (one copy kernel)."""
+    p = _aug_params(cfg, kw)
+    out = _hflip_raw("keypoints", model, im, target_scale, target_max_size, boxes, p)
+    return _transform(out, True, _flip_perm("keypoints", out.shape[1]))
+
+
+def im_detect_keypoints_scale(model, im, target_scale, target_max_size, boxes, hflip=False, cfg=None, **kw):
+    """lib/core/test.py:667-677."""
+    out = _scale_raw("keypoints", model, im, target_scale, target_max_size, boxes, hflip, _aug_params(cfg, kw))
+    return _transform(out, hflip, _flip_perm("keypoints", out.shape[1]) if hflip else None)
+
+
+def im_detect_keypoints_aspect_ratio(model, im, aspect_ratio, boxes, hflip=False, cfg=None, **kw):
+    """lib/core/test.py:680-697."""
+    out = _aspect_ratio_raw("keypoints", model, im, aspect_ratio, boxes, hflip, _aug_params(cfg, kw))
+    return _transform(out, hflip, _flip_perm("keypoints", out.shape[1]) if hflip else None)
+
+
+def combine_heatmaps_size_dep(hms_ts, ds_ts, us_ts, boxes, heur, cfg=None, **kw):
+    """lib/core/test.py:700-729: per object, the heatmaps of the transforms it keeps (no downscaled ones for objects with
+    area < KPS_AUG.AREA_TH, no upscaled ones for the others) combined by heur ('HM_AVG' / 'HM_MAX', or np.mean / np.amax).
+    hms_ts: (R, J, M, M) float32 CUDA tensors (or numpy).  Returns a float32 CUDA tensor."""
+    assert len(hms_ts) == len(ds_ts) and len(ds_ts) == len(us_ts), \
+        'All sets of hms must be tagged with downscaling and upscaling flags'
+    p = _aug_params(cfg, kw)
+    heur = {np.mean: "HM_AVG", np.amax: "HM_MAX", np.max: "HM_MAX"}.get(heur, heur)
+    if heur not in _KPS_HEURS:
+        raise NotImplementedError('Heuristic {} not supported'.format(heur))
+    comb = _RunningCombine(heur)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    for hms_t, ds_t, us_t in zip(hms_ts, ds_ts, us_ts):
+        t = hms_t if torch.is_tensor(hms_t) else torch.from_numpy(np.ascontiguousarray(hms_t, dtype=np.float32))
+        comb.add(t.to(dev, dtype=torch.float32), include=_size_dep_include(boxes, ds_t, us_t, p["kps_aug"]["area_th"]))
+    return comb.result()

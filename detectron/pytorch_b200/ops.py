@@ -943,6 +943,71 @@ def image_blob_raw(images, scales, flipped, pixel_means, stride, out=None):
 
 
 # ------------------------------------------------------------------------------------------------
+# Test-time augmentation of the mask / keypoint heads (lib/core/test.py:365-729), aspect_ratio_rel (lib/utils/image.py:27-32)
+# ------------------------------------------------------------------------------------------------
+TTA_HEURISTICS = {"SOFT_AVG": 0, "HM_AVG": 0, "SOFT_MAX": 1, "HM_MAX": 1, "LOGIT_AVG": 2}
+TTA_SKIP, TTA_START, TTA_FOLD = 0, 1, 2
+
+
+def tta_combine_raw(src, acc, heur, op=TTA_FOLD, hflip=False, channel_perm=None, row_op=None):
+    """Fold one transform's head output src (R, C, M, M) float32 CUDA into acc (same shape, written in place) the way numpy's
+    mean / amax over the stacked transforms does (see b200_tta_combine): heur 0 / 1 / 2 = AVG / MAX / LOGIT_AVG.  src is read
+    mirrored along its last axis when hflip, through channel_perm (C,) int32 CUDA (output channel c reads channel_perm[c]) when
+    given.  row_op (R,) uint8 CUDA, per row TTA_SKIP / TTA_START / TTA_FOLD, overrides op (TTA_START or TTA_FOLD for every row)."""
+    _need_cuda_f32(src, "src"); _need_cuda_f32(acc, "acc")
+    if src.dim() != 4 or src.size(2) != src.size(3) or tuple(acc.shape) != tuple(src.shape) or not acc.is_contiguous():
+        raise ValueError("tta_combine_raw: src %s and acc %s must be (R, C, M, M), acc contiguous" % (tuple(src.shape), tuple(acc.shape)))
+    R, C, M = int(src.size(0)), int(src.size(1)), int(src.size(2))
+    src = src.contiguous()
+    if channel_perm is not None:
+        perm_host = channel_perm.cpu().numpy() if torch.is_tensor(channel_perm) else np.asarray(channel_perm)
+        if perm_host.shape != (C,) or (C and (perm_host.min() < 0 or perm_host.max() >= C)):
+            raise ValueError("tta_combine_raw: channel_perm must be (%d,) indices in [0, %d)" % (C, C))
+        channel_perm = channel_perm.to(src.device, dtype=torch.int32).contiguous() if torch.is_tensor(channel_perm) else \
+            torch.from_numpy(np.ascontiguousarray(perm_host, dtype=np.int32)).to(src.device)
+    if row_op is not None:
+        if tuple(row_op.shape) != (R,) or row_op.dtype != torch.uint8 or not row_op.is_cuda:
+            raise ValueError("tta_combine_raw: row_op must be a (%d,) uint8 CUDA tensor" % R)
+        row_op = row_op.contiguous()
+    _launch("b200_tta_combine", src.device, src.data_ptr(), acc.data_ptr(), R, C, M, _ptr(channel_perm), _ptr(row_op), int(op),
+            int(bool(hflip)), int(heur))
+    return acc
+
+
+def tta_finish_raw(acc, heur, count=None, row_count=None):
+    """Finish a combine in place: AVG divides each row by its transform count (row_count (R,) int32 CUDA, or `count` for every row),
+    LOGIT_AVG also applies the sigmoid; MAX is already finished.  Returns acc."""
+    _need_cuda_f32(acc, "acc")
+    if row_count is not None:
+        row_count = row_count.to(acc.device, dtype=torch.int32).contiguous()
+    _launch("b200_tta_finish", acc.device, acc.data_ptr(), int(acc.size(0)), int(acc.size(1)), int(acc.size(2)), _ptr(row_count),
+            int(count or 0), int(heur))
+    return acc
+
+
+def resize_width_u8(im, out_width):
+    """cv2.resize(im, (out_width, h)) of a uint8 (h, w, 3) image (host array or CUDA tensor), INTER_LINEAR's 8-bit fixed-point
+    arithmetic with IPP off, on the device.  Returns a contiguous uint8 CUDA tensor (h, out_width, 3)."""
+    if torch.is_tensor(im) and im.is_cuda:
+        t = im
+        if t.dim() == 3 and (t.stride(2) != 1 or t.stride(1) != 3):
+            t = t.contiguous()
+    else:
+        t = torch.from_numpy(np.ascontiguousarray(im.numpy() if torch.is_tensor(im) else im))
+        if t.dtype == torch.uint8:
+            t = t.to(torch.device("cuda", torch.cuda.current_device()))
+    if t.dtype != torch.uint8 or t.dim() != 3 or t.size(2) != 3 or t.size(0) < 1 or t.size(1) < 1:
+        raise ValueError("resize_width_u8: im must be a uint8 (H, W, 3) image, got %s %s" % (t.dtype, tuple(t.shape)))
+    out_width = int(out_width)
+    if out_width < 1:
+        raise ValueError("resize_width_u8: output width %d (cv2.resize raises)" % out_width)
+    H, W = int(t.size(0)), int(t.size(1))
+    out = torch.empty((H, out_width, 3), dtype=torch.uint8, device=t.device)
+    _launch("b200_resize_width_u8", t.device, t.data_ptr(), int(t.stride(0)), H, W, out_width, out.data_ptr())
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
 # COCO evaluation stages (pycocotools COCOeval.evaluate / accumulate; datasets/coco_eval.py drives them)
 # ------------------------------------------------------------------------------------------------
 def coco_rank_raw(pair_det_begin, pair_entry_begin, det_score, num_entries):

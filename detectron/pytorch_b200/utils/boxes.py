@@ -28,3 +28,19 @@ def nms(dets, thresh):
     order = np.argsort(-dets[:, 4], kind="stable")                  # the batched NMS expects score-sorted rows
     keep, num = ops.nms_batched_raw(torch.from_numpy(dets[order]).cuda(), [dets.shape[0]], float(thresh), cython=True)
     return np.sort(order[keep[:int(num[0])].cpu().numpy()]).astype(np.int64)
+
+
+def flip_boxes(boxes, im_width):
+    """lib/utils/boxes.py:252-257: boxes (R, 4k) mirrored in an image of width im_width (x -> im_width - x - 1), host numpy."""
+    boxes_flipped = boxes.copy()
+    boxes_flipped[:, 0::4] = im_width - boxes[:, 2::4] - 1
+    boxes_flipped[:, 2::4] = im_width - boxes[:, 0::4] - 1
+    return boxes_flipped
+
+
+def aspect_ratio(boxes, aspect_ratio):
+    """lib/utils/boxes.py:260-265: the x coordinates of boxes (R, 4k) scaled by aspect_ratio, host numpy."""
+    boxes_ar = boxes.copy()
+    boxes_ar[:, 0::4] = aspect_ratio * boxes[:, 0::4]
+    boxes_ar[:, 2::4] = aspect_ratio * boxes[:, 2::4]
+    return boxes_ar

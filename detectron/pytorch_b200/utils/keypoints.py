@@ -54,3 +54,36 @@ def keypoints_to_heatmap_labels(keypoints, rois, heatmap_size=None, cfg=None):
         heatmap_size = cfg.KRCNN.HEATMAP_SIZE
     dev = _device_of(keypoints, rois)
     return ops.keypoints_to_heatmap_labels_raw(keypoints, _f32(rois, dev), heatmap_size)
+
+
+# The 17 COCO person keypoints in the dataset's order and their left / right pairs (lib/utils/keypoints.py:30-63).
+KEYPOINTS = ["nose", "left_eye", "right_eye", "left_ear", "right_ear", "left_shoulder", "right_shoulder", "left_elbow",
+             "right_elbow", "left_wrist", "right_wrist", "left_hip", "right_hip", "left_knee", "right_knee", "left_ankle", "right_ankle"]
+KEYPOINT_FLIP_MAP = {"left_" + p: "right_" + p for p in ("eye", "ear", "shoulder", "elbow", "wrist", "hip", "knee", "ankle")}
+
+
+def get_keypoints():
+    """(keypoint names, left -> right flip map) like lib/utils/keypoints.py:30-63."""
+    return list(KEYPOINTS), dict(KEYPOINT_FLIP_MAP)
+
+
+def flip_permutation(num_keypoints=None):
+    """(J,) int32: channel c of a horizontally flipped heatmap stack comes from channel perm[c] (each left / right pair of
+    get_keypoints() swapped, the others in place), the channel half of flip_heatmaps.  J defaults to the 17 COCO keypoints."""
+    keypoints, flip_map = get_keypoints()
+    perm = np.arange(len(keypoints) if num_keypoints is None else int(num_keypoints), dtype=np.int32)
+    for lkp, rkp in flip_map.items():
+        lid, rid = keypoints.index(lkp), keypoints.index(rkp)
+        perm[rid], perm[lid] = lid, rid
+    return perm
+
+
+def flip_heatmaps(heatmaps):
+    """lib/utils/keypoints.py:90-100 on the device: heatmaps (R, J, M, M) (numpy or float32 CUDA) with the left / right
+    keypoint channels swapped and mirrored along the last axis, in one launch (ops.tta_combine_raw copying through the
+    permutation).  Returns a float32 CUDA tensor."""
+    dev = _device_of(heatmaps)
+    src = _f32(heatmaps, dev).contiguous()
+    out = torch.empty_like(src)
+    return ops.tta_combine_raw(src, out, ops.TTA_HEURISTICS["HM_MAX"], op=ops.TTA_START, hflip=True,
+                               channel_perm=flip_permutation(src.size(1)))

@@ -488,6 +488,30 @@ typedef struct b200_image_blob_desc {
 B200_API int b200_image_blob(const unsigned char* src_dev, const b200_image_blob_desc* descs_dev, int num_images, const float* mean_table_dev,
                              int blob_h, int blob_w, float* out_dev, b200_stream_t stream);
 
+/* ---- test-time augmentation of the mask / keypoint heads (lib/core/test.py:365-729) and aspect_ratio_rel
+ *      (lib/utils/image.py:27-32) -----------------------------------------------------------------------------------------------
+ * b200_tta_combine folds one transform's head output src_dev (R, C, M, M) float32 into acc_dev (R, C, M, M), as numpy's
+ *   np.mean / np.amax over the stacked transforms do, one transform at a time in transform order:
+ *   heur 0 (SOFT_AVG / HM_AVG) sums (the first transform of a row: 0 + a), heur 1 (SOFT_MAX / HM_MAX) keeps np.maximum (the first
+ *   transform of a row: a copy; NaN propagates), heur 2 (LOGIT_AVG) sums -1.0 * log((1 - y) / np.maximum(y, 1e-20)).
+ *   The source element (r, c, y, x) read is (r, channel_perm_dev[c], y, hflip ? M - 1 - x : x); channel_perm_dev (C,) int32 may be
+ *   null (identity) and must hold indices in [0, C).  row_op_dev (R,) uint8 may be null, then every row takes `op`; per row:
+ *   0 leave acc untouched, 1 start the row with this transform, 2 fold this transform into it.  op: 1 or 2 (ignored with row_op_dev).
+ *   src_dev and acc_dev must not overlap.  One launch (none when R = 0).
+ * b200_tta_finish turns acc_dev into the combined result in place: heur 0 divides by the row's transform count, heur 2 divides
+ *   and applies 1 / (1 + exp(-m)), heur 1 launches nothing.  The count is row_count_dev[r] (R,) int32 (>= 1), or `count` (>= 1)
+ *   for every row when row_count_dev is null.
+ * b200_resize_width_u8 writes dst_dev (height, out_width, 3) uint8, contiguous: cv2.resize(src, (out_width, height)) of the
+ *   (height, width, 3) uint8 image at src_dev (row pitch src_pitch bytes) with INTER_LINEAR's 8-bit fixed-point arithmetic,
+ *   IPP off.  An out_width equal to width copies.  One launch.
+ * Bad sizes, modes or null pointers: B200_ROI_EINVAL before any launch (device tables are not read by the host). */
+B200_API int b200_tta_combine(const float* src_dev, float* acc_dev, int num_rows, int num_channels, int resolution, const int* channel_perm_dev,
+                              const unsigned char* row_op_dev, int op, int hflip, int heur, b200_stream_t stream);
+B200_API int b200_tta_finish(float* acc_dev, int num_rows, int num_channels, int resolution, const int* row_count_dev, int count, int heur,
+                             b200_stream_t stream);
+B200_API int b200_resize_width_u8(const unsigned char* src_dev, long long src_pitch, int height, int width, int out_width,
+                                  unsigned char* dst_dev, b200_stream_t stream);
+
 /* ---- COCO evaluation (lib/datasets/json_dataset_evaluator.py:38-233, 320-430 -> pycocotools COCOeval) --------------------
  * The device stages of COCOeval.evaluate() and accumulate() for one iouType.  Work is grouped per (image, category) pair; pairs
  * are ordered image-major.  Pair p owns detections pair_det_begin[p] .. [p + 1] - 1 (results order), ground truth
