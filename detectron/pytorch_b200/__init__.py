@@ -14,7 +14,7 @@ __version__ = "0.1.0"
 
 
 def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=False, keypoints=False, voc=False, losses=False,
-                              test_aug=False):
+                              test_aug=False, bbox=False):
     """Register this package's op modules in sys.modules under the reference's import paths.
 
     After this, `from modeling.roi_xfrom.roi_align.functions.roi_align import RoIAlignFunction`
@@ -42,6 +42,12 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
     generic_rpn_losses calls), `modeling.FPN.fpn_rpn_losses`, `modeling.mask_rcnn_heads.mask_rcnn_losses` and
     `modeling.keypoint_rcnn_heads.keypoint_losses` (`modeling/` here), each reading its reference module's `cfg` at call time;
     those reference modules must be importable.
+    `test_aug=True` re-points the reference's `core.test` im_detect_mask(_aug) and im_detect_keypoints(_aug) (and, with them,
+    segm_results and keypoint_results) at the device test-time augmentation (`core/test.py` here).
+    `bbox=True` re-points the reference's `core.test` im_detect_bbox, im_detect_bbox_aug, im_detect_bbox_hflip,
+    im_detect_bbox_scale, im_detect_bbox_aspect_ratio and box_results_with_nms_and_limit (whose inputs are then CUDA tensors)
+    at the device box decode and combine (`core/test.py` here).  Each reads the reference's `cfg` at call time; with
+    `bbox=True, test_aug=True` the reference's im_detect_all runs unmodified with no head output leaving the device.
     """
     import importlib
     import sys
@@ -88,6 +94,13 @@ def install_reference_aliases(overwrite=True, proposals=False, nms=False, segms=
         ours_test = importlib.import_module(__name__ + ".core.test")
         for name in ("im_detect_mask", "im_detect_mask_aug", "im_detect_keypoints", "im_detect_keypoints_aug"):
             setattr(ref_test, name, (lambda f: lambda *a: f(*a, cfg=ref_test.cfg))(getattr(ours_test, name)))
+            installed.append("core.test." + name)
+    if bbox:
+        ref_test = importlib.import_module("core.test")              # the reference's module
+        ours_test = importlib.import_module(__name__ + ".core.test")
+        for name in ("im_detect_bbox", "im_detect_bbox_aug", "im_detect_bbox_hflip", "im_detect_bbox_scale",
+                     "im_detect_bbox_aspect_ratio", "box_results_with_nms_and_limit"):
+            setattr(ref_test, name, (lambda f: lambda *a, **k: f(*a, cfg=ref_test.cfg, **k))(getattr(ours_test, name)))
             installed.append("core.test." + name)
     if segms:
         ref_test = importlib.import_module("core.test")              # the reference's module

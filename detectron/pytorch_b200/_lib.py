@@ -155,6 +155,10 @@ _SIGNATURES = {
     "b200_tta_finish": (ctypes.c_int, [_c_float_p] + [ctypes.c_int] * 3 + [ctypes.c_void_p] + [ctypes.c_int] * 2 + [_stream_t]),
     # (src, src_pitch, height, width, out_width, dst, stream)
     "b200_resize_width_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_longlong] + [ctypes.c_int] * 3 + [ctypes.c_void_p, _stream_t]),
+    # (boxes, box_stride, box_col, im_scale, deltas, delta_stride, agnostic, R, K, bbox_reg, weights, xform_clip, im_h, im_w,
+    #  flip_width, ar_inv, pred_boxes, stream)
+    "b200_bbox_decode": (ctypes.c_int, [_c_float_p, ctypes.c_int, ctypes.c_int, ctypes.c_double, _c_float_p] + [ctypes.c_int] * 5 +
+                         [ctypes.c_void_p, ctypes.c_double] + [ctypes.c_int] * 3 + [ctypes.c_double, _c_float_p, _stream_t]),
     # (P, pair_det_begin, pair_entry_begin, det_score, entry_det, entry_rank, entry_score, stream)
     "b200_coco_rank": (ctypes.c_int, [ctypes.c_int] + [ctypes.c_void_p] * 6 + [_stream_t]),
     # (P, pair_gt_begin, pair_entry_begin, pair_iou_begin, entry_det, det_box, gt_box, gt_flags, ious, stream)

@@ -36,6 +36,10 @@ is built on the device from the uint8 image (utils/blob.py).
 `im_detect_mask_aug` / `im_detect_keypoints_aug` (lib/core/test.py:365-729) run the heads over the test-time transforms in the
 reference's order, build every transform's blob on the device and fold each head output into one running CUDA accumulator
 (ops.tta_combine_raw); the combined masks / heatmaps are CUDA tensors for segm_results / keypoint_results.
+
+`im_detect_bbox` / `im_detect_bbox_aug` (lib/core/test.py:127-362) decode the box head on the device, one launch per transform with
+the transform's inverse in the same store (ops.bbox_decode_raw), and combine the transforms there; scores and boxes are CUDA tensors
+for box_results_with_nms_and_limit.
 """
 import numpy as np
 import torch
@@ -230,17 +234,16 @@ def keypoint_results(cls_boxes, pred_heatmaps, ref_boxes, cfg=None, **kw):
     return cls_keyps
 
 
-def get_blobs(im, rois, target_scale, target_max_size, cfg=None, **kw):
+def get_blobs(im, rois, target_scale, target_max_size, cfg=None, _hflip=False, **kw):
     """_get_blobs with _get_rois_blob (lib/core/test.py:869-929): blobs['data'] is the device image blob (utils/blob.py),
     blobs['im_info'] the float32 (1, 3) numpy (Hp, Wp, im_scale); with rois (R, 4) in image coordinates, blobs['rois'] is
-    the float32 (R, 5) [0, x1, y1, x2, y2] projection, multiplied in float64 like _project_im_rois.  Returns (blobs, im_scale)."""
+    the float32 (R, 5) [0, x1, y1, x2, y2] projection, multiplied in float64 like _project_im_rois.  Returns (blobs, im_scale).
+    _hflip: the blobs of im[:, ::-1, :] (the rois are taken as given)."""
     from ..utils import blob as blob_utils
     blobs = {}
-    blobs["data"], im_scale, blobs["im_info"] = blob_utils.get_image_blob(im, target_scale, target_max_size, cfg, **kw)
+    blobs["data"], im_scale, blobs["im_info"] = blob_utils.get_image_blob(im, target_scale, target_max_size, cfg, _hflip=_hflip, **kw)
     if rois is not None:
-        r = np.asarray(rois).astype(np.float64, copy=False) * im_scale
-        levels = np.zeros((r.shape[0], 1), dtype=np.int64)
-        blobs["rois"] = np.hstack((levels, r)).astype(np.float32, copy=False)
+        blobs["rois"] = _get_rois_blob(rois, im_scale)
     return blobs, im_scale
 
 
@@ -259,22 +262,36 @@ def _aug_params(cfg, kw):
         return dict(heur=a.HEUR, h_flip=a.H_FLIP, scales=tuple(a.SCALES), max_size=a.MAX_SIZE, scale_h_flip=a.SCALE_H_FLIP,
                     scale_size_dep=a.SCALE_SIZE_DEP, area_th=a.AREA_TH, aspect_ratios=tuple(a.ASPECT_RATIOS),
                     aspect_ratio_h_flip=a.ASPECT_RATIO_H_FLIP)
+    def bbox_aug(a):
+        return dict(score_heur=a.SCORE_HEUR, coord_heur=a.COORD_HEUR, h_flip=a.H_FLIP, scales=tuple(a.SCALES), max_size=a.MAX_SIZE,
+                    scale_h_flip=a.SCALE_H_FLIP, scale_size_dep=a.SCALE_SIZE_DEP, aspect_ratios=tuple(a.ASPECT_RATIOS),
+                    aspect_ratio_h_flip=a.ASPECT_RATIO_H_FLIP)
     if cfg is not None:
         p = dict(num_classes=cfg.MODEL.NUM_CLASSES, resolution=cfg.MRCNN.RESOLUTION, cls_specific_mask=cfg.MRCNN.CLS_SPECIFIC_MASK,
                  num_keypoints=cfg.KRCNN.NUM_KEYPOINTS, heatmap_size=cfg.KRCNN.HEATMAP_SIZE, test_scale=cfg.TEST.SCALE,
                  test_max_size=cfg.TEST.MAX_SIZE, multilevel_rois=cfg.FPN.MULTILEVEL_ROIS, roi_min_level=cfg.FPN.ROI_MIN_LEVEL,
                  roi_max_level=cfg.FPN.ROI_MAX_LEVEL, roi_canonical_scale=cfg.FPN.ROI_CANONICAL_SCALE,
                  roi_canonical_level=cfg.FPN.ROI_CANONICAL_LEVEL, mask_aug=aug(cfg.TEST.MASK_AUG), kps_aug=aug(cfg.TEST.KPS_AUG),
+                 faster_rcnn=bool(cfg.MODEL.FASTER_RCNN), dedup_boxes=cfg.DEDUP_BOXES, bbox_reg=bool(cfg.TEST.BBOX_REG),
+                 cls_agnostic_bbox_reg=bool(cfg.MODEL.CLS_AGNOSTIC_BBOX_REG), bbox_reg_weights=tuple(cfg.MODEL.BBOX_REG_WEIGHTS),
+                 bbox_xform_clip=float(cfg.BBOX_XFORM_CLIP),
+                 bbox_normalize_targets_precomputed=bool(cfg.TRAIN.BBOX_NORMALIZE_TARGETS_PRECOMPUTED),
+                 bbox_aug=bbox_aug(cfg.TEST.BBOX_AUG),
                  blob=dict(pixel_means=cfg.PIXEL_MEANS, fpn_on=bool(cfg.FPN.FPN_ON), coarsest_stride=int(cfg.FPN.COARSEST_STRIDE)))
     else:
         from ..utils.blob import blob_params
         defaults = dict(heur=None, h_flip=False, scales=(), max_size=4000, scale_h_flip=False, scale_size_dep=False, area_th=180 ** 2,
-                        aspect_ratios=(), aspect_ratio_h_flip=False)             # lib/core/config.py:289-354
+                        aspect_ratios=(), aspect_ratio_h_flip=False)             # lib/core/config.py:249-354
         p = dict(num_classes=None, resolution=14, cls_specific_mask=True, num_keypoints=17, heatmap_size=56, test_scale=600,
                  test_max_size=1000, multilevel_rois=False, roi_min_level=2, roi_max_level=5, roi_canonical_scale=224,
                  roi_canonical_level=4, mask_aug=dict(defaults, heur="SOFT_AVG"), kps_aug=dict(defaults, heur="HM_AVG"),
+                 faster_rcnn=False, dedup_boxes=1. / 16., bbox_reg=True, cls_agnostic_bbox_reg=False,
+                 bbox_reg_weights=(10., 10., 5., 5.), bbox_xform_clip=float(np.log(1000. / 16.)),
+                 bbox_normalize_targets_precomputed=False,                       # lib/core/config.py:96, 196, 408-430, 931-936
+                 bbox_aug=dict(defaults, score_heur="UNION", coord_heur="UNION"),
                  blob=blob_params())
-    for key in ("mask_aug", "kps_aug", "blob"):
+        del p["bbox_aug"]["heur"], p["bbox_aug"]["area_th"]
+    for key in ("mask_aug", "kps_aug", "bbox_aug", "blob"):
         p[key] = dict(p[key], **kw.pop(key, {}))
     for key in ("pixel_means", "fpn_on", "coarsest_stride"):
         if key in kw:
@@ -554,3 +571,168 @@ def combine_heatmaps_size_dep(hms_ts, ds_ts, us_ts, boxes, heur, cfg=None, **kw)
         t = hms_t if torch.is_tensor(hms_t) else torch.from_numpy(np.ascontiguousarray(hms_t, dtype=np.float32))
         comb.add(t.to(dev, dtype=torch.float32), include=_size_dep_include(boxes, ds_t, us_t, p["kps_aug"]["area_th"]))
     return comb.result()
+
+
+# ------------------------------------------------------------------------------------------------
+# The box head and its test-time augmentation (lib/core/test.py:127-362)
+# ------------------------------------------------------------------------------------------------
+_BBOX_HEURS = ("ID", "AVG", "UNION")
+
+
+def _head_rows(t):
+    """The reference's `.squeeze()` then `.reshape([-1, shape[-1]])` (one proposal gives a 1-D squeeze), on the device."""
+    t = t.detach() if torch.is_tensor(t) else torch.from_numpy(np.ascontiguousarray(t))
+    t = t.to(torch.device("cuda", torch.cuda.current_device()) if not t.is_cuda else t.device, dtype=torch.float32).squeeze()
+    return t.reshape(-1, t.shape[-1])
+
+
+def _detect_bbox(model, im, target_scale, target_max_size, boxes, hflip, ar_inv, p):
+    """im_detect_bbox on im (im[:, ::-1, :] when hflip, read mirrored by the blob kernel), with the transform's inverse
+    (flip_boxes with im's width when hflip, then x * float32(ar_inv)) applied in the decode's store.  boxes: the proposals the
+    model sees (already flipped / aspect-scaled), or None with FASTER_RCNN.  Returns (scores, pred_boxes, im_scale, blob_conv)."""
+    if p["bbox_reg"] and p["bbox_normalize_targets_precomputed"]:
+        # the reference's `box_deltas.view(-1, 4)` on a numpy array raises too (lib/core/test.py:172-175)
+        raise NotImplementedError("TRAIN.BBOX_NORMALIZE_TARGETS_PRECOMPUTED is not supported at test time")
+    inputs, im_scale = get_blobs(im, boxes, target_scale, target_max_size, _hflip=hflip, **p["blob"])
+    dedup = p["dedup_boxes"] > 0 and not p["faster_rcnn"]
+    if dedup:
+        v = np.array([1, 1e3, 1e6, 1e9, 1e12])
+        hashes = np.round(inputs["rois"] * p["dedup_boxes"]).dot(v)
+        _, index, inv_index = np.unique(hashes, return_index=True, return_inverse=True)
+        inputs["rois"] = inputs["rois"][index, :]
+        boxes = boxes[index, :]
+    if p["multilevel_rois"] and not p["faster_rcnn"]:
+        _add_multilevel_rois_for_test(inputs, "rois", p)
+    inputs["data"] = [inputs["data"]]
+    inputs["im_info"] = [torch.from_numpy(inputs["im_info"])]
+    return_dict = model(**inputs)
+
+    scores = _head_rows(return_dict["cls_score"])
+    K = int(scores.shape[1])
+    if p["faster_rcnn"]:
+        rois, scale = return_dict["rois"], im_scale
+        rois = rois.detach() if torch.is_tensor(rois) else torch.from_numpy(np.ascontiguousarray(rois))
+    else:
+        rois, scale = torch.from_numpy(np.ascontiguousarray(boxes, dtype=np.float32)), None
+    rois = rois.to(scores.device, dtype=torch.float32)
+    deltas = _head_rows(return_dict["bbox_pred"]) if p["bbox_reg"] else None
+    pred_boxes = ops.bbox_decode_raw(rois, deltas, K, int(im.shape[0]), int(im.shape[1]), im_scale=scale, bbox_reg=p["bbox_reg"],
+                                     weights=p["bbox_reg_weights"], xform_clip=p["bbox_xform_clip"],
+                                     agnostic=p["cls_agnostic_bbox_reg"], flip_width=int(im.shape[1]) if hflip else None, ar_inv=ar_inv)
+    if dedup:
+        inv = torch.from_numpy(np.asarray(inv_index, dtype=np.int64).reshape(-1)).to(scores.device)
+        scores, pred_boxes = scores[inv], pred_boxes[inv]
+    return scores, pred_boxes, im_scale, return_dict["blob_conv"]
+
+
+def im_detect_bbox(model, im, target_scale, target_max_size, boxes=None, cfg=None, **kw):
+    """lib/core/test.py:127-189: the model on the device blob of im (with the proposals `boxes` (R, 4) unless FASTER_RCNN),
+    the deltas decoded and clipped on the device (ops.bbox_decode_raw).  Returns (scores float32 CUDA (R, K), pred_boxes float32
+    CUDA (R, 4K), im_scale, blob_conv); box_results_with_nms_and_limit takes both tensors as they are.  The host keeps only the
+    small arrays the reference builds there: im_info, the rois / FPN level blobs and the DEDUP_BOXES hashes.
+    TRAIN.BBOX_NORMALIZE_TARGETS_PRECOMPUTED raises NotImplementedError (the reference's own line fails on its numpy deltas)."""
+    return _detect_bbox(model, im, target_scale, target_max_size, boxes, False, 1.0, _aug_params(cfg, kw))
+
+
+def _bbox_hflip(model, im, target_scale, target_max_size, box_proposals, ar_inv, p):
+    from ..utils.boxes import flip_boxes
+    box_proposals_hf = None if p["faster_rcnn"] else flip_boxes(box_proposals, int(im.shape[1]))
+    scores_hf, boxes_inv, im_scale, _ = _detect_bbox(model, im, target_scale, target_max_size, box_proposals_hf, True, ar_inv, p)
+    return scores_hf, boxes_inv, im_scale
+
+
+def im_detect_bbox_hflip(model, im, target_scale, target_max_size, box_proposals=None, cfg=None, **kw):
+    """lib/core/test.py:289-310: detections on the flipped image (the blob kernel reads im mirrored), flipped back in the decode.
+    Returns (scores, boxes, im_scale), CUDA like im_detect_bbox."""
+    return _bbox_hflip(model, im, target_scale, target_max_size, box_proposals, 1.0, _aug_params(cfg, kw))
+
+
+def _bbox_scale(model, im, target_scale, target_max_size, box_proposals, hflip, p):
+    if hflip:
+        return _bbox_hflip(model, im, target_scale, target_max_size, box_proposals, 1.0, p)[:2]
+    return _detect_bbox(model, im, target_scale, target_max_size, box_proposals, False, 1.0, p)[:2]
+
+
+def im_detect_bbox_scale(model, im, target_scale, target_max_size, box_proposals=None, hflip=False, cfg=None, **kw):
+    """lib/core/test.py:313-326.  Returns (scores, boxes), CUDA."""
+    return _bbox_scale(model, im, target_scale, target_max_size, box_proposals, hflip, _aug_params(cfg, kw))
+
+
+def _bbox_aspect_ratio(model, im, aspect_ratio, box_proposals, hflip, p):
+    from ..utils.boxes import aspect_ratio as boxes_aspect_ratio
+    from ..utils.image import aspect_ratio_rel
+    im_ar = aspect_ratio_rel(im, aspect_ratio)
+    box_proposals_ar = None if p["faster_rcnn"] else boxes_aspect_ratio(box_proposals, aspect_ratio)
+    ar_inv = 1.0 / aspect_ratio
+    if hflip:
+        return _bbox_hflip(model, im_ar, p["test_scale"], p["test_max_size"], box_proposals_ar, ar_inv, p)[:2]
+    return _detect_bbox(model, im_ar, p["test_scale"], p["test_max_size"], box_proposals_ar, False, ar_inv, p)[:2]
+
+
+def im_detect_bbox_aspect_ratio(model, im, aspect_ratio, box_proposals=None, hflip=False, cfg=None, **kw):
+    """lib/core/test.py:329-362: detections on the image resized by utils/image.py aspect_ratio_rel on the device, the boxes
+    mapped back (`x * float32(1 / aspect_ratio)`) in the decode.  Returns (scores, boxes), CUDA."""
+    return _bbox_aspect_ratio(model, im, aspect_ratio, box_proposals, hflip, _aug_params(cfg, kw))
+
+
+class _BoxCombine:
+    """One of SCORE_HEUR / COORD_HEUR over the transforms, as they arrive: UNION concatenates on the device, AVG folds each
+    (R, C) output into _RunningCombine as an (R, C, 1, 1) view (np.mean over the stacked float32 outputs, bit for bit), ID keeps
+    the identity transform's output."""
+
+    def __init__(self, heur):
+        self.heur, self.parts = heur, []
+        self.mean = _RunningCombine("SOFT_AVG") if heur == "AVG" else None
+
+    def add(self, out, identity):
+        if self.heur == "UNION" or (self.heur == "ID" and identity):
+            self.parts.append(out)
+        elif self.heur == "AVG":
+            self.mean.add(out.reshape(out.shape[0], out.shape[1], 1, 1))
+
+    def result(self):
+        if self.heur == "AVG":
+            out = self.mean.result()
+            return out.reshape(out.shape[0], out.shape[1])
+        return self.parts[0] if len(self.parts) == 1 else torch.cat(self.parts, dim=0)
+
+
+def im_detect_bbox_aug(model, im, box_proposals=None, cfg=None, **kw):
+    """lib/core/test.py:192-286: scores and boxes over TEST.BBOX_AUG's transforms (H_FLIP, SCALES with SCALE_H_FLIP,
+    ASPECT_RATIOS with ASPECT_RATIO_H_FLIP, then the identity last), the model called in the reference's order, every head
+    output decoded and combined on the device (SCORE_HEUR / COORD_HEUR: UNION concatenates, AVG averages as np.mean does, ID
+    takes the identity's).  Returns (scores float32 CUDA, boxes float32 CUDA, im_scale, blob_conv) of the identity transform.
+    An unknown heuristic raises NotImplementedError before the first model call (the reference raises after the last)."""
+    p = _aug_params(cfg, kw)
+    a = p["bbox_aug"]
+    assert not a["scale_size_dep"], 'Size dependent scaling not implemented'
+    assert not a["score_heur"] == 'UNION' or a["coord_heur"] == 'UNION', \
+        'Coord heuristic must be union whenever score heuristic is union'
+    assert not a["coord_heur"] == 'UNION' or a["score_heur"] == 'UNION', \
+        'Score heuristic must be union whenever coord heuristic is union'
+    assert not p["faster_rcnn"] or a["score_heur"] == 'UNION', \
+        'Union heuristic must be used to combine Faster RCNN predictions'
+    if a["score_heur"] not in _BBOX_HEURS:
+        raise NotImplementedError('Score heur {} not supported'.format(a["score_heur"]))
+    if a["coord_heur"] not in _BBOX_HEURS:
+        raise NotImplementedError('Coord heur {} not supported'.format(a["coord_heur"]))
+    scores_c, boxes_c = _BoxCombine(a["score_heur"]), _BoxCombine(a["coord_heur"])
+
+    def add_preds_t(scores_t, boxes_t, identity=False):
+        scores_c.add(scores_t, identity)
+        boxes_c.add(boxes_t, identity)
+
+    if a["h_flip"]:
+        add_preds_t(*_bbox_hflip(model, im, p["test_scale"], p["test_max_size"], box_proposals, 1.0, p)[:2])
+    for scale in a["scales"]:
+        add_preds_t(*_bbox_scale(model, im, scale, a["max_size"], box_proposals, False, p))
+        if a["scale_h_flip"]:
+            add_preds_t(*_bbox_scale(model, im, scale, a["max_size"], box_proposals, True, p))
+    for aspect_ratio in a["aspect_ratios"]:
+        add_preds_t(*_bbox_aspect_ratio(model, im, aspect_ratio, box_proposals, False, p))
+        if a["aspect_ratio_h_flip"]:
+            add_preds_t(*_bbox_aspect_ratio(model, im, aspect_ratio, box_proposals, True, p))
+    # the identity transform last, so that its blob_conv / im_scale are returned (postcondition of im_detect_bbox)
+    scores_i, boxes_i, im_scale_i, blob_conv_i = _detect_bbox(model, im, p["test_scale"], p["test_max_size"], box_proposals, False, 1.0, p)
+    add_preds_t(scores_i, boxes_i, identity=True)
+    return scores_c.result(), boxes_c.result(), im_scale_i, blob_conv_i

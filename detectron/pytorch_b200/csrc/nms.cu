@@ -463,11 +463,25 @@ static int nms_batched(const float* boxes, const int* counts, int num_problems, 
         const size_t sm_r = sizeof(u64) * ((size_t)r * cb * kNmsTile + 4 * (size_t)cb) + 16;
         if (sm_r <= 224 * 1024) { reach = r; smem_res = sm_r; break; }
     }
-    if (reach == 0) return B200_ROI_EINVAL;                      // a problem too large for the pipelined scan: the caller loops over b200_nms
     u64* ws = (u64*)workspace;
     if (nb.tile_off[num_problems] > 0)
         (cython ? nms_mask_batched_kernel<true> : nms_mask_batched_kernel<false>)<<<(unsigned)nb.tile_off[num_problems], kNmsTile, 0, stream>>>(
             boxes, nb, dim, thresh, lo, hi, ws);
+    if (reach == 0) {
+        // a problem too large for the pipelined scan (> ~13.8k boxes): b200_nms's unpipelined scan, one launch per problem
+        const size_t smem = sizeof(u64) * (size_t)cb;
+        if (smem > 48 * 1024) {
+            cudaError_t e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) return (int)e;
+        }
+        for (int p = 0; p < num_problems; ++p) {
+            const int n = nb.n[p];
+            if (n == 0) nms_empty_kernel<<<1, 1, 0, stream>>>(num_out + p);
+            else nms_scan_kernel<<<1, kScanThreads, sizeof(u64) * (size_t)((n + kNmsTile - 1) / kNmsTile), stream>>>(
+                ws + nb.mask_off[p], n, (n + kNmsTile - 1) / kNmsTile, keep_out + nb.box_off[p], num_out + p);
+        }
+        return finish_launch(1 + num_problems);
+    }
     void (*kern)(const u64*, const NmsBatch, int*, int*) =
         (reach == 4) ? nms_scan_resolver_batched_kernel<4> : (reach == 3) ? nms_scan_resolver_batched_kernel<3> : nms_scan_resolver_batched_kernel<2>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_res);

@@ -7,13 +7,13 @@
 // drops it by the `valid` flag after NMS -- the candidate list keeps its length and no stream synchronisation or
 // compaction is needed between decode and NMS.
 //
-// Arithmetic follows the reference's numpy lines as they evaluate under numpy >= 2 (oracle/proposals.py, pinned by
-// tests/golden/proposals.npz): float32 for widths, centres and `dx * w + ctr`; float64 for min(dw, BBOX_XFORM_CLIP),
-// exp, `exp * w` and `ctr -/+ 0.5 * pred_w (- 1)`, rounded to float32 once.
+// The decode and clip are bbox_transform.cuh's, with weights (1, 1, 1, 1) (oracle/proposals.py, pinned by
+// tests/golden/proposals.npz).
 //
 // Semantics: lib/modeling/generate_proposals.py:66-89 (anchor enumeration), :108-150 (order, decode, clip, filter),
 // :171-182 (_filter_boxes); lib/utils/boxes.py:138-154 (clip_tiled_boxes), :157-196 (bbox_transform); lib/core/config.py:936.
 #include "common.cuh"
+#include "bbox_transform.cuh"
 
 namespace b200 {
 
@@ -39,23 +39,12 @@ proposal_decode_kernel(const float* __restrict__ deltas,        // (4A, H, W) of
     const float dx = deltas[(size_t)(4 * a + 0) * plane + cell], dy = deltas[(size_t)(4 * a + 1) * plane + cell];
     const float dw = deltas[(size_t)(4 * a + 2) * plane + cell], dh = deltas[(size_t)(4 * a + 3) * plane + cell];
 
-    const float widths = __fadd_rn(__fsub_rn(x2, x1), 1.f), heights = __fadd_rn(__fsub_rn(y2, y1), 1.f);
-    const float ctr_x = __fadd_rn(x1, __fmul_rn(.5f, widths)), ctr_y = __fadd_rn(y1, __fmul_rn(.5f, heights));
-    const float pcx = __fadd_rn(__fmul_rn(dx, widths), ctr_x), pcy = __fadd_rn(__fmul_rn(dy, heights), ctr_y);
-    const double kClip = 4.135166556742356;                      // log(1000 / 16)
-    // np.minimum(d, clip): a NaN delta stays NaN (fmin would return the clip)
-    const double dwc = (double)dw > kClip ? kClip : (double)dw, dhc = (double)dh > kClip ? kClip : (double)dh;
-    const double pw = __dmul_rn(exp(dwc), (double)widths);
-    const double ph = __dmul_rn(exp(dhc), (double)heights);
-    const double hw = __dmul_rn(.5, pw), hh = __dmul_rn(.5, ph);
-    float bx1 = (float)__dsub_rn((double)pcx, hw), by1 = (float)__dsub_rn((double)pcy, hh);
-    float bx2 = (float)__dsub_rn(__dadd_rn((double)pcx, hw), 1.0), by2 = (float)__dsub_rn(__dadd_rn((double)pcy, hh), 1.0);
+    const float4 p = bbox_transform(x1, y1, x2, y2, dx, dy, dw, dh, 1.f, 1.f, 1.f, 1.f, 4.135166556742356);   // log(1000 / 16)
 
-    // NaN survives the reference's np.minimum / np.maximum clip and fails _filter_boxes; fminf / fmaxf would clip it, so test it first
-    const bool finite_box = !(bx1 != bx1 || by1 != by1 || bx2 != bx2 || by2 != by2);
+    // NaN survives the reference's np.minimum / np.maximum clip and fails _filter_boxes
+    const bool finite_box = !(p.x != p.x || p.y != p.y || p.z != p.z || p.w != p.w);
     const float wmax = __fsub_rn(im_w, 1.f), hmax = __fsub_rn(im_h, 1.f);
-    bx1 = fmaxf(fminf(bx1, wmax), 0.f); by1 = fmaxf(fminf(by1, hmax), 0.f);
-    bx2 = fmaxf(fminf(bx2, wmax), 0.f); by2 = fmaxf(fminf(by2, hmax), 0.f);
+    const float bx1 = clip_coord(p.x, wmax), by1 = clip_coord(p.y, hmax), bx2 = clip_coord(p.z, wmax), by2 = clip_coord(p.w, hmax);
 
     const float ws = __fadd_rn(__fsub_rn(bx2, bx1), 1.f), hs = __fadd_rn(__fsub_rn(by2, by1), 1.f);
     const float xc = __fadd_rn(bx1, __fmul_rn(ws, .5f)), yc = __fadd_rn(by1, __fmul_rn(hs, .5f));

@@ -985,6 +985,36 @@ def tta_finish_raw(acc, heur, count=None, row_count=None):
     return acc
 
 
+def bbox_decode_raw(boxes, deltas, num_classes, im_h, im_w, im_scale=None, bbox_reg=True, weights=(10.0, 10.0, 5.0, 5.0),
+                    xform_clip=float(np.log(1000.0 / 16.0)), agnostic=False, flip_width=None, ar_inv=1.0):
+    """pred_boxes (R, 4K) float32 CUDA of one test-time transform (b200_bbox_decode): the box head's bbox_transform +
+    clip_tiled_boxes to the transform's (im_h, im_w) image, then the transform's inverse (flip_boxes with flip_width, then x times
+    float32(ar_inv)).  boxes: the model's rois (R, 5) with im_scale (divided in double), or float32 proposals (R, 4) with
+    im_scale None.  deltas: bbox_pred (R, 4K), or with agnostic (R, >= 4) whose last 4 columns are used; ignored (may be None)
+    without bbox_reg, which tiles the boxes.  Both float32 CUDA."""
+    _need_cuda_f32(boxes, "boxes")
+    K = int(num_classes)
+    cols = 5 if im_scale is not None else 4
+    if boxes.dim() != 2 or boxes.size(1) != cols:
+        raise ValueError("boxes must be (R, %d) %s, got %s" % (cols, "rois" if cols == 5 else "proposals", tuple(boxes.shape)))
+    if K < 1 or (im_scale is not None and not float(im_scale) > 0):
+        raise ValueError("bbox_decode_raw: num_classes %d, im_scale %r" % (K, im_scale))
+    R = int(boxes.size(0))
+    boxes = boxes.contiguous()
+    if bbox_reg:
+        _need_cuda_f32(deltas, "deltas")
+        if deltas.dim() != 2 or deltas.size(0) != R or deltas.size(1) < 4 or (not agnostic and deltas.size(1) != 4 * K):
+            raise ValueError("deltas must be (%d, %s), got %s" % (R, ">= 4" if agnostic else 4 * K, tuple(deltas.shape)))
+        if len(weights) != 4:
+            raise ValueError("bbox_decode_raw: 4 weights expected, got %r" % (weights,))
+        deltas = deltas.contiguous()
+    out = torch.empty((R, 4 * K), dtype=torch.float32, device=boxes.device)
+    _launch("b200_bbox_decode", boxes.device, _ptr(boxes), cols, cols - 4, float(im_scale or 0.0),
+            _ptr(deltas) if bbox_reg else None, int(deltas.size(1)) if bbox_reg else 0, int(bool(agnostic)), R, K, int(bool(bbox_reg)),
+            _host_array(ctypes.c_float, weights), float(xform_clip), int(im_h), int(im_w), int(flip_width or 0), float(ar_inv), _ptr(out))
+    return out
+
+
 def resize_width_u8(im, out_width):
     """cv2.resize(im, (out_width, h)) of a uint8 (h, w, 3) image (host array or CUDA tensor), INTER_LINEAR's 8-bit fixed-point
     arithmetic with IPP off, on the device.  Returns a contiguous uint8 CUDA tensor (h, out_width, 3)."""

@@ -29,13 +29,14 @@ def blob_params(cfg=None, **kw):
     return p
 
 
-def get_image_blob(im, target_scale, target_max_size, cfg=None, **kw):
+def get_image_blob(im, target_scale, target_max_size, cfg=None, _hflip=False, **kw):
     """lib/utils/blob.py:37-60 on the device.  im: a decoded uint8 (H, W, 3) BGR image, a host array or a CUDA tensor.
-    Returns (blob float32 CUDA (1, 3, Hp, Wp), im_scale float, im_info float32 numpy (1, 3) = (Hp, Wp, im_scale))."""
+    Returns (blob float32 CUDA (1, 3, Hp, Wp), im_scale float, im_info float32 numpy (1, 3) = (Hp, Wp, im_scale)).
+    _hflip: the blob of im[:, ::-1, :], read mirrored by the blob kernel (the box head's flipped test-time transforms)."""
     p = blob_params(cfg, **kw)
     h, w = int(im.shape[0]), int(im.shape[1])
     im_scale = get_target_scale(min(h, w), max(h, w), target_scale, target_max_size)
-    blob, _ = ops.image_blob_raw([im], [im_scale], [False], p["pixel_means"], p["coarsest_stride"] if p["fpn_on"] else None)
+    blob, _ = ops.image_blob_raw([im], [im_scale], [_hflip], p["pixel_means"], p["coarsest_stride"] if p["fpn_on"] else None)
     im_info = np.hstack((blob.shape[2], blob.shape[3], im_scale))[np.newaxis, :]
     return blob, im_scale, im_info.astype(np.float32)
 

@@ -512,6 +512,20 @@ B200_API int b200_tta_finish(float* acc_dev, int num_rows, int num_channels, int
 B200_API int b200_resize_width_u8(const unsigned char* src_dev, long long src_pitch, int height, int width, int out_width,
                                   unsigned char* dst_dev, b200_stream_t stream);
 
+/* ---- the box head's decode of one test-time transform (lib/core/test.py:127-189, 289-362) ------------------------------------
+ * b200_bbox_decode writes pred_boxes_dev (num_rows, 4 * num_classes) float32, 16-byte aligned.  Row r's input box is
+ *   boxes_dev[r * box_stride + box_col + 0..3]: with im_scale > 0 the model's rois divided by im_scale in double (box_col 1 of
+ *   (R, 5) rois), with im_scale == 0 float32 image-space proposals taken as they are.
+ *   bbox_reg != 0: the box decoded by deltas_dev[r * delta_stride + 4j + 0..3] (agnostic: the row's last 4 columns, the same for
+ *   every class) with weights_host (wx, wy, ww, wh) and the log-space clip xform_clip, then clipped to [0, im_w - 1] x
+ *   [0, im_h - 1] (NaN propagates); bbox_reg == 0: the box itself, tiled.
+ *   Then x1, x2 are mirrored when flip_width > 0 (x' = (flip_width - x) - 1, x1 and x2 swapped) and multiplied by ar_inv
+ *   (1.0 for none): in float32 after a decode or for proposals, in double for undecoded rois, rounded to float32 at the store.
+ *   One launch (none when num_rows = 0).  Bad sizes, null pointers: B200_ROI_EINVAL before any launch. */
+B200_API int b200_bbox_decode(const float* boxes_dev, int box_stride, int box_col, double im_scale, const float* deltas_dev, int delta_stride,
+                              int agnostic, int num_rows, int num_classes, int bbox_reg, const float* weights_host, double xform_clip,
+                              int im_h, int im_w, int flip_width, double ar_inv, float* pred_boxes_dev, b200_stream_t stream);
+
 /* ---- COCO evaluation (lib/datasets/json_dataset_evaluator.py:38-233, 320-430 -> pycocotools COCOeval) --------------------
  * The device stages of COCOeval.evaluate() and accumulate() for one iouType.  Work is grouped per (image, category) pair; pairs
  * are ordered image-major.  Pair p owns detections pair_det_begin[p] .. [p + 1] - 1 (results order), ground truth
