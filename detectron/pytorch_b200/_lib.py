@@ -202,6 +202,12 @@ _SIGNATURES = {
     # (R, C, B, cls_score, bbox_pred, labels, label_is_int64, targets, inside, outside, grad_losses, cls_grad_out, bbox_grad_out, stream)
     "b200_fast_rcnn_loss_backward": (ctypes.c_int, [ctypes.c_int] * 3 + [ctypes.c_void_p] * 3 + [ctypes.c_int] + [ctypes.c_void_p] * 6 +
                                      [_stream_t]),
+    "b200_jpeg_decode_workspace_bytes": (ctypes.c_size_t, [ctypes.c_longlong] * 2),
+    # (data, descs, N, intervals, num_intervals, tables, subseq_bits, total_blocks, total_subseqs, max_blocks, max_pixels, workspace,
+    #  workspace_bytes, out, status, stream)
+    "b200_jpeg_decode": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                        ctypes.c_int] + [ctypes.c_longlong] * 4 + [ctypes.c_void_p, ctypes.c_size_t] +
+                         [ctypes.c_void_p] * 2 + [_stream_t]),
 }
 
 EXPORTED_SYMBOLS = tuple(sorted(_SIGNATURES))

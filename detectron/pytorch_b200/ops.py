@@ -1038,6 +1038,95 @@ def resize_width_u8(im, out_width):
 
 
 # ------------------------------------------------------------------------------------------------
+# JPEG decode (cv2.imread / cv2.imdecode with IMREAD_COLOR; utils/jpeg.py parses, utils/image.py imdecode / imread)
+# ------------------------------------------------------------------------------------------------
+JPEG_DECODED, JPEG_FORMAT_FALLBACK, JPEG_ENTROPY_ERROR = 0, 1, 2
+JPEG_SUBSEQ_BITS = 256          # subsequence length of the parallel Huffman decode (any value >= 1 gives the same pixels)
+_JPEG_DESC = np.dtype([("out_offset", "<i8"), ("first_block", "<i8"), ("height", "<i4"), ("width", "<i4"), ("ncomp", "<i4"),
+                       ("h", "<i4"), ("v", "<i4"), ("mcus_x", "<i4"), ("mcus_y", "<i4"), ("orientation", "<i4"), ("table", "<i4"),
+                       ("reserved", "<i4"), ("quant", "<u2", (3, 64))])
+_JPEG_INTERVAL = np.dtype([("data_offset", "<i8"), ("nbytes", "<i4"), ("image", "<i4"), ("first_mcu", "<i4"), ("num_mcus", "<i4"),
+                           ("first_subseq", "<i8")])
+assert _JPEG_DESC.itemsize == 440 and _JPEG_INTERVAL.itemsize == 32
+
+
+def _align16(n):
+    return (n + 15) & ~15
+
+
+def jpeg_decode_raw(parsed, out=None, subseq_bits=JPEG_SUBSEQ_BITS, device=None):
+    """Decode the device-decodable images among `parsed` (utils/jpeg.Parsed, in order) with one upload and three launches.
+
+    Returns (images, status): images[i] is a uint8 CUDA (H, W, 3) BGR view into one allocation -- None for a file that parse()
+    sent to the fallback -- and status a uint8 CUDA tensor (N,): JPEG_DECODED, JPEG_FORMAT_FALLBACK (not sent to the device) or
+    JPEG_ENTROPY_ERROR (its entropy data did not decode; its view is left unwritten).  Nothing here synchronises.
+    `out`: an optional contiguous uint8 CUDA tensor of at least the decoded images' total bytes to write into."""
+    N = len(parsed)
+    if N < 1:
+        raise ValueError("jpeg_decode_raw: no images")
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    dev_idx = [i for i, p in enumerate(parsed) if not p.fallback]
+    status = torch.full((N,), JPEG_FORMAT_FALLBACK, dtype=torch.uint8, device=dev)
+    images = [None] * N
+    if not dev_idx:
+        return images, status
+    n = len(dev_idx)
+    descs = np.zeros((n,), _JPEG_DESC)
+    ivs, tables, datas = [], [], []
+    out_bytes = blocks = subseqs = data_bytes = 0
+    max_blocks = max_pixels = 0
+    for d, i in enumerate(dev_idx):
+        p = parsed[i]
+        e = descs[d]
+        e["out_offset"], e["first_block"] = out_bytes, blocks
+        e["height"], e["width"], e["ncomp"], e["h"], e["v"] = p.height, p.width, p.ncomp, p.h, p.v
+        e["mcus_x"], e["mcus_y"], e["orientation"], e["table"] = p.mcus_x, p.mcus_y, p.orientation, len(tables)
+        e["quant"][:p.ncomp] = p.quant
+        tables.extend(t.packed() for t in p.dc + p.ac)
+        bpm = p.blocks_per_mcu
+        for first_mcu, num_mcus, buf in p.intervals:
+            if len(buf) >= 1 << 28:
+                raise ValueError("jpeg_decode_raw: a restart interval of %d bytes (at most 2^28 - 1)" % len(buf))
+            ivs.append((data_bytes, len(buf), d, first_mcu, num_mcus, subseqs))
+            datas.append((data_bytes, buf))
+            data_bytes += _align16(len(buf))
+            subseqs += max(1, -(-8 * len(buf) // subseq_bits))
+        out_bytes += 3 * p.height * p.width
+        blocks += p.num_blocks
+        max_blocks, max_pixels = max(max_blocks, p.num_blocks), max(max_pixels, p.height * p.width)
+    iv_arr = np.array(ivs, dtype=_JPEG_INTERVAL)
+    tab_arr = np.stack(tables)
+    o_iv = _align16(descs.nbytes)
+    o_tab = o_iv + _align16(iv_arr.nbytes)
+    o_data = o_tab + _align16(tab_arr.nbytes)
+    staging = torch.empty((o_data + data_bytes,), dtype=torch.uint8, pin_memory=True)
+    st = staging.numpy()
+    st[:descs.nbytes] = descs.view(np.uint8)
+    st[o_iv:o_iv + iv_arr.nbytes] = iv_arr.view(np.uint8)
+    st[o_tab:o_tab + tab_arr.nbytes] = tab_arr.view(np.uint8).reshape(-1)
+    for off, buf in datas:
+        st[o_data + off:o_data + off + len(buf)] = np.frombuffer(buf, np.uint8)
+    buf = torch.empty((o_data + data_bytes,), dtype=torch.uint8, device=dev)
+    buf.copy_(staging, non_blocking=True)          # pinned, stream-ordered: the allocator keeps `staging` until it completes
+    if out is None:
+        out = torch.empty((out_bytes,), dtype=torch.uint8, device=dev)
+    elif not (out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= out_bytes and out.device == dev):
+        raise ValueError("out must be a contiguous uint8 CUDA tensor of at least %d bytes on %s" % (out_bytes, dev))
+    dstatus = torch.empty((n,), dtype=torch.uint8, device=dev)
+    ws, ws_ptr = _workspace(_lib.load().b200_jpeg_decode_workspace_bytes(blocks, subseqs), dev)
+    base = buf.data_ptr()
+    _launch("b200_jpeg_decode", dev, base + o_data, base, n, base + o_iv, len(ivs), base + o_tab, int(subseq_bits), blocks, subseqs,
+            max_blocks, max_pixels, ws_ptr, ws.numel(), out.data_ptr(), dstatus.data_ptr())
+    status[torch.as_tensor(dev_idx, device=dev)] = dstatus
+    flat = out.reshape(-1)
+    for d, i in enumerate(dev_idx):
+        oh, ow = parsed[i].out_shape
+        o = int(descs[d]["out_offset"])
+        images[i] = flat[o:o + 3 * oh * ow].view(oh, ow, 3)
+    return images, status
+
+
+# ------------------------------------------------------------------------------------------------
 # COCO evaluation stages (pycocotools COCOeval.evaluate / accumulate; datasets/coco_eval.py drives them)
 # ------------------------------------------------------------------------------------------------
 def coco_rank_raw(pair_det_begin, pair_entry_begin, det_score, num_entries):

@@ -695,6 +695,74 @@ B200_API int b200_fast_rcnn_loss_backward(int num_rois, int num_classes, int bbo
                                           const float* inside_weights_dev, const float* outside_weights_dev, const float* grad_losses_dev,
                                           float* cls_grad_out_dev, float* bbox_grad_out_dev, b200_stream_t stream);
 
+/* ---- JPEG decode (cv2.imread / cv2.imdecode, IMREAD_COLOR: lib/roi_data/minibatch.py:58, lib/core/test_engine.py:252,
+ *      tools/infer_simple.py:144) ------------------------------------------------------------------------------------------
+ * Baseline Huffman JPEG, 8-bit, one interleaved scan: 3 YCbCr components with luma sampling h, v in {1, 2} and chroma 1x1, or
+ * 1 component; restart intervals allowed.  The host parses the headers (detectron/pytorch_b200/utils/jpeg.py), derives the
+ * Huffman decode tables and cuts each scan into restart intervals with the 0xFF00 stuffing removed.  The device decodes every
+ * interval in parallel by self-synchronisation, then dequantises with libjpeg's islow IDCT, upsamples the chroma with
+ * libjpeg-turbo's fancy filters, converts with its integer YCbCr -> BGR tables and applies the EXIF orientation; the result
+ * equals cv2's pixels bit for bit.  Three kernel launches for all images of a call (csrc/jpeg.cu).
+ *
+ * b200_jpeg_huff_table: one derived Huffman table (T.81 F.2.2.3):
+ *   lookup[p]  (length << 8) | symbol of the code of length <= 9 that prefixes the 9-bit window p, 0 when there is none;
+ *   maxcode[l] the largest code of length l (-1: none), l = 1..16; valoff[l]: values index of a code of length l minus the code.
+ * b200_jpeg_desc, one per image (all offsets non-negative):
+ *   out_offset    byte offset of the image's (out_h, out_w, 3) uint8 BGR output in out_dev, out_h x out_w = height x width,
+ *                 transposed for orientations 5-8;
+ *   first_block   its first 8x8 block in the workspace; its blocks are mcus_x * mcus_y * (h * v + 2) (3 components) or
+ *                 mcus_x * mcus_y (1 component, h = v = 1), and the images' block ranges must not overlap;
+ *   height, width the coded size; ncomp 1 or 3; h, v the luma sampling factors; mcus_x, mcus_y the MCU grid;
+ *   orientation   the EXIF orientation 1-8 (cv2's transform: 2 flips x, 3 both, 4 y, 5 transposes, 6-8 transpose then flip);
+ *   table         index in tables_dev of its DC tables for components 0 .. ncomp - 1, followed by their AC tables;
+ *   quant         per component its quantisation table in natural order, values 1-255.
+ * b200_jpeg_interval, one per restart interval (the whole scan when there are none), those of an image in scan order:
+ *   data_offset / nbytes  its unstuffed entropy data in data_dev, nbytes < 2^28;
+ *   image, first_mcu, num_mcus  its image and MCU range;
+ *   first_subseq  its first slot in the per-subsequence state: it takes max(1, ceil(8 nbytes / subseq_bits)) slots, and the
+ *                 intervals' slot ranges must not overlap (total_subseqs slots in all).
+ * subseq_bits is the subsequence length S of the parallel decode (any S >= 1 gives the same result; it sets the work split).
+ * max_blocks / max_pixels: the largest block count / height * width of one image of the call (grid sizes).
+ * status_dev (num_images) uint8: 0 = decoded, B200_JPEG_ENTROPY_ERROR = the entropy data of the image does not decode to exactly
+ *   its blocks (a bad code, a truncated interval, a coefficient index past 63); that image's output is not written and the
+ *   caller decodes it another way.  Every read is bounded by its interval and every write by its blocks.
+ * Bad sizes or null pointers: B200_ROI_EINVAL; a workspace smaller than b200_jpeg_decode_workspace_bytes(total_blocks,
+ * total_subseqs): B200_ROI_EWORKSPACE; both before any launch (the descriptors live on the device and are not read by the host). */
+#define B200_JPEG_ENTROPY_ERROR 2
+
+typedef struct b200_jpeg_huff_table {
+    unsigned short lookup[512];
+    int maxcode[18];
+    int valoff[18];
+    unsigned char values[256];
+} b200_jpeg_huff_table;
+
+typedef struct b200_jpeg_desc {
+    long long out_offset;
+    long long first_block;
+    int height, width;
+    int ncomp, h, v;
+    int mcus_x, mcus_y;
+    int orientation;
+    int table, reserved;
+    unsigned short quant[3][64];
+} b200_jpeg_desc;
+
+typedef struct b200_jpeg_interval {
+    long long data_offset;
+    int nbytes;
+    int image;
+    int first_mcu, num_mcus;
+    long long first_subseq;
+} b200_jpeg_interval;
+
+B200_API size_t b200_jpeg_decode_workspace_bytes(long long total_blocks, long long total_subseqs);
+B200_API int b200_jpeg_decode(const unsigned char* data_dev, const b200_jpeg_desc* descs_dev, int num_images,
+                              const b200_jpeg_interval* intervals_dev, int num_intervals, const b200_jpeg_huff_table* tables_dev,
+                              int subseq_bits, long long total_blocks, long long total_subseqs, long long max_blocks, long long max_pixels,
+                              void* workspace, size_t workspace_bytes, unsigned char* out_dev, unsigned char* status_dev,
+                              b200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
