@@ -9,8 +9,7 @@
 namespace b200 {
 unsigned long long g_launch_count = 0;
 
-static const char* const kOptionNames[kNumOptions] = {"B200_ROI_ALIGN_PATH", "B200_ROI_ALIGN_BWD_PATH", "B200_ROI_ALIGN_BWD_CPL",
-                                                      "B200_NMS_SCAN"};
+static const char* const kOptionNames[kNumOptions] = {"B200_ROI_ALIGN_PATH", "B200_ROI_ALIGN_BWD_PATH"};
 static int g_options[kNumOptions];
 static std::once_flag g_options_once;
 
@@ -129,10 +128,9 @@ unsigned long long b200_roi_ops_launch_count(void) { return g_launch_count; }
 
 int b200_roi_ops_set_option(const char* name, const char* value) { return option_set(name, value); }
 
-void b200_roi_ops_debug_timing_buffer(void* device_u64x16) {
-    nms_set_timing_buffer((unsigned long long*)device_u64x16);
-    roi_align_stream_set_debug_buffer((unsigned long long*)device_u64x16);      // watchdog records of the streaming-strip path
-    roi_align_strip_set_debug_buffer((unsigned long long*)device_u64x16);       // watchdog records of the quad-strip path
+void b200_roi_ops_debug_timing_buffer(void* host_pinned) {
+    roi_align_stream_set_debug_buffer((unsigned long long*)host_pinned);      // watchdog records of the streaming-strip path
+    roi_align_strip_set_debug_buffer((unsigned long long*)host_pinned);       // watchdog records of the quad-strip path
 }
 
 size_t b200_roi_align_workspace_bytes(int batch_size, int num_rois, int height, int width, int aligned_height,

@@ -28,8 +28,6 @@ constexpr int kPathDeclined = 1000;
 enum Option {
     kOptFwdPath = 0,      // B200_ROI_ALIGN_PATH      = auto | generic | tiled | stream | quad (auto: stream first, then quad; api.cu)
     kOptBwdPath,          // B200_ROI_ALIGN_BWD_PATH  = auto | generic | nhwc | rows
-    kOptBwdCpl,           // B200_ROI_ALIGN_BWD_CPL   = 4 | 2
-    kOptNmsScan,          // B200_NMS_SCAN            = resolver | simple
     kNumOptions
 };
 int option_get(Option which);
@@ -65,8 +63,7 @@ int roi_align_backward_rows(const float* top_diff, float scale, int N, int R, in
 // Transposes a channel-innermost gradient image back to NCHW (roi_align_bwd_nhwc.cu; RoICrop's backward uses it too).
 void launch_nhwc_to_nchw(const float* scratch, float* dx, int N, int C, int HW, cudaStream_t stream);
 
-// Debug records (b200_roi_ops_debug_timing_buffer): NMS timing (nms.cu) and the watchdogs of the streaming and quad-strip paths.
-void nms_set_timing_buffer(unsigned long long* buf);
+// Watchdog records of the streaming and quad-strip paths (b200_roi_ops_debug_timing_buffer).
 void roi_align_stream_set_debug_buffer(unsigned long long* host_pinned);
 void roi_align_strip_set_debug_buffer(unsigned long long* host_pinned);
 

@@ -46,9 +46,6 @@ __device__ __forceinline__ void mbar_wait(u64* bar, unsigned parity) {
         "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
 
-// Debug: per-phase clock64 totals of the resolver warp (tools/nms_probe.py); null by default.
-__device__ unsigned long long* g_nms_timing = nullptr;
-
 struct __align__(16) ColBox {
     float x0, y0, x1, y1;
 };
@@ -165,13 +162,7 @@ __device__ __forceinline__ void nms_mask_tile(const float* __restrict__ boxes, i
     }
 }
 
-__global__ void __launch_bounds__(kNmsTile)
-nms_mask_kernel(const float* __restrict__ boxes, int n, int dim, float thresh, float lo, float hi,
-                u64* __restrict__ mask, u64* __restrict__ diag_t) {
-    nms_mask_tile<false>(boxes, n, dim, thresh, lo, hi, mask, diag_t, (int)blockIdx.x);
-}
-
-// ---- several independent problems in one launch (SURVEY 8f N1: the (image, level) proposal sets of one step) ----
+// ---- independent problems in one launch (SURVEY 8f N1: the (image, level) proposal sets of one step; b200_nms is one problem) ----
 constexpr int kNmsMaxProblems = 64;
 struct NmsBatch {
     int count;
@@ -291,14 +282,10 @@ __device__ __forceinline__ void nms_scan_resolver_body(const u64* __restrict__ m
 #pragma unroll
         for (int t = 0; t < REACH; ++t) c[t] = 0;
         int count = 0;
-        unsigned long long* const timing = g_nms_timing;
-        long long t_wait = 0, t_res = 0, t_rest = 0, t_keep = 0, rounds = 0;
         const u64 bit0 = 1ULL << lane, bit1 = 1ULL << (lane + 32);
         for (int b = 0; b < col_blocks; ++b) {
             const u64 T0 = D[b * kNmsTile + lane], T1 = D[b * kNmsTile + lane + 32];
-            const long long t0 = timing ? clock64() : 0;
             if (b >= REACH) mbar_wait(&fold_bar[b - REACH], 0);
-            const long long t1 = timing ? clock64() : 0;
             const int lim = min(kNmsTile, n - b * kNmsTile);
             u64 rem = *reinterpret_cast<volatile u64*>(&remv[b]) | c[1];
             if (lim < kNmsTile) rem |= ~((1ULL << lim) - 1ULL);       // padded rows: decided, never kept
@@ -312,10 +299,8 @@ __device__ __forceinline__ void nms_scan_resolver_body(const u64* __restrict__ m
                 const unsigned r_lo = __ballot_sync(0xffffffffu, nr0), r_hi = __ballot_sync(0xffffffffu, nr1);
                 kept |= ((u64)k_hi << 32) | k_lo;
                 rem |= ((u64)r_hi << 32) | r_lo;
-                if (timing) ++rounds;
             }
             if (lane == 0) { kept_hist[b] = kept; mbar_arrive(&res_bar[b]); }
-            const long long t2 = timing ? clock64() : 0;
             // contributions of this block's kept rows to the next REACH-1 columns; shift the carries by one column
             const bool ka = (kept >> lane) & 1ULL, kb2 = (kept >> (lane + 32)) & 1ULL;
 #pragma unroll
@@ -328,15 +313,12 @@ __device__ __forceinline__ void nms_scan_resolver_body(const u64* __restrict__ m
                 const u64 kt = ((u64)hi << 32) | lo;
                 c[t] = ((t + 1 < REACH) ? c[t + 1] : 0ULL) | kt;
             }
-            const long long t2b = timing ? clock64() : 0;
             const u64 lo_mask = (1ULL << lane) - 1ULL;
             if (ka) keep_out[count + __popcll(kept & lo_mask)] = b * kNmsTile + lane;
             if (kb2) keep_out[count + __popcll(kept & ((lo_mask << 32) | 0xffffffffULL))] = b * kNmsTile + lane + 32;
             count += __popcll(kept);
-            if (timing) { const long long t3 = clock64(); t_wait += t1 - t0; t_res += t2 - t1; t_rest += t3 - t2; t_keep += t3 - t2b; }
         }
         if (lane == 0) *num_out = count;
-        if (timing && lane == 0) { timing[0] = t_wait; timing[1] = t_res; timing[2] = t_rest; timing[3] = col_blocks; timing[4] = rounds; timing[8] = t_keep; }
     } else if ((warp & 3) != 0) {
         // Workers sit on warp slots with (warp & 3) != 0: warp w issues from scheduler w & 3, so the resolver warp has
         // scheduler 0 to itself and its dependent chain is never delayed by the workers' polling loops.  Group g folds
@@ -345,12 +327,8 @@ __device__ __forceinline__ void nms_scan_resolver_body(const u64* __restrict__ m
         const int ww = (warp >> 2) * 3 + (warp & 3) - 1;
         const int g = ww / kFoldWarps, wi = ww - g * kFoldWarps;
         unsigned* remv32 = reinterpret_cast<unsigned*>(remv);
-        unsigned long long* const timing = (ww == 0) ? g_nms_timing : nullptr;
-        long long t_spin = 0, t_fold = 0, folds = 0;
         for (int b = g; b < col_blocks; b += kFoldGroups) {
-            const long long t0 = timing ? clock64() : 0;
             mbar_wait(&res_bar[b], 0);
-            const long long t1 = timing ? clock64() : 0;
             const u64 kept = *reinterpret_cast<volatile u64*>(&kept_hist[b]);
             const int ncols = col_blocks - (b + REACH);
             if (ncols > 0) {
@@ -388,17 +366,8 @@ __device__ __forceinline__ void nms_scan_resolver_body(const u64* __restrict__ m
             }
             __syncwarp();
             if (lane == 0) mbar_arrive(&fold_bar[b]);
-            if (timing) { const long long t2 = clock64(); t_spin += t1 - t0; t_fold += t2 - t1; ++folds; }
         }
-        if (timing && lane == 0) { timing[5] = t_spin; timing[6] = t_fold; timing[7] = folds; }
     }
-}
-
-template <int REACH>
-__global__ void __launch_bounds__(kScanThreads)
-nms_scan_resolver_kernel(const u64* __restrict__ mask, const u64* __restrict__ diag_t, int n, int col_blocks,
-                         int* __restrict__ keep_out, int* __restrict__ num_out) {
-    nms_scan_resolver_body<REACH>(mask, diag_t, n, col_blocks, keep_out, num_out);
 }
 
 // one CTA per problem
@@ -414,8 +383,6 @@ nms_scan_resolver_batched_kernel(const u64* __restrict__ ws, const __grid_consta
 }
 
 __global__ void nms_empty_kernel(int* num_out) { *num_out = 0; }
-
-void nms_set_timing_buffer(unsigned long long* buf) { cudaMemcpyToSymbol(g_nms_timing, &buf, sizeof(buf)); }
 
 // ---- batched entry: `num_problems` independent score-sorted box sets, stored back to back in `boxes` ----
 static bool nms_batch_plan(const int* counts, int num_problems, NmsBatch* nb, size_t* ws_words, int* max_n) {
@@ -468,7 +435,7 @@ static int nms_batched(const float* boxes, const int* counts, int num_problems, 
         (cython ? nms_mask_batched_kernel<true> : nms_mask_batched_kernel<false>)<<<(unsigned)nb.tile_off[num_problems], kNmsTile, 0, stream>>>(
             boxes, nb, dim, thresh, lo, hi, ws);
     if (reach == 0) {
-        // a problem too large for the pipelined scan (> ~13.8k boxes): b200_nms's unpipelined scan, one launch per problem
+        // a problem too large for the pipelined scan (> ~13.8k boxes): the unpipelined scan, one launch per problem
         const size_t smem = sizeof(u64) * (size_t)cb;
         if (smem > 48 * 1024) {
             cudaError_t e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -511,36 +478,9 @@ int b200_nms(const float* boxes, int n, int dim, float thresh, int* keep_out, in
         return finish_launch();
     }
     if (workspace == nullptr || workspace_bytes < b200_nms_workspace_bytes(n)) return B200_ROI_EWORKSPACE;
-    const int cb = (n + kNmsTile - 1) / kNmsTile;
-    u64* mask = (u64*)workspace;
-    u64* diag_t = mask + (size_t)n * cb;
-    float lo = -INFINITY, hi = INFINITY;            // decision band of the division-free IoU test (see nms_mask_kernel)
-    if (thresh >= 9.5367431640625e-07f && thresh <= 1048576.f) {
-        lo = (float)((double)thresh * (1.0 - 3.814697265625e-06));
-        hi = (float)((double)thresh * (1.0 + 3.814697265625e-06));
-    }
-    const long long tiles = (long long)cb * (cb + 1) / 2;
-    if (tiles > 0x7fffffffLL) return B200_ROI_EINVAL;
-    nms_mask_kernel<<<(unsigned)tiles, kNmsTile, 0, stream>>>(boxes, n, dim, thresh, lo, hi, mask, diag_t);
-    const bool simple = option_get(kOptNmsScan) == 's';       // "simple" selects the unpipelined scan (A/B tests)
-    for (int reach = 4; reach >= 2 && !simple; --reach) {
-        const size_t smem_res = sizeof(u64) * ((size_t)reach * cb * kNmsTile + 4 * (size_t)cb) + 16;
-        if (smem_res > 224 * 1024) continue;
-        void (*kern)(const u64*, const u64*, int, int, int*, int*) =
-            (reach == 4) ? nms_scan_resolver_kernel<4> : (reach == 3) ? nms_scan_resolver_kernel<3> : nms_scan_resolver_kernel<2>;
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_res);
-        if (e != cudaSuccess) return (int)e;
-        kern<<<1, kScanThreads, smem_res, stream>>>(mask, diag_t, n, cb, keep_out, num_out);
-        return finish_launch(2);
-    }
-    // very large inputs (> ~13.8k boxes): the near-diagonal words do not fit shared memory; unpipelined scan
-    const size_t smem = sizeof(u64) * (size_t)cb;
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return (int)e;
-    }
-    nms_scan_kernel<<<1, kScanThreads, smem, stream>>>(mask, n, cb, keep_out, num_out);
-    return finish_launch(2);
+    // a batch of one problem: its mask words start at the workspace and its transposed diagonal words follow them, the
+    // layout b200_nms_workspace_bytes sizes
+    return nms_batched(boxes, &n, 1, dim, thresh, false, keep_out, num_out, workspace, workspace_bytes, stream);
 }
 
 size_t b200_nms_batched_workspace_bytes(const int* counts, int num_problems) {

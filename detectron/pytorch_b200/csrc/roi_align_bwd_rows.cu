@@ -436,11 +436,11 @@ int roi_align_backward_rows(const float* top_diff, float scale, int N, int R, in
         reinterpret_cast<AxisEntry*>(ws + p.xtab_off), reinterpret_cast<int*>(ws + p.zero_off),
         reinterpret_cast<uint2*>(ws + p.row_list_off), p.row_cap, reinterpret_cast<uint4*>(ws + p.ovf_off),
         reinterpret_cast<float*>(ws + p.dyt_off), row_map);
-    const bool want4 = option_get(kOptBwdCpl) != '2';           // channels per lane of the main kernel: 2 | 4 (A/B tests)
+    // channels per lane of the main kernel: 4 where PW == 7 and C % 128 == 0, else 2
     int rc;
     if (PW == 7) {
-        if (want4 && (C % 128) == 0) rc = (sr == 1) ? launch_rows<7, 1, 4, 12>(p, ws, bottom_diff, N, C, H, W, PH, stream)
-                                                     : launch_rows<7, 2, 4, 12>(p, ws, bottom_diff, N, C, H, W, PH, stream);
+        if ((C % 128) == 0) rc = (sr == 1) ? launch_rows<7, 1, 4, 12>(p, ws, bottom_diff, N, C, H, W, PH, stream)
+                                           : launch_rows<7, 2, 4, 12>(p, ws, bottom_diff, N, C, H, W, PH, stream);
         else rc = (sr == 1) ? launch_rows<7, 1, 2, 12>(p, ws, bottom_diff, N, C, H, W, PH, stream)
                             : launch_rows<7, 2, 2, 12>(p, ws, bottom_diff, N, C, H, W, PH, stream);
     } else {

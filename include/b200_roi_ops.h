@@ -278,16 +278,15 @@ B200_API int b200_nms_oks(const float* xy_preds_dev, const float* rois_dev, int 
  * Number of kernel launches the library has enqueued since load (all entry points). */
 B200_API unsigned long long b200_roi_ops_launch_count(void);
 /* Path-selection switches (A/B runs and tests reach paths the dispatch otherwise picks by shape): name is one of
- * "B200_ROI_ALIGN_PATH" (auto|generic|tiled|stream|quad), "B200_ROI_ALIGN_BWD_PATH" (auto|generic|nhwc|rows),
- * "B200_ROI_ALIGN_BWD_CPL" (4|2), "B200_NMS_SCAN" (resolver|simple);
+ * "B200_ROI_ALIGN_PATH" (auto|generic|tiled|stream|quad) or "B200_ROI_ALIGN_BWD_PATH" (auto|generic|nhwc|rows);
  * value NULL or "" restores the default.  Each switch takes its initial value from the
  * environment variable of the same name, read once at first use -- no entry point calls getenv() on the hot path.
  * Returns 0, or B200_ROI_EINVAL for an unknown name. */
 B200_API int b200_roi_ops_set_option(const char* name, const char* value);
-/* Debug: register (or clear with NULL) one buffer with two uses.  The NMS kernels add their phase clock deltas to its
- * first 16 uint64 words.  The two streaming RoIAlign forwards write a watchdog record into [CTA][32] uint64 (one word per
- * warp) when a wait has spun half way to its trap; host-pinned memory keeps those records readable after the trap. */
-B200_API void b200_roi_ops_debug_timing_buffer(void* device_u64x16);
+/* Debug: register (or clear with NULL) a host-pinned buffer of [CTA][32] uint64 (one word per warp) for watchdog records.
+ * The two streaming RoIAlign forwards write a record there when a wait has spun half way to its trap; host-pinned memory
+ * keeps the records readable after the trap.  Nothing else writes to it. */
+B200_API void b200_roi_ops_debug_timing_buffer(void* host_pinned);
 
 /* ---- RPN proposal decode (SURVEY.md 8f N1: the GPU-resident proposal layer) --------------------------------
  * replaces the numpy block of GenerateProposalsOp.proposals_for_one_image, lib/modeling/generate_proposals.py:108-150

@@ -151,16 +151,17 @@ def test_workspace_sizing_is_host_arithmetic(lib_option):
     assert lib.b200_roi_align_backward_ws(None, 0.25, 1, 4, 10, -1, 3, 7, 7, 2, None, None, None, 0, None) == -1
 
 
-KEPT_SWITCHES = {"B200_ROI_ALIGN_PATH": b"generic", "B200_ROI_ALIGN_BWD_PATH": b"generic", "B200_ROI_ALIGN_BWD_CPL": b"2",
-                 "B200_NMS_SCAN": b"simple"}
-# tuning and timing switches of earlier versions (variants the dispatch never chose, probes with undefined output)
-RETIRED_SWITCHES = ["B200_" + s for s in ("STREAM_STAGE", "STREAM_PHASES", "STRIP_ROWCOST", "STRIP_PDL", "FWD_ZERO", "BWD_TRCH", "FPN_PATH")]
+KEPT_SWITCHES = {"B200_ROI_ALIGN_PATH": b"generic", "B200_ROI_ALIGN_BWD_PATH": b"generic"}
+# tuning and timing switches of earlier versions (variants the dispatch never chose, probes with undefined output) and the
+# forced backward channels-per-lane and NMS scan variants
+RETIRED_SWITCHES = ["B200_" + s for s in ("STREAM_STAGE", "STREAM_PHASES", "STRIP_ROWCOST", "STRIP_PDL", "FWD_ZERO", "BWD_TRCH", "FPN_PATH",
+                                          "ROI_ALIGN_BWD_CPL", "NMS_SCAN")]
 
 
 @pytest.mark.parametrize("name", ["NO_SUCH_SWITCH"] + RETIRED_SWITCHES + sorted(KEPT_SWITCHES))
 def test_set_option_accepts_only_path_switches(name):
-    """b200_roi_ops_set_option knows the four switches that force a path the dispatch otherwise picks by shape; any other
-    name, including the retired tuning and timing switches, is B200_ROI_EINVAL."""
+    """b200_roi_ops_set_option knows the two switches that force a path the dispatch otherwise picks by shape; any other
+    name, including the retired tuning, timing and variant switches, is B200_ROI_EINVAL."""
     lib = _lib.load()
     if name not in KEPT_SWITCHES:
         assert lib.b200_roi_ops_set_option(name.encode(), b"x") == -1

@@ -17,7 +17,7 @@ def greedy(sup, removed0):
 
 
 def fixed_point(sup, removed0):
-    """sup[j, i] (j < i): box j suppresses box i.  Rounds as in nms_scan_resolver_kernel: an undecided box whose
+    """sup[j, i] (j < i): box j suppresses box i.  Rounds as in nms_scan_resolver_body: an undecided box whose
     suppressors are all removed is kept; one with a kept suppressor is removed."""
     n = sup.shape[0]
     T = sup.T                                                   # T[i, j]: j suppresses i  (the transposed diagonal word)

@@ -5,8 +5,8 @@ the unfused oracle bit for bit, the fused oracle within 1e-4, the fp64 backward 
 
 GPU part (`-m gpu`):
   * every case under each forced forward path (generic, tiled, stream, quad) and each forced backward path (generic, nhwc,
-    rows with 2 and 4 channels per lane).  The launch counter proves which path ran: a case a path must accept runs it
-    (forward: stream 3 launches, quad 2, tiled 2; backward: rows 2, nhwc 2), a case it must decline falls back to the
+    rows: 4 channels per lane at P = 7 and C % 128 == 0, else 2).  The launch counter proves which path ran: a case a path
+    must accept runs it (forward: stream 3 launches, quad 2, tiled 2; backward: rows 2, nhwc 2), a case it must decline falls back to the
     generic kernel (1 launch).  Values against the oracle with the tolerances of test_gpu_parity.py (generic forward
     bit-exact; tiled / stream / quad forward 1e-6; backward 1e-5 against fp64), and on the rectangular-bin cases against
     the reference kernel's sm_90a build (tests/golden/roi_align_geometry_sm90a.npz);
@@ -32,7 +32,6 @@ GRAD_TOL = dict(rtol=1e-5, atol=1e-5)
 NAMES = sorted(GC.GEOMETRY_CASES)
 FWD_LAUNCHES = {"generic": 1, "tiled": 2, "stream": 3, "quad": 2}     # prepass + main (+ fill for stream); memsets are not counted
 BWD_LAUNCHES = {"generic": 1, "nhwc": 2, "rows": 2}
-BWD_VARIANTS = {"generic": ("generic", None), "nhwc": ("nhwc", None), "rows-cpl2": ("rows", "2"), "rows-cpl4": ("rows", "4")}
 SENTINEL = 0x7FC0DEAD                 # a quiet NaN with a payload no kernel produces
 GUARD = 1024                          # elements behind every output buffer that must stay untouched
 
@@ -126,16 +125,13 @@ def test_forward_forced_path(name, path, lib_option):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", sorted(BWD_VARIANTS))
+@pytest.mark.parametrize("path", ["generic", "nhwc", "rows"])
 @pytest.mark.parametrize("name", NAMES)
-def test_backward_forced_path(name, variant, lib_option):
+def test_backward_forced_path(name, path, lib_option):
     from detectron.pytorch_b200 import _lib, ops
     c, f, r, dy, _, ref_dx = oracle_case(name)
     PH, PW, s, sr = c["PH"], c["PW"], c["scale"], c["sr"]
-    path, cpl = BWD_VARIANTS[variant]
     lib_option("B200_ROI_ALIGN_BWD_PATH", path)
-    if cpl:
-        lib_option("B200_ROI_ALIGN_BWD_CPL", cpl)
     DY, Rt = dev(dy), dev(r)
     before = _lib.launch_count()
     dx = ops.roi_align_backward(DY, Rt, c["shape"], PH, PW, s, sr)

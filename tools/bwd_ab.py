@@ -1,5 +1,5 @@
 """A/B timing of the RoIAlign backward at BASELINE cfg2 with CUDA events (rotating inputs larger than L2).
-    python tools/bwd_ab.py [--iters 60]        # options come from the environment (B200_ROI_ALIGN_BWD_PATH, B200_ROI_ALIGN_BWD_CPL)
+    python tools/bwd_ab.py [--iters 60]        # options come from the environment (B200_ROI_ALIGN_BWD_PATH)
 """
 import argparse, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

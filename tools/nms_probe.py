@@ -1,8 +1,10 @@
-"""Runs nms_gpu a few times on BASELINE cfg3 (6000 boxes) -- target for `ncu -k regex:nms`."""
-import os, sys
+"""NMS on BASELINE cfg3 (6000 boxes): time per call (CUDA events) and the kept count; prints the card and its power limit."""
+import os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from detectron.pytorch_b200 import ops, synthetic as S
+card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+print("card:", card)
 b = torch.from_numpy(S.make_nms_boxes(6000)).cuda()
 for _ in range(3):
     keep, num = ops.nms_raw(b, 0.7)
@@ -13,13 +15,3 @@ for _ in range(20):
     ops.nms_raw(b, 0.7)
 e1.record(); torch.cuda.synchronize()
 print("nms 6000: %.1f us/call, kept %d" % (e0.elapsed_time(e1) / 20 * 1e3, int(num.item())))
-
-from detectron.pytorch_b200 import _lib
-buf = torch.zeros(16, dtype=torch.int64, device="cuda")
-lib = _lib.load(); lib.b200_roi_ops_debug_timing_buffer(buf.data_ptr())
-ops.nms_raw(b, 0.7); torch.cuda.synchronize(); lib.b200_roi_ops_debug_timing_buffer(None)
-t = buf.tolist()
-if t[3]:
-    print("resolver cycles/block: wait-for-folds %.0f  resolve %.0f  carry+keep %.0f  (blocks %d, resolve rounds/block %.1f)" % (t[0] / t[3], t[1] / t[3], t[2] / t[3], t[3], t[4] / t[3]))
-    if t[7]:
-        print("worker 0 cycles/fold: wait-for-resolver %.0f  fold %.0f  (folds %d); resolver keep-stores %.0f/block" % (t[5] / t[7], t[6] / t[7], t[7], t[8] / t[3]))
