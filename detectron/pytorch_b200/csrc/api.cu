@@ -2,12 +2,50 @@
 // and the RoIAlign forward / backward path dispatch (see include/b200_roi_ops.h).  Every other entry point is defined beside
 // its kernels, in its op's translation unit.
 #include "common.cuh"
+#include <map>
 #include <mutex>
 #include <stdlib.h>
 #include <string.h>
+#include <utility>
 
 namespace b200 {
 unsigned long long g_launch_count = 0;
+
+// Per-device kernel setup: the dynamic shared-memory limit recorded for each (kernel, device) pair and each device's SM
+// count.  Both live in the device's context, so they are kept per device ordinal.
+static std::mutex g_setup_mu;
+static std::map<std::pair<const void*, int>, size_t> g_smem_limit;
+static std::map<int, int> g_sm_count;
+
+int smem_opt_in(const void* kernel, size_t bytes) {
+    if (bytes <= 48 * 1024) return B200_ROI_OK;
+    int dev = 0;
+    cudaError_t err = cudaGetDevice(&dev);
+    if (err != cudaSuccess) { (void)cudaGetLastError(); return (int)err; }
+    std::lock_guard<std::mutex> lock(g_setup_mu);
+    size_t& limit = g_smem_limit[{kernel, dev}];
+    if (limit >= bytes) return B200_ROI_OK;
+    err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (err != cudaSuccess) { (void)cudaGetLastError(); return (int)err; }
+    limit = bytes;
+    return B200_ROI_OK;
+}
+
+int device_sm_count(int* sm_count) {
+    int dev = 0;
+    cudaError_t err = cudaGetDevice(&dev);
+    if (err != cudaSuccess) { (void)cudaGetLastError(); return (int)err; }
+    std::lock_guard<std::mutex> lock(g_setup_mu);
+    auto it = g_sm_count.find(dev);
+    if (it == g_sm_count.end()) {
+        int n = 0;
+        err = cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+        if (err != cudaSuccess) { (void)cudaGetLastError(); return (int)err; }
+        it = g_sm_count.emplace(dev, n).first;
+    }
+    *sm_count = it->second;
+    return B200_ROI_OK;
+}
 
 static const char* const kOptionNames[kNumOptions] = {"B200_ROI_ALIGN_PATH", "B200_ROI_ALIGN_BWD_PATH"};
 static int g_options[kNumOptions];

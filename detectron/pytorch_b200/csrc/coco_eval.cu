@@ -606,8 +606,7 @@ int b200_coco_match(int num_pairs, int T, const double* iou_thrs_host, int A, co
     mp.T = T; mp.A = A;
     for (int t = 0; t < T; ++t) mp.thr[t] = iou_thrs_host[t];
     for (int a = 0; a < A; ++a) { mp.area_lo[a] = area_rng_host[2 * a]; mp.area_hi[a] = area_rng_host[2 * a + 1]; }
-    if (smem > 48 * 1024 && cudaFuncSetAttribute(coco_match_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return finish_launch(0);
+    if (const int rc = smem_opt_in(coco_match_kernel, smem)) return rc;
     coco_match_kernel<<<num_pairs, 64, smem, stream>>>(mp, pair_gt_begin, pair_entry_begin, pair_iou_begin, pair_cat, entry_det, det_area,
                                                        gt_area, gt_flags, ious, num_entries, entry_flags, npig);
     return finish_launch();

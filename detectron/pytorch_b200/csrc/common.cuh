@@ -17,6 +17,17 @@ inline int finish_launch(int n_launches = 1) {
 
 constexpr int kNumSMs = 132;   // H100 SXM
 
+// ---- per-device kernel setup (api.cu) -------------------------------------------------------------
+// Makes `kernel` launchable with `bytes` of dynamic shared memory on the current device.  The limit only ever rises: it is
+// set under one lock, the first time a (kernel, device) pair needs more than the limit already recorded for it, so calls
+// from several host threads never lower a limit another call is about to launch with.  Requests of 48 KB or less return at
+// once.  On failure, clears the CUDA error and returns it; the caller decides whether that means decline or error.
+int smem_opt_in(const void* kernel, size_t bytes);
+template <class K> int smem_opt_in(K* kernel, size_t bytes) { return smem_opt_in((const void*)kernel, bytes); }
+
+// SM count of the current device, queried once per device (0 / error status on failure).
+int device_sm_count(int* sm_count);
+
 // Status of a fast path that does not apply to the shape or workspace it was given: the caller falls back to another path.
 // Neither B200_ROI_OK, a negative B200_ROI_E* code nor a CUDA runtime error (those stop at cudaErrorUnknown = 999).
 constexpr int kPathDeclined = 1000;

@@ -436,11 +436,7 @@ static int nms_batched(const float* boxes, const int* counts, int num_problems, 
             boxes, nb, dim, thresh, lo, hi, ws);
     if (reach == 0) {
         // a problem too large for the pipelined scan (> ~13.8k boxes): the unpipelined scan, one launch per problem
-        const size_t smem = sizeof(u64) * (size_t)cb;
-        if (smem > 48 * 1024) {
-            cudaError_t e = cudaFuncSetAttribute(nms_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return (int)e;
-        }
+        if (const int rc = smem_opt_in(nms_scan_kernel, sizeof(u64) * (size_t)cb)) return rc;
         for (int p = 0; p < num_problems; ++p) {
             const int n = nb.n[p];
             if (n == 0) nms_empty_kernel<<<1, 1, 0, stream>>>(num_out + p);
@@ -451,8 +447,7 @@ static int nms_batched(const float* boxes, const int* counts, int num_problems, 
     }
     void (*kern)(const u64*, const NmsBatch, int*, int*) =
         (reach == 4) ? nms_scan_resolver_batched_kernel<4> : (reach == 3) ? nms_scan_resolver_batched_kernel<3> : nms_scan_resolver_batched_kernel<2>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_res);
-    if (e != cudaSuccess) return (int)e;
+    if (const int rc = smem_opt_in(kern, smem_res)) return rc;
     kern<<<num_problems, kScanThreads, smem_res, stream>>>(ws, nb, keep_out, num_out);
     return finish_launch(2);
 }

@@ -155,21 +155,10 @@ int roi_align_backward_nhwc(const float* top_diff, float scale, int N, int R, in
     const size_t smem = sizeof(float) * (size_t)PH * PW * c_pad;
     if (smem > 200 * 1024) return kPathDeclined;
     dim3 grid(R, (C + kBwChunk - 1) / kBwChunk);
-#define B200_LAUNCH_BW(SRV)                                                                                              \
-    do {                                                                                                                 \
-        if (smem > 48 * 1024) {                                                                                          \
-            err = cudaFuncSetAttribute(roi_align_bwd_nhwc_scatter<SRV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-            if (err != cudaSuccess) return (int)err;                                                                     \
-        }                                                                                                                \
-        roi_align_bwd_nhwc_scatter<SRV><<<grid, kBwThreads, smem, stream>>>(top_diff, rois, scratch, scale, N, C, H, W, PH, PW, c_pad, row_map); \
-    } while (0)
-    switch (sr) {
-        case 1: B200_LAUNCH_BW(1); break;
-        case 2: B200_LAUNCH_BW(2); break;
-        case 3: B200_LAUNCH_BW(3); break;
-        default: B200_LAUNCH_BW(4); break;
-    }
-#undef B200_LAUNCH_BW
+    const auto scatter = sr == 1 ? roi_align_bwd_nhwc_scatter<1> : sr == 2 ? roi_align_bwd_nhwc_scatter<2>
+                       : sr == 3 ? roi_align_bwd_nhwc_scatter<3> : roi_align_bwd_nhwc_scatter<4>;
+    if (const int rc = smem_opt_in(scatter, smem)) return rc;
+    scatter<<<grid, kBwThreads, smem, stream>>>(top_diff, rois, scratch, scale, N, C, H, W, PH, PW, c_pad, row_map);
     const int HW = H * W;
     dim3 tgrid((HW + 31) / 32, (C + 31) / 32, N);
     nhwc_to_nchw_kernel<<<tgrid, 256, 0, stream>>>(scratch, bottom_diff, C, HW);

@@ -394,10 +394,9 @@ static int launch_rows(const RowsPlan& p, unsigned char* ws, float* dx, int N, i
     constexpr int NX = PW * SR;
     const size_t smem = (size_t)WARPS * rows_warp_smem<CPL, NX>();
     auto kern = roi_align_bwd_rows<PW, SR, CPL, WARPS>;
-    cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (err != cudaSuccess) return (int)err;
+    if (const int rc = smem_opt_in(kern, smem)) return rc;
     int per_sm = 0;
-    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WARPS * 32, smem);
+    cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WARPS * 32, smem);
     if (err != cudaSuccess) return (int)err;
     if (per_sm < 1) return kPathDeclined;
     const int items = N * H * p.tiles_x * (C / (32 * CPL));
@@ -424,10 +423,8 @@ int roi_align_backward_rows(const float* top_diff, float scale, int N, int R, in
     if (tr_ch > C) tr_ch = (C + 31) / 32 * 32;
     const size_t smem_tr = (size_t)tr_ch * (bins | 1) * sizeof(float);
     if (smem_tr > 200 * 1024) return kPathDeclined;
-    cudaError_t err = cudaSuccess;
-    if (smem_tr > 48 * 1024) err = cudaFuncSetAttribute(roi_align_bwd_rows_tables, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tr);
-    if (err != cudaSuccess) return (int)err;
-    err = cudaMemsetAsync(ws + p.zero_off, 0, p.zero_bytes, stream);    // item counter, overflow count, units per row
+    if (const int rc = smem_opt_in(roi_align_bwd_rows_tables, smem_tr)) return rc;
+    cudaError_t err = cudaMemsetAsync(ws + p.zero_off, 0, p.zero_bytes, stream);    // item counter, overflow count, units per row
     if (err != cudaSuccess) return (int)err;
     const int cblocks = (C + tr_ch - 1) / tr_ch;
     const int table_ctas = (R * (p.ny + p.nx) + kTableThreads - 1) / kTableThreads;

@@ -38,7 +38,6 @@
 // Semantics: lib/modeling/roi_xfrom/roi_align/src/roi_align_kernel.cu (reference) :16-63, :65-121.
 #include "common.cuh"
 #include "strip_prep.cuh"
-#include <mutex>
 #include <type_traits>
 #include <string.h>
 #include <stdlib.h>
@@ -914,38 +913,6 @@ bool stream_geometry(int levels, const float* const* bottoms, const int* heights
     return true;
 }
 
-struct DeviceInfo {
-    bool ok = false;
-    int sm_count = 0;
-};
-
-// per device, set up once under a lock (the reference calls these ops from one host thread per GPU)
-bool stream_device_info(int* sm_count) {
-    static std::mutex mu;
-    static DeviceInfo info[64];
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return false;
-    std::lock_guard<std::mutex> lock(mu);
-    if (!info[dev].ok) {
-        const int max_dyn = (int)kSmemBudget;
-        bool ok = cudaDeviceGetAttribute(&info[dev].sm_count, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess;
-#define B200_STREAM_ATTR(SRV, MV) \
-        ok = ok && cudaFuncSetAttribute(roi_align_stream_fwd<SRV, MV>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_dyn) == cudaSuccess
-        B200_STREAM_ATTR(1, 1); B200_STREAM_ATTR(1, 2); B200_STREAM_ATTR(1, 3);
-        B200_STREAM_ATTR(2, 1); B200_STREAM_ATTR(2, 2); B200_STREAM_ATTR(2, 3);
-#undef B200_STREAM_ATTR
-        ok = ok && cudaFuncSetAttribute(stream_prep<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmemMax) == cudaSuccess;
-        ok = ok && cudaFuncSetAttribute(stream_prep<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPrepSmemMax) == cudaSuccess;
-        if (!ok) {
-            (void)cudaGetLastError();
-            return false;
-        }
-        info[dev].ok = true;
-    }
-    *sm_count = info[dev].sm_count;
-    return true;
-}
-
 size_t stream_fpn_workspace_bytes(int levels, const int* heights, const int* widths, int N, int R, int PH, int PW, int sr) {
     StreamGeom g;
     StreamLayout lay;
@@ -962,7 +929,7 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
     if (workspace == nullptr || C <= 0) return kPathDeclined;
     if ((long long)N * C >= (1LL << 31) || (long long)R * C * PH * PW >= (1LL << 31)) return kPathDeclined;
     int sm_count = 0;
-    if (!stream_device_info(&sm_count)) return kPathDeclined;
+    if (device_sm_count(&sm_count) != B200_ROI_OK) return kPathDeclined;
     StreamGeom g;
     StreamLayout lay;
     unsigned smem = 0;
@@ -981,22 +948,20 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
     ws.tmp = (uint4*)(wsb + lay.tmp_off);
     ws.tmpcnt = (int*)(wsb + lay.tmpcnt_off);
 
+    const int m = (g.SX - 1) / 32;
+    const auto prep = sr == 1 ? stream_prep<1> : stream_prep<2>;
+    const auto fwd = sr == 1 ? (m == 1 ? roi_align_stream_fwd<1, 1> : m == 2 ? roi_align_stream_fwd<1, 2> : roi_align_stream_fwd<1, 3>)
+                             : (m == 1 ? roi_align_stream_fwd<2, 1> : m == 2 ? roi_align_stream_fwd<2, 2> : roi_align_stream_fwd<2, 3>);
+    if (smem_opt_in(prep, kPrepSmemMax) != B200_ROI_OK || smem_opt_in(fwd, kSmemBudget) != B200_ROI_OK) return kPathDeclined;
     // prepass grid: one CTA per RoI when they are all resident at once (the kernel has a grid barrier), else a resident grid
     int per_sm = 0;
-    cudaError_t err = sr == 1 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, stream_prep<1>, kPrepThreads, lay.prep_smem)
-                              : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, stream_prep<2>, kPrepThreads, lay.prep_smem);
+    cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, prep, kPrepThreads, lay.prep_smem);
     if (err != cudaSuccess || per_sm < 1) { (void)cudaGetLastError(); return kPathDeclined; }
     const long long cap = (long long)per_sm * sm_count;
     const int prep_grid = (int)(R < cap ? R : cap);
     const int n16 = (int)(lay.zero_bytes / 16);
     // the main kernel has a grid barrier too: one CTA per SM must be resident at its shared-memory size
-    const int m = (g.SX - 1) / 32;
-#define B200_STREAM_OCC(SRV, MV) err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, roi_align_stream_fwd<SRV, MV>, kStreamThreads, smem)
-#define B200_STREAM_OCC_M(SRV) if (m == 1) B200_STREAM_OCC(SRV, 1); else if (m == 2) B200_STREAM_OCC(SRV, 2); else B200_STREAM_OCC(SRV, 3)
-    if (sr == 1) { B200_STREAM_OCC_M(1); }
-    else         { B200_STREAM_OCC_M(2); }
-#undef B200_STREAM_OCC_M
-#undef B200_STREAM_OCC
+    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fwd, kStreamThreads, smem);
     if (err != cudaSuccess || (long long)per_sm * sm_count < g.pieces) { (void)cudaGetLastError(); return kPathDeclined; }
 
     StreamArgs a;
@@ -1021,18 +986,12 @@ int roi_align_forward_stream_fpn(int levels, const float* const* bottoms, const 
     cfg.stream = stream;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    err = sr == 1 ? cudaLaunchKernelEx(&cfg, stream_prep<1>, rois, g, ws, top, row_map)
-                  : cudaLaunchKernelEx(&cfg, stream_prep<2>, rois, g, ws, top, row_map);
+    err = cudaLaunchKernelEx(&cfg, prep, rois, g, ws, top, row_map);
     if (err != cudaSuccess) return (int)err;
     cfg.gridDim = dim3((unsigned)g.pieces);
     cfg.blockDim = dim3(kStreamThreads);
     cfg.dynamicSmemBytes = smem;
-#define B200_STREAM_LAUNCH(SRV, MV) err = cudaLaunchKernelEx(&cfg, roi_align_stream_fwd<SRV, MV>, a)
-#define B200_STREAM_LAUNCH_M(SRV) if (m == 1) B200_STREAM_LAUNCH(SRV, 1); else if (m == 2) B200_STREAM_LAUNCH(SRV, 2); else B200_STREAM_LAUNCH(SRV, 3)
-    if (sr == 1) { B200_STREAM_LAUNCH_M(1); }
-    else         { B200_STREAM_LAUNCH_M(2); }
-#undef B200_STREAM_LAUNCH_M
-#undef B200_STREAM_LAUNCH
+    err = cudaLaunchKernelEx(&cfg, fwd, a);
     if (err != cudaSuccess) return (int)err;
     return finish_launch(3);
 }

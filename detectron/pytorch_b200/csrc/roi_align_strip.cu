@@ -44,7 +44,6 @@
 #include "common.cuh"
 #include "strip_prep.cuh"
 #include <cuda.h>                                              // CUtensorMap types only: the encoder is fetched with cudaGetDriverEntryPoint
-#include <mutex>
 #include <string.h>
 
 namespace b200 {
@@ -68,6 +67,7 @@ constexpr int kPrepThreads = 128;
 constexpr int kMaxKeys = 6144;                                // CSR scan lives in shared memory
 constexpr int kMaxK = 48;
 constexpr unsigned kSmemBudget = 227u * 1024u;
+constexpr unsigned kPrepSmemMax = 2 * (kMaxKeys + 1) * 4 + kAxisMaxS * kAxisMaxS * 12;     // strip_prep at the largest scan and fragment list
 constexpr unsigned kFragCost = 10u, kPassCost = 9u;           // cost model of the partition (units ~ 10 instructions)
 constexpr unsigned kRowCost = 44u;                            // cost of streaming one row in the same units
 
@@ -951,40 +951,6 @@ bool make_quad_map(CUtensorMap* map, const float* bottom, int N, int C, int H, i
                   CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-struct StripDevice {
-    bool ok = false;
-    int sm_count = 0;
-    int prep_ctas_per_sm[2] = {0, 0};                         // resident strip_prep<SR> CTAs per SM at the largest dynamic shared memory
-};
-
-bool strip_device_info(StripDevice* out) {
-    static std::mutex mu;
-    static StripDevice info[64];
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return false;
-    std::lock_guard<std::mutex> lock(mu);
-    if (!info[dev].ok) {
-        const int max_dyn = (int)kSmemBudget;
-        bool ok = cudaDeviceGetAttribute(&info[dev].sm_count, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess;
-#define B200_STRIP_ATTR(SRV, XOV) \
-        ok = ok && cudaFuncSetAttribute(roi_align_strip_fwd<SRV, XOV, kCellTma>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_dyn) == cudaSuccess; \
-        ok = ok && cudaFuncSetAttribute(roi_align_strip_fwd<SRV, XOV, kCellAsync>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_dyn) == cudaSuccess
-        B200_STRIP_ATTR(1, 4); B200_STRIP_ATTR(1, 8); B200_STRIP_ATTR(1, 12);
-        B200_STRIP_ATTR(2, 4); B200_STRIP_ATTR(2, 8); B200_STRIP_ATTR(2, 12);
-#undef B200_STRIP_ATTR
-        const int prep_dyn = 2 * (kMaxKeys + 1) * 4 + kAxisMaxS * kAxisMaxS * 12;
-        ok = ok && cudaFuncSetAttribute(strip_prep<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, prep_dyn) == cudaSuccess;
-        ok = ok && cudaFuncSetAttribute(strip_prep<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, prep_dyn) == cudaSuccess;
-        if (!ok) {
-            (void)cudaGetLastError();
-            return false;
-        }
-        info[dev].ok = true;
-    }
-    *out = info[dev];
-    return true;
-}
-
 }  // namespace
 
 void roi_align_strip_set_debug_buffer(unsigned long long* host_pinned) {
@@ -1009,15 +975,15 @@ int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const i
                                 const int* row_map, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
     if (workspace == nullptr || C <= 0) return kPathDeclined;
     if ((long long)N * C >= (1LL << 31) || (long long)R * C * PH * PW >= (1LL << 31)) return kPathDeclined;
-    StripDevice dev;
-    if (!strip_device_info(&dev)) return kPathDeclined;
+    int sm_count = 0;
+    if (device_sm_count(&sm_count) != B200_ROI_OK) return kPathDeclined;
     StripGeom g;
     StripLayout lay;
     unsigned smem = 0;
     // rows by TMA when every level has an x-quad view (W % 4 == 0, 16-byte aligned base) -- else cp.async producers
     bool tma = encode_tiled_fn() != nullptr;
     for (int l = 0; tma && l < levels; ++l) tma = (widths[l] & 3) == 0 && ((uintptr_t)bottoms[l] & 15u) == 0;
-    if (!strip_geometry(levels, bottoms, heights, widths, scales, level_roi_begin, N, R, C, PH, PW, sr, dev.sm_count,
+    if (!strip_geometry(levels, bottoms, heights, widths, scales, level_roi_begin, N, R, C, PH, PW, sr, sm_count,
                         tma ? kCellTma : kCellAsync, &g, &lay, &smem)) return kPathDeclined;
     if (workspace_bytes < lay.ws_bytes) return kPathDeclined;
     unsigned char* wsb = (unsigned char*)workspace;
@@ -1033,19 +999,25 @@ int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const i
     ws.tmp = (uint4*)(wsb + lay.tmp_off);
     ws.tmpcnt = (int*)(wsb + lay.tmpcnt_off);
 
+    const int xo = g.SX / 8;
+    const auto prep = sr == 1 ? strip_prep<1> : strip_prep<2>;
+    const auto fwd =
+        tma ? (sr == 1 ? (xo == 4 ? roi_align_strip_fwd<1, 4, kCellTma> : xo == 8 ? roi_align_strip_fwd<1, 8, kCellTma> : roi_align_strip_fwd<1, 12, kCellTma>)
+                       : (xo == 4 ? roi_align_strip_fwd<2, 4, kCellTma> : xo == 8 ? roi_align_strip_fwd<2, 8, kCellTma> : roi_align_strip_fwd<2, 12, kCellTma>))
+            : (sr == 1 ? (xo == 4 ? roi_align_strip_fwd<1, 4, kCellAsync> : xo == 8 ? roi_align_strip_fwd<1, 8, kCellAsync> : roi_align_strip_fwd<1, 12, kCellAsync>)
+                       : (xo == 4 ? roi_align_strip_fwd<2, 4, kCellAsync> : xo == 8 ? roi_align_strip_fwd<2, 8, kCellAsync> : roi_align_strip_fwd<2, 12, kCellAsync>));
+    if (smem_opt_in(prep, kPrepSmemMax) != B200_ROI_OK || smem_opt_in(fwd, kSmemBudget) != B200_ROI_OK) return kPathDeclined;
     // prepass grid: one CTA per RoI when they are all resident at once (the kernel has a grid barrier), else a resident grid
     const size_t prep_dyn = (size_t)2 * (g.keys + 1) * 4 + (size_t)g.cap_r * 12;
     int per_sm = 0;
-    cudaError_t err = sr == 1 ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, strip_prep<1>, kPrepThreads, prep_dyn)
-                              : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, strip_prep<2>, kPrepThreads, prep_dyn);
+    cudaError_t err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, prep, kPrepThreads, prep_dyn);
     if (err != cudaSuccess || per_sm < 1) { (void)cudaGetLastError(); return kPathDeclined; }
-    long long cap = (long long)per_sm * dev.sm_count;
+    long long cap = (long long)per_sm * sm_count;
     const int prep_grid = (int)(R < cap ? R : cap);
 
     err = cudaMemsetAsync(zero, 0, lay.zero_bytes, stream);
     if (err != cudaSuccess) return (int)err;
-    if (sr == 1) strip_prep<1><<<prep_grid, kPrepThreads, prep_dyn, stream>>>(rois, g, ws, top, row_map);
-    else         strip_prep<2><<<prep_grid, kPrepThreads, prep_dyn, stream>>>(rois, g, ws, top, row_map);
+    prep<<<prep_grid, kPrepThreads, prep_dyn, stream>>>(rois, g, ws, top, row_map);
 
     StripArgs a;
     a.ytab = ws.ytab; a.xtab = ws.xtab; a.entries = ws.entries; a.rowptr = ws.rowptr; a.maxend = ws.maxend;
@@ -1071,12 +1043,7 @@ int roi_align_forward_strip_fpn(int levels, const float* const* bottoms, const i
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    const int xo = g.SX / 8;
-#define B200_STRIP_LAUNCH(SRV, XOV) \
-    err = tma ? cudaLaunchKernelEx(&cfg, roi_align_strip_fwd<SRV, XOV, kCellTma>, maps, a) : cudaLaunchKernelEx(&cfg, roi_align_strip_fwd<SRV, XOV, kCellAsync>, maps, a)
-    if (sr == 1) { if (xo == 4) B200_STRIP_LAUNCH(1, 4); else if (xo == 8) B200_STRIP_LAUNCH(1, 8); else B200_STRIP_LAUNCH(1, 12); }
-    else         { if (xo == 4) B200_STRIP_LAUNCH(2, 4); else if (xo == 8) B200_STRIP_LAUNCH(2, 8); else B200_STRIP_LAUNCH(2, 12); }
-#undef B200_STRIP_LAUNCH
+    err = cudaLaunchKernelEx(&cfg, fwd, maps, a);
     if (err != cudaSuccess) return (int)err;
     return finish_launch(2);
 }

@@ -27,7 +27,6 @@
 // Semantics: lib/modeling/roi_xfrom/roi_align/src/roi_align_kernel.cu (reference) :16-63, :65-121.
 #include "roi_align_tiled.cuh"
 #include <stdlib.h>
-#include <mutex>
 
 namespace b200 {
 
@@ -350,23 +349,11 @@ int roi_align_forward_tiled(const float* bottom, float scale, int N, int R, int 
     int* tile_count = zero + 4;
     unsigned* tile_list = (unsigned*)(ws + p.tile_list_off);
 
-    static std::mutex attr_mu;              // several host threads may make their first call at once
-    static bool attr_set[64] = {false};     // per device: the attribute lives in the device's context
-    static int sm_count[64] = {0};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kPathDeclined;
-    std::unique_lock<std::mutex> attr_lock(attr_mu);
-    if (!attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(roi_align_tiled_fwd<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (228 * 1024 - kTiledCtasPerSM * 1024) / kTiledCtasPerSM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(roi_align_tiled_fwd<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (228 * 1024 - kTiledCtasPerSM * 1024) / kTiledCtasPerSM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(roi_align_tiled_fwd<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (228 * 1024 - kTiledCtasPerSM * 1024) / kTiledCtasPerSM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(roi_align_tiled_fwd<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (228 * 1024 - kTiledCtasPerSM * 1024) / kTiledCtasPerSM);
-        if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sm_count[dev], cudaDevAttrMultiProcessorCount, dev);
-        if (e != cudaSuccess) return (int)e;
-        attr_set[dev] = true;
-    }
-    const int sms = sm_count[dev];
-    attr_lock.unlock();
+    const auto fwd = sr == 1 ? roi_align_tiled_fwd<1> : sr == 2 ? roi_align_tiled_fwd<2> : sr == 3 ? roi_align_tiled_fwd<3> : roi_align_tiled_fwd<4>;
+    int sms = 0;
+    int rc = smem_opt_in(fwd, (228 * 1024 - kTiledCtasPerSM * 1024) / kTiledCtasPerSM);
+    if (rc == B200_ROI_OK) rc = device_sm_count(&sms);
+    if (rc != B200_ROI_OK) return rc;
     cudaError_t err = cudaMemsetAsync(zero, 0, p.zero_bytes, stream);
     if (err != cudaSuccess) return (int)err;
     // The bins the main kernel accumulates into must start at zero.  With a dense output one memset of the whole tensor
@@ -383,17 +370,9 @@ int roi_align_forward_tiled(const float* bottom, float scale, int N, int R, int 
     const int n_cgroups = (C + kCG - 1) / kCG;
     const int n_work = p.tiles_total * n_cgroups;
     const int grid = n_work < kTiledCtasPerSM * sms ? n_work : kTiledCtasPerSM * sms;      // persistent CTAs
-#define B200_LAUNCH_TILED(SRV)                                                                                              \
-    roi_align_tiled_fwd<SRV><<<grid, kTiledThreads, p.smem_bytes, stream>>>(bottom, ytab, xtab, work_counter, tile_count,   \
-        tile_list, R * p.groups_max, top, N, R, C, H, W, PH, PW, p.ny, p.nx, p.core_h, p.core_w, p.tile_h, p.tiles_y, p.tiles_x, \
-        n_cgroups, n_work, row_map)
-    switch (sr) {
-        case 1: B200_LAUNCH_TILED(1); break;
-        case 2: B200_LAUNCH_TILED(2); break;
-        case 3: B200_LAUNCH_TILED(3); break;
-        default: B200_LAUNCH_TILED(4); break;
-    }
-#undef B200_LAUNCH_TILED
+    fwd<<<grid, kTiledThreads, p.smem_bytes, stream>>>(bottom, ytab, xtab, work_counter, tile_count, tile_list, R * p.groups_max, top,
+                                                       N, R, C, H, W, PH, PW, p.ny, p.nx, p.core_h, p.core_w, p.tile_h, p.tiles_y,
+                                                       p.tiles_x, n_cgroups, n_work, row_map);
     return finish_launch(2);
 }
 

@@ -153,8 +153,7 @@ static int roi_crop_backward_nhwc(const float* grad_output, const float* grids, 
     const bool own = scratch == nullptr || workspace_bytes < bytes;      // no caller scratch: stream-ordered allocation
     if (own && cudaMallocAsync((void**)&scratch, bytes, stream) != cudaSuccess) { (void)cudaGetLastError(); return kPathDeclined; }
     cudaError_t err = cudaMemsetAsync(scratch, 0, bytes, stream);
-    if (err == cudaSuccess && smem > 48 * 1024)
-        err = cudaFuncSetAttribute(roi_crop_bwd_nhwc_scatter, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err == cudaSuccess) err = (cudaError_t)smem_opt_in(roi_crop_bwd_nhwc_scatter, smem);
     if (err == cudaSuccess) {
         dim3 grid(R, (C + kCropChunk - 1) / kCropChunk);
         roi_crop_bwd_nhwc_scatter<<<grid, 256, smem, stream>>>(grad_output, grids, scratch, N, C, H, W, R, oh, ow, c_pad);

@@ -254,14 +254,9 @@ int b200_topk_batched(const float* const* scores_dev_ptrs_host, const int* A_hos
     int m2 = 1;
     while (m2 < kmax) m2 <<= 1;
     const size_t smem = (size_t)m2 * sizeof(u64);
-    static bool attr_done[64] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return B200_ROI_EWORKSPACE;
-    if (!__atomic_load_n(&attr_done[dev], __ATOMIC_ACQUIRE)) {
-        if (cudaFuncSetAttribute(topk_collect_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTopkMaxK * (int)sizeof(u64)) != cudaSuccess)
-            return (int)cudaGetLastError();
-        __atomic_store_n(&attr_done[dev], true, __ATOMIC_RELEASE);
-    }
+    if (cudaGetDevice(&dev) != cudaSuccess) return B200_ROI_EWORKSPACE;
+    if (const int rc = smem_opt_in(topk_collect_sort_kernel, kTopkMaxK * sizeof(u64))) return rc;
     topk_collect_sort_kernel<<<num_problems, kSortThreads, smem, stream>>>(tb, hist, order_out, scores_out);
     return finish_launch(4);
 }
